@@ -1,6 +1,6 @@
 """Camera model — drop-in for the reference's camera_handler.py (same names and signatures).
 
-Reference: /root/reference/camera_handler.py (fov/focal helpers :8-12, getProjectionMatrix :14-34, Camera :36-50,
+Reference: camera_handler.py (fov/focal helpers :8-12, getProjectionMatrix :14-34, Camera :36-50,
 get_camera :53-108).  The 4x4 matrix algebra is tiny host-side set-up (one camera per call) and stays in torch; the
 matrices are handed to the colour kernels by value (g2pc_camera_t).
 """

@@ -387,7 +387,7 @@ extern "C" int g2pc_preprocess(const void* geom, const float* colours, const flo
     if (smem > 48 * 1024)
         G2PC_CUDA(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int threads = smem <= 56 * 1024 ? 256 : smem <= 113 * 1024 ? 512 : 1024;
-    int dev = 0, sms = 148, per_sm = 1;
+    int dev = 0, sms = 132, per_sm = 1;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, preprocess_kernel, threads, smem) != cudaSuccess || per_sm < 1)

@@ -19,8 +19,8 @@
 //            the staged ids) straight into shared memory, no register round trip
 //   stage C  chunk c is blended
 // so the dependent id -> record latency of the next chunks hides under the arithmetic of the current one.  Per thread
-// and Gaussian the row-dependent terms are formed once; the per-pixel arithmetic runs on the packed FP32x2 pipe (FADD2 /
-// FFMA2 / FMUL2, two pixels per instruction, scalar broadcast operands): 8 packed ops + 2 EX2 + 2 FMNMX per pixel pair.
+// and Gaussian the row-dependent terms are formed once; the per-pixel arithmetic is 8 FP32 ops (FADD / FFMA / FMUL, each
+// rounded on its own, never contracted) + 1 EX2 + 1 FMNMX per pixel.
 // The per-Gaussian maximum is a redux.sync (u32 max of the non-negative float bits) per warp, merged across warps in
 // shared memory and published with ONE 64-bit atomicMax per (CTA, Gaussian): key = (contribution bits << 32) |
 // ~(leaf-pixel index), so ties go to the earliest leaf / lowest pixel, deterministically.
@@ -62,6 +62,17 @@ __device__ __forceinline__ float ex2f(float x) {
     float r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));  // results below FLT_MIN flush to 0 (see header comment)
     return r;
+}
+
+// per-lane FP32 on a pixel pair with a scalar operand; the _rn intrinsics keep every op rounded on its own (no FMA
+// contraction), which fixes the results bit for bit
+__device__ __forceinline__ float2 add2(float2 a, float b) { return make_float2(__fadd_rn(a.x, b), __fadd_rn(a.y, b)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b, c.x), __fmaf_rn(a.y, b, c.y));
+}
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c), __fmaf_rn(a.y, b.y, c));
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -157,8 +168,7 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
         x0 = active ? (quad - row * qpr) * 4 : 0;
     }
 
-    // two pixel pairs per thread: Blackwell's packed FP32x2 pipe (FADD2 / FMUL2 / FFMA2) takes a scalar broadcast operand,
-    // so the per-Gaussian scalars feed both pixels of a pair without extra moves
+    // four pixels per thread, held as two pairs; the per-Gaussian scalars are shared by all four
     float2 T01, T23, px01, px23;
     float2 Cr01 = make_float2(0.f, 0.f), Cr23 = Cr01, Cg01 = Cr01, Cg23 = Cr01, Cb01 = Cr01, Cb23 = Cr01;
     {
@@ -236,24 +246,22 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
                     const float Bq = dy * q0.w;
                     const float Cq = fmaf(dy * dy, q1.x, q1.y);  // + log2(opacity): alpha = min(0.99, exp2(e))
                     const float nmx = -q0.x;
-                    const float2 dx01 = __fadd2_rn(px01, make_float2(nmx, nmx));
-                    const float2 dx23 = __fadd2_rn(px23, make_float2(nmx, nmx));
-                    const float2 e01 = __ffma2_rn(dx01, __ffma2_rn(dx01, make_float2(q0.z, q0.z), make_float2(Bq, Bq)),
-                                                  make_float2(Cq, Cq));
-                    const float2 e23 = __ffma2_rn(dx23, __ffma2_rn(dx23, make_float2(q0.z, q0.z), make_float2(Bq, Bq)),
-                                                  make_float2(Cq, Cq));
+                    const float2 dx01 = add2(px01, nmx);
+                    const float2 dx23 = add2(px23, nmx);
+                    const float2 e01 = fma2(dx01, fma2(dx01, q0.z, make_float2(Bq, Bq)), Cq);
+                    const float2 e23 = fma2(dx23, fma2(dx23, q0.z, make_float2(Bq, Bq)), Cq);
                     const float2 a01 = make_float2(fminf(0.99f, ex2f(e01.x)), fminf(0.99f, ex2f(e01.y)));
                     const float2 a23 = make_float2(fminf(0.99f, ex2f(e23.x)), fminf(0.99f, ex2f(e23.y)));
-                    const float2 c01 = __fmul2_rn(T01, a01);
-                    const float2 c23 = __fmul2_rn(T23, a23);
-                    Cr01 = __ffma2_rn(c01, make_float2(q1.z, q1.z), Cr01);
-                    Cr23 = __ffma2_rn(c23, make_float2(q1.z, q1.z), Cr23);
-                    Cg01 = __ffma2_rn(c01, make_float2(q1.w, q1.w), Cg01);
-                    Cg23 = __ffma2_rn(c23, make_float2(q1.w, q1.w), Cg23);
-                    Cb01 = __ffma2_rn(c01, make_float2(bl, bl), Cb01);
-                    Cb23 = __ffma2_rn(c23, make_float2(bl, bl), Cb23);
-                    T01 = __ffma2_rn(c01, make_float2(-1.0f, -1.0f), T01);  // T - T*alpha (one rounding)
-                    T23 = __ffma2_rn(c23, make_float2(-1.0f, -1.0f), T23);
+                    const float2 c01 = mul2(T01, a01);
+                    const float2 c23 = mul2(T23, a23);
+                    Cr01 = fma2(c01, q1.z, Cr01);
+                    Cr23 = fma2(c23, q1.z, Cr23);
+                    Cg01 = fma2(c01, q1.w, Cg01);
+                    Cg23 = fma2(c23, q1.w, Cg23);
+                    Cb01 = fma2(c01, bl, Cb01);
+                    Cb23 = fma2(c23, bl, Cb23);
+                    T01 = fma2(c01, -1.0f, T01);  // T - T*alpha (one rounding)
+                    T23 = fma2(c23, -1.0f, T23);
                     // arg-max bookkeeping only if some contribution can beat what the Gaussian already holds
                     const float v = fmaxf(fmaxf(c01.x, c01.y), fmaxf(c23.x, c23.y));
                     if (__any_sync(FULLM, v > bt.y)) {
@@ -383,7 +391,7 @@ extern "C" int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, 
     p.stats = (unsigned long long*)stats;
     static int resident = 0;  // persistent grid: every SM filled to the kernel's occupancy (device constant)
     if (resident == 0) {
-        int dev = 0, sms = 148, per_sm = 8;
+        int dev = 0, sms = 132, per_sm = 8;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blend_kernel, BT, 0) != cudaSuccess || per_sm < 1)

@@ -743,7 +743,7 @@ extern "C" int g2pc_tiles_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_o
     p.W = width; p.H = height;
     for (int i = 0; i < 3; ++i) p.bg[i] = background3_host[i];
     p.work_counter = work_counters; p.stats = (unsigned long long*)stats;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaStream_t st = (cudaStream_t)stream;

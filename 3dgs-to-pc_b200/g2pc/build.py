@@ -1,4 +1,4 @@
-"""Build libg2pc.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libg2pc.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m g2pc.build            (from 3dgs-to-pc_b200/)   or   g2pc.build.build()
 
@@ -16,7 +16,7 @@ CSRC = os.path.join(PKG_ROOT, "csrc")
 LIB_PATH = os.path.join(HERE, "libg2pc.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

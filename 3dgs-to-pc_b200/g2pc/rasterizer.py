@@ -4,7 +4,7 @@ Reference call surface restated here (same names, argument order, defaults, retu
     GaussianRasterizationSettings     gaussian_pointcloud_rasterization/__init__.py:21-35
     GaussianRasterizer                :37-220   (constructor :38-76, forward :90-140, getters :160-220)
     _C.rasterize_gaussians            ext.cpp:15-17 / rasterize_points.cu:36-145  (22 arguments -> 11-tuple)
-The work is done by the sm_100a kernels of csrc/s7_tiles.cu + the shared depth sort / multisplit (csrc/s4_tree.cu) behind
+The work is done by the sm_90a kernels of csrc/s7_tiles.cu + the shared depth sort / multisplit (csrc/s4_tree.cu) behind
 the C ABI (include/g2pc.h, g2pc_tiles_*).  Differences that are deliberate and documented:
   * results are deterministic (the reference's max-contribution / surface-distance updates race, SURVEY.md §2.1);
   * one camera costs no host synchronisation (g2pc/frames.py) — the reference runs with debug=True, i.e. a

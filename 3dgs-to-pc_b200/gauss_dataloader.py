@@ -1,6 +1,6 @@
 """Gaussian file I/O — thin host-side counterpart of the reference's gauss_dataloader.py (same function names).
 
-Reference: /root/reference/gauss_dataloader.py (load_ply_data :16-82, load_splat_data :84-115, save_xyz_to_ply :118-202,
+Reference: gauss_dataloader.py (load_ply_data :16-82, load_splat_data :84-115, save_xyz_to_ply :118-202,
 load_gaussians :204-211).  Outside the timed hot path (SURVEY.md §2 row 12, §8f N3): a small numpy PLY reader replaces the
 `plyfile` dependency, and the PLY vertex records are assembled on the GPU (byte views of the f32 / u8 tensors) so the
 point cloud crosses PCIe once, already in file layout.

@@ -1,7 +1,7 @@
 """Scene model of the hot path — drop-in for the reference's gauss_handler.py (same names, arguments, attributes).
 
-Reference: /root/reference/gauss_handler.py (Gaussians :65-279, covariance helpers :12-63).  The arithmetic-heavy
-members run as hand-written sm_100a kernels behind the C ABI (include/g2pc.h):
+Reference: gauss_handler.py (Gaussians :65-279, covariance helpers :12-63).  The arithmetic-heavy
+members run as hand-written sm_90a kernels behind the C ABI (include/g2pc.h):
     build_covariance_from_scaling_rotation -> g2pc_cov_build        (csrc/s1_cov.cu)
     Gaussians.calculate_normals            -> g2pc_normals
     torch.linalg.eigvals(...).real         -> g2pc_eigvals_sym3     (used by validate_covariances / magnitudes)

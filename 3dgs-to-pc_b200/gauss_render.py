@@ -1,12 +1,12 @@
 """Colour stage — drop-in for the reference's gauss_render.py.
 
-Reference: /root/reference/gauss_render.py.  `get_renderer` (:467-493) is the plugin boundary: it returns a callable
+Reference: gauss_render.py.  `get_renderer` (:467-493) is the plugin boundary: it returns a callable
 `renderer(camera) -> (image, radii|None, invdepth|None, depth|None)` that, as a side effect, keeps for every Gaussian
 the largest contribution alpha*T it made to any pixel of any camera and the blended colour of that pixel, plus the
 getters used by the pipeline (gauss_to_pc.py:481-513).
 
 `renderer_type="python"` reproduces GaussPythonRenderer (:210-465): quadtree tiles, every Gaussian of a tile blended
-into every pixel of the tile — but as sm_100a kernels behind the C ABI (csrc/s3_preprocess.cu, s4_tree.cu,
+into every pixel of the tile — but as sm_90a kernels behind the C ABI (csrc/s3_preprocess.cu, s4_tree.cu,
 s5_blend.cu), one camera = 8 asynchronous entry-point calls and no host wait.  The tile parameters the reference derives
 from free GPU memory at call time (:440-444) are pinned (g2pc.config.MAX_TILE_SIZE / MAX_GAUSSIANS_PER_TILE).
 """
@@ -36,7 +36,7 @@ def strip_symmetric(sym):
 
 
 class GaussPythonRenderer(FrameQueue):
-    """B200 implementation of the reference's pure-torch tile renderer (same constructor arguments, attributes and
+    """H100 implementation of the reference's pure-torch tile renderer (same constructor arguments, attributes and
     getters as gauss_render.py:210-264).
 
     One camera ("frame") = 8 asynchronous entry-point calls and NO host wait: every size the later kernels need lives
@@ -334,7 +334,7 @@ def get_renderer(renderer_type: str, xyz, opacities, colours, covariances, shs=N
                                    visible_gaussian_threshold=visible_gaussian_threshold, shs=shs)
     if renderer_type == "cuda":
         # the reference's CUDA back-end semantics (16x16 tiles, alpha / transmittance cut-offs, depth maps, surface
-        # distances) on the sm_100a kernels of csrc/s7_tiles.cu — gauss_render.py:469-488
+        # distances) on the sm_90a kernels of csrc/s7_tiles.cu — gauss_render.py:469-488
         from g2pc.rasterizer import GaussianRasterizer as GaussianPCRasterizer
         means2D = None  # (the reference allocates a zero tensor nobody reads, :476)
         common = dict(cov3D_precomp=covariances.to(torch.float), visible_gaussian_threshold=visible_gaussian_threshold,

@@ -1,9 +1,9 @@
 """3DGS -> point cloud: CLI, pipeline driver and the sampling stage — drop-in for the reference's gauss_to_pc.py.
 
-Reference: /root/reference/gauss_to_pc.py.  Same flags (:607-646), same settings tuple (:26-60), same public
+Reference: gauss_to_pc.py.  Same flags (:607-646), same settings tuple (:26-60), same public
 functions and argument order (distribute_points :73, mahalanobis :92, calculate_bin_sizes :105,
 sample_from_multivariate_normal :140, create_new_gaussian_points :157, generate_pointcloud :277,
-convert_3dgs_to_pc :373).  The sampling stage runs as two fused sm_100a kernels (csrc/s2_sample.cu) driven by
+convert_3dgs_to_pc :373).  The sampling stage runs as two fused sm_90a kernels (csrc/s2_sample.cu) driven by
 g2pc/sampler.py; the colour stage runs through gauss_render.get_renderer.  No CPU fallback.
 """
 from typing import NamedTuple

@@ -1,6 +1,6 @@
 """Camera pose / intrinsics loaders — thin host-side counterpart of the reference's transform_dataloader.py.
 
-Reference: /root/reference/transform_dataloader.py (COLMAP bin :115-167, COLMAP txt :169-205, transforms.json :207-277,
+Reference: transform_dataloader.py (COLMAP bin :115-167, COLMAP txt :169-205, transforms.json :207-277,
 dispatch :280-299).  Host parsing only, outside the hot path (SURVEY.md §2 row 13).  Returns
 ({image name: 4x4 c2w nested list (OpenGL)}, {image name: [w, h, fx, fy]}).
 """

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — Mpoints/s (sample + colour) of the 3DGS-to-PC hot path on B200.
+"""bench.py — Mpoints/s (sample + colour) of the 3DGS-to-PC hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torch.distributed.run, one rank per GPU)
     python bench.py --impl reference ...                      (the reference's own code on the host cores)
+    python bench.py ... --dump-outputs DIR                    (also write the last timed step's point cloud as .npy)
 
 One "step" = one pass of the hot path over the whole synthetic scene: covariance build (S1) -> colour stage over all
 cameras (S3-S6, SH evaluated per camera) -> culls -> validate covariances -> magnitudes / points-per-Gaussian / bins ->
@@ -18,7 +19,7 @@ c4 = c3's scene, 50M points, surface_distance_std 2.0, exact_num_points (rendere
 Extra objects in the JSON line (all measured in this run, on this box):
   roofline        the dominant kernel of the step (by summed CUDA-event time) against the roof that bounds it
   rooflines       every hand-written kernel: algorithmic bytes / event time vs the measured HBM peak
-  ref_cuda        the UNMODIFIED reference pipeline with its CUDA rasterizer (baseline/_ref, built for sm_100) on the same
+  ref_cuda        the UNMODIFIED reference pipeline with its CUDA rasterizer (oracle/_ref, built for sm_90) on the same
                   workload and GPU — the ">= 10x" comparator of BASELINE.md §3.5
   c1              config C1 like for like: this build (GPU) next to the reference's own code on the host cores, in full
   cpu_baseline    the reference's own python path on a bounded sample of the workload (host cores)
@@ -50,7 +51,7 @@ WORKLOADS = {
     "c5": dict(n=6_000_000, cams=500, points=100_000_000, res=1920, sh=3, colours=True, seed=1234 + 4),
     "tiny": dict(n=100_000, cams=4, points=400_000, res=720, sh=3, colours=True, seed=1234 + 9),
 }
-METRIC = "Mpoints/sec (sample+colour) at 3M Gaussians/200 cams, 1/2/4/8 B200 vs CPU ref"
+METRIC = "Mpoints/sec (sample+colour) at 3M Gaussians/200 cams, 1/2/4/8 H100 vs CPU ref"
 UNIT = "Mpoints/s"
 
 
@@ -70,6 +71,9 @@ def parse():
     ap.add_argument("--no-c1", action="store_true")
     ap.add_argument("--cpu-sample-gaussians", type=int, default=30000)
     ap.add_argument("--cpu-sample-cams", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the point cloud of the last timed step to DIR/<name>.npy (float32; a fixed seeded "
+                         "sample of at most DUMP_MAX_POINTS points, with its indices)")
     return ap.parse_args()
 
 
@@ -161,6 +165,28 @@ def _calibration():
         return json.load(open(os.path.join(ROOT, "profiles", "r02_calibration.json")))
     except Exception:
         return {}
+
+
+DUMP_MAX_POINTS = 1 << 20  # 3 float32 arrays of (n, 3) + the indices: 40 MB at most
+
+
+def dump_outputs(pc, out_dir):
+    """What a caller of convert_gaussians_to_pc receives (points, colours, normals), as float32 .npy files.  Clouds larger
+    than DUMP_MAX_POINTS are reduced to the same seeded sample of rows for every array; `sample_index` holds the row
+    numbers (float64, exact) and `num_points` the full count, so two builds can be compared row for row."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = int(pc.points.shape[0])
+    if n > DUMP_MAX_POINTS:
+        idx = np.sort(np.random.default_rng(0).choice(n, DUMP_MAX_POINTS, replace=False))
+    else:
+        idx = np.arange(n)
+    sel = torch.as_tensor(idx, device=pc.points.device)
+    for name in ("points", "colours", "normals"):
+        t = getattr(pc, name)
+        if t is not None:
+            np.save(os.path.join(out_dir, name + ".npy"), t.index_select(0, sel).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "sample_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "num_points.npy"), np.array([n], dtype=np.float64))
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -281,6 +307,8 @@ def run_ours(args):
         clk.mark_begin()
         ms, npts, pc = timed(step_resident, args.steps)
         clk.mark_end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(pc, args.dump_outputs)
     launches = capi.LAUNCHES
     ms_step = ms / args.steps
     value = npts / (ms_step * 1e-3) / 1e6
@@ -335,7 +363,7 @@ def run_ours(args):
                                f"width {wl['res']}, SH deg {wl['sh']}, visibility_threshold 0.05, renderer_type={rtype} "
                                "semantics", "points_out": npts,
                    "blend_t_stop": config.BLEND_T_STOP, "frame_slots": config.FRAME_SLOTS,
-                   "l2": ("inputs larger than L2 (per-step working set >> 126 MB)" if h2d_bytes * world > 4 * 126e6 else
+                   "l2": ("inputs larger than L2 (per-step working set >> 50 MB)" if h2d_bytes * world > 4 * 50e6 else
                           "working set below L2 and not flushed (non-headline workload)"),
                    "parallelism": "1 GPU" if world == 1 else f"cameras sharded x{world} (colour), Gaussians sharded x{world} (sampling)"},
         "e2e": {"value": round(e2e_pts / (e2e_step * 1e-3) / 1e6, 3), "unit": UNIT, "ms_per_step": round(e2e_step, 3),
@@ -363,8 +391,8 @@ def rooflines(wl, timing, warp_gaussians, g2p, pc, world, clocks):
     ncu capture (profiles/r02_calibration.json)."""
     peaks = _peaks()
     cal = _calibration()
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-    src = "measured" if peaks else "fallback"
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
+    src = "measured" if peaks else "H100 SXM data sheet"
     cams_rank = max(1, (wl["cams"] + world - 1) // world) if wl["cams"] else 0
     n = wl["n"]
     ncoef = (wl["sh"] + 1) ** 2
@@ -393,7 +421,7 @@ def rooflines(wl, timing, warp_gaussians, g2p, pc, world, clocks):
     if blend:
         tot_ms = float(np.sum(blend))
         ipi = cal.get("blend_inst_per_warp_gaussian")
-        sm_mhz = clocks.get("sm_mhz") or peaks.get("sm_max_mhz") or 1965.0
+        sm_mhz = clocks.get("sm_mhz") or peaks.get("sm_max_mhz") or 1980.0
         sms = torch.cuda.get_device_properties(0).multi_processor_count
         peak_issue = sms * 4 * sm_mhz * 1e6 / 1e9  # G warp-instructions / s
         entry = {"kernel": "blend_kernel", "bound": "issue", "unit": "Gwarp-inst/s", "peak": round(peak_issue, 1),
@@ -435,13 +463,13 @@ def host_threads():
 
 
 def ref_cuda_leg(wl, our_e2e):
-    """The unmodified reference pipeline, renderer_type=cuda (its own CUDA rasterizer recompiled for sm_100), same
+    """The unmodified reference pipeline, renderer_type=cuda (its own CUDA rasterizer recompiled for sm_90), same
     workload, same GPU, one warm-up pass + one timed pass (BASELINE.md §3.5)."""
     try:
-        from baseline import ref_run
+        from oracle import ref_run
         from g2pc import synth
         if not (ref_run.available() and ref_run.cuda_extension_available()):
-            return {"unavailable": "baseline/_ref not staged (run baseline/build_ref.py in the build container)"}
+            return {"unavailable": "reference not staged (G2PC_REFERENCE_ROOT + oracle/build_ref.py)"}
         sc = _scene_for(wl)
         cams, intr = synth.make_cameras(wl["cams"])
         kw = dict(renderer_type="cuda", num_points=wl["points"], colour_resolution=wl["res"], max_sh_degree=wl["sh"],
@@ -507,9 +535,9 @@ def c1_leg(g2p, capi, sampler, dev):
 
 
 def reference_c1(steps=5):
-    """The reference's OWN code (unmodified, staged under baseline/_ref/py or /root/reference) on C1 in full, CPU."""
+    """The reference's OWN code (unmodified, found through G2PC_REFERENCE_ROOT) on C1 in full, CPU."""
     try:
-        from baseline import ref_run
+        from oracle import ref_run
         if not ref_run.available():
             return {"unavailable": "reference sources not staged"}
         wl = WORKLOADS["c1"]
@@ -543,7 +571,7 @@ def cpu_sample_run(wl, n_s, cams_s, threads):
     points = max(200, int(round(wl["points"] * frac)))
     desc = dict(gaussians=n_s, cameras=len(cams), points_requested=points)
     try:
-        from baseline import ref_run
+        from oracle import ref_run
         if ref_run.available():
             pc, dt = ref_run.run(sc, cams, intr, device="cpu", renderer_type="python", num_points=points,
                                  render_colours=wl["colours"] and bool(cams), colour_resolution=wl["res"],

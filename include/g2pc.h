@@ -1,5 +1,5 @@
 /*
- * g2pc.h — C ABI of libg2pc.so: B200-native (sm_100a) kernels for the 3DGS-to-PC hot path
+ * g2pc.h — C ABI of libg2pc.so: H100-native (sm_90a) kernels for the 3DGS-to-PC hot path
  * (per-Gaussian point sampling + Mahalanobis cull, per-camera colour / visibility rasterisation).
  *
  * This is the drop-in boundary.  The reference has two native/op boundaries on this path:

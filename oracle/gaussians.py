@@ -1,6 +1,6 @@
 """Oracle restatement of the per-Gaussian scene model on the hot path (TEST INFRASTRUCTURE, see oracle/__init__.py).
 
-Follows /root/reference/gauss_handler.py; torch-CPU ops are used where the reference's arithmetic is a torch
+Follows gauss_handler.py; torch-CPU ops are used where the reference's arithmetic is a torch
 library routine (bmm, eigvals, eigh) so that the CPU result has the same rounding behaviour.
 """
 import math

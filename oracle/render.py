@@ -1,6 +1,6 @@
 """Oracle restatement of the colour stage, renderer_type=python (TEST INFRASTRUCTURE, see oracle/__init__.py).
 
-Follows /root/reference/gauss_render.py:101-193 (EWA covariance, projection, radius, rect), :266-402 (quadtree tiling,
+Follows gauss_render.py:101-193 (EWA covariance, projection, radius, rect), :266-402 (quadtree tiling,
 front-to-back blend, per-Gaussian max contribution + colour) and camera_handler.py:14-50.  Written as an explicit
 BFS over tiles and a *sequential* per-pixel blend (running transmittance), i.e. the way a kernel does it, rather than
 with the reference's dense cumprod tensors.  torch-CPU float32 ops are used for the per-Gaussian geometry so that the

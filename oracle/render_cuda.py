@@ -10,8 +10,8 @@ Follows the reference's CUDA back-end on the CPU in numpy float32:
 with the racy parts replaced by what they aim at (SURVEY.md §2.1, §8a): per-Gaussian contribution = max over pixels,
 arg-max = lowest pixel id among equals, surface distance = min over the tile's threads after every round of 256 entries
 (threads outside the image hold expected depth 0, masked pixels have left the loop).
-PARITY PIN: the reference extension cannot run in the build container (no GPU); tests/test_tiles_gpu.py compares this
-oracle AND the kernels with the unmodified extension on the GPU box when baseline/_ref is staged.
+PARITY PIN: the reference extension needs a GPU; tests/test_tiles_gpu.py compares the kernels with this oracle and with
+stored outputs of the unmodified extension (golden tiles_ref, written on an H100 by tests/golden/make_golden.py --gpu).
 """
 import math
 

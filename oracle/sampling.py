@@ -1,6 +1,6 @@
 """Oracle restatement of the sampling stage (TEST INFRASTRUCTURE, see oracle/__init__.py).
 
-Follows /root/reference/gauss_to_pc.py:73-371 and torch.distributions.MultivariateNormal
+Follows gauss_to_pc.py:73-371 and torch.distributions.MultivariateNormal
 (torch 2.11 multivariate_normal.py:194 Cholesky, :251-254 rsample = loc + L @ eps).  torch-CPU routines are used
 for Cholesky / inverse / bmm so the arithmetic matches the reference's CPU run; the random draw is injected
 (`eps_fn`) because the product defines its own counter-based stream (oracle/philox.py).

@@ -14,7 +14,7 @@ def pytest_configure(config):
     # the GPU box has >100 host cores: torch-CPU oracle ops on small tensors crawl when oversubscribed
     import torch
     torch.set_num_threads(min(8, os.cpu_count() or 1))
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,11 +1,10 @@
-"""Generate the golden vectors that pin the oracle: outputs of the UNMODIFIED reference (/root/reference) run on
-CPU through oracle/ref_shim.py on small seeded scenes.  Run in the build container (the reference does not exist on
-the GPU box):
+"""Generate the golden vectors that pin the oracle and the kernels: outputs of the UNMODIFIED reference, on small
+seeded scenes.  Inputs are regenerated from the seeds by g2pc.synth, so only outputs are stored.
 
-    python tests/golden/make_golden.py
-
-Writes tests/golden/sampling_*.npz (and colour_*.npz).  Inputs are regenerated from the seeds by g2pc.synth, so only
-outputs are stored.
+    G2PC_REFERENCE_ROOT=<reference checkout> python tests/golden/make_golden.py          CPU vectors, through
+                                                                                         oracle/ref_shim.py
+    python tests/golden/make_golden.py --gpu        tiles_ref.npz: the reference's CUDA rasterizer (compiled into
+                                                    oracle/_ref by oracle/build_ref.py), run on an H100
 """
 import os
 import sys
@@ -97,9 +96,129 @@ def make_sh(name="sh_a", n=400, seed=1320):
     print(name, {k: v.shape for k, v in out.items()})
 
 
+def _sha(a):
+    import hashlib
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), dtype=np.uint8)
+
+
+def make_live_small(name="live_small"):
+    """generate_pointcloud of the reference on a 600-Gaussian scene (eps keyed by seed 5): the shape and the SHA-256 of
+    the exact bytes of its points and colours (bit-exact comparison without storing the cloud)."""
+    ref = ref_shim.load()
+    sc = synth.make_scene(600, seed=77)
+    eps_fn = lambda g, k, a: philox.draw_eps(g, k, a, 5, 0)
+    with ref_shim.cpu_redirect():
+        G = ref.gauss_handler.Gaussians(sc["xyz"].clone(), sc["scales"].clone(), sc["rots"].clone(),
+                                        sc["colours"].clone() * 255, sc["opacities"].clone())
+        G.calculate_normals()
+        G.validate_covariances()
+        with ref_shim.EpsInjector(ref, G.xyz, eps_fn):
+            pts, cols, nrm = ref.gauss_to_pc.generate_pointcloud(G, 5000, device="cpu", quiet=True)
+    np.savez_compressed(os.path.join(HERE, name + ".npz"), meta=np.array([600, 77, 5000, 5], dtype=np.int64),
+                        points_shape=np.array(pts.shape, dtype=np.int64), points_dtype=np.array(str(pts.dtype)),
+                        colours_dtype=np.array(str(cols.dtype)), points_sha256=_sha(pts.numpy()),
+                        colours_sha256=_sha(cols.numpy()))
+    print(name, "points", tuple(pts.shape), pts.dtype, cols.dtype)
+
+
+def make_transforms(name="transforms_ref"):
+    """load_transform_data of the reference on the transforms.json / COLMAP text / COLMAP binary files that
+    tests/test_io_cpu.py writes, skip rates 0 and 2: names, 4x4 matrices and intrinsics."""
+    import tempfile
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_io_cpu import write_transforms_json, _write_colmap
+    ref = ref_shim.load()
+    cams, intr = synth.make_cameras(7)
+    out = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        for kind in ("json", "colmap_txt", "colmap_bin"):
+            if kind == "json":
+                path = os.path.join(tmp, "transforms.json")
+                write_transforms_json(path, cams, intr)
+            else:
+                path = os.path.join(tmp, kind)
+                _write_colmap(path, cams, binary=(kind == "colmap_bin"))
+            for skip in (0, 2):
+                tr, ik = ref.transform_dataloader.load_transform_data(path, skip_rate=skip)
+                key = f"{kind}_{skip}"
+                out[key + "_names"] = np.array(list(tr.keys()))
+                out[key + "_matrices"] = np.array([np.asarray(tr[k], dtype=np.float64) for k in tr])
+                out[key + "_intrinsics"] = np.array([[float(v) for v in ik[k]] for k in tr], dtype=np.float64)
+    np.savez_compressed(os.path.join(HERE, name + ".npz"), **out)
+    print(name, sorted(out))
+
+
+TILES_REF = dict(n=8000, scene_seed=1253, ncams=4, res=720, pixels=1024, pixel_seed=7)
+
+
+def _reference_C():
+    """The reference's compiled `_C` from oracle/_ref, loaded on its own (the product ships a package of the same name)."""
+    import glob
+    import importlib.util
+    so = glob.glob(os.path.join(ROOT, "oracle", "_ref", "gaussian_pointcloud_rasterization", "_C*.so"))
+    if not so:
+        raise SystemExit("oracle/_ref holds no reference extension: run oracle/build_ref.py first")
+    spec = importlib.util.spec_from_file_location("g2pc_reference_ext._C", so[0])
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def make_tiles_ref(name="tiles_ref"):
+    """The reference's CUDA rasterizer (rasterize_gaussians, surface distance on) over TILES_REF's scene and cameras,
+    camera matrices from oracle.render_cuda.RasterSettings, per-camera outputs accumulated as the reference's
+    GaussianRasterizer.forward does.  Stored: radii per camera, colour + depth at a seeded sample of pixels per camera,
+    the accumulated max / total contributions and the low-surface-distance mask (std 2.0)."""
+    from oracle import gaussians as og, render_cuda as orc
+    C = _reference_C()
+    t = TILES_REF
+    dev = "cuda:0"
+    sc = synth.make_scene(t["n"], seed=t["scene_seed"], sh_degree=3)
+    cov = og.build_covariance(sc["scales"], sc["rots"])
+    cov6 = cov.reshape(-1, 9)[:, [0, 1, 2, 4, 5, 8]].float().to(dev)
+    xyz, col = sc["xyz"].float().to(dev), sc["colours"].float().to(dev)
+    opa = sc["opacities"].float().unsqueeze(1).to(dev)
+    n = t["n"]
+    kmax = torch.zeros(n, device=dev)
+    ktot = torch.zeros(n, device=dev)
+    kdist = torch.full((n,), torch.finfo(torch.float).max, device=dev)
+    empty = torch.Tensor([])
+    cams, intr = synth.make_cameras(t["ncams"])
+    radii, img_s, dep_s = [], [], []
+    for c2w, k in zip(cams, intr):
+        rs = orc.RasterSettings(c2w, k, colour_resolution=t["res"])
+        H, W = rs.image_height, rs.image_width
+        mask = torch.ones(H * W, dtype=torch.int32, device=dev)
+        out = C.rasterize_gaussians(torch.as_tensor(rs.bg, device=dev), xyz, col, opa, empty, empty, 1.0, cov6,
+                                    rs.viewmatrix.to(dev), rs.projmatrix.to(dev), rs.tanfovx, rs.tanfovy, H, W, empty, 3,
+                                    rs.campos.to(dev), mask, False, False, True, True)
+        _, colour, depth, r, _, _, _, _, contrib, surf, _ = out
+        upd = contrib > kmax
+        kmax[upd] = contrib[upd]
+        ktot += contrib
+        kdist = torch.minimum(kdist, surf)
+        pix = np.random.default_rng(t["pixel_seed"]).choice(H * W, t["pixels"], replace=False)
+        p = torch.as_tensor(pix, device=dev)
+        radii.append(r.cpu().numpy().astype(np.int16))
+        img_s.append(colour.reshape(3, -1)[:, p].cpu().numpy())
+        dep_s.append(depth.reshape(-1)[p].cpu().numpy())
+    fin = kdist < torch.finfo(torch.float).max
+    low = kdist < kdist[fin].mean() * 2.0
+    np.savez_compressed(os.path.join(HERE, name + ".npz"), meta=np.array([t[k] for k in TILES_REF], dtype=np.int64),
+                        radii=np.stack(radii), image_sample=np.stack(img_s), depth_sample=np.stack(dep_s),
+                        max_contribution=kmax.cpu().numpy(), total_contribution=ktot.cpu().numpy(),
+                        low_surface=low.cpu().numpy(), gpu=np.array(torch.cuda.get_device_name(0)))
+    print(name, "radii", np.stack(radii).shape, "seen", int((kmax > 0).sum()))
+
+
 if __name__ == "__main__":
     torch.manual_seed(0)
+    if "--gpu" in sys.argv:
+        make_tiles_ref()
+        raise SystemExit(0)
     make_sh()
+    make_live_small()
+    make_transforms()
     for name, args in SAMPLING_CASES.items():
         make_sampling(name, *args)
     for name, args in COLOUR_CASES.items():

@@ -1,12 +1,17 @@
 """Tiny run of both colour back-ends + the sampler, meant to be executed under compute-sanitizer
 (tests/test_sanitizer_gpu.py): memcheck over every g2pc kernel, racecheck over the shared-memory protocols of the blend
-(TMA / cp.async staging buffers, s_best merge) and the multisplit bit matrix."""
+(TMA / cp.async staging buffers, s_best merge) and the multisplit bit matrix.
+
+Without the sanitizer (tests/test_sanitizer_gpu.py runs it directly when the tool does not support the GPU):
+  G2PC_TARGET_POISON=<byte>   every block PyTorch's caching allocator hands out afterwards starts filled with <byte>
+  G2PC_TARGET_OUT=<file.npz>  every output of the run is saved there, for bit-for-bit comparison between runs"""
 import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "3dgs-to-pc_b200"))
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import camera_handler as ch  # noqa: E402
@@ -16,6 +21,24 @@ import gauss_to_pc as g2p  # noqa: E402
 from g2pc import synth  # noqa: E402
 
 dev = "cuda:0"
+
+
+def poison_allocator(byte):
+    """Fill and release blocks of both pools of the caching allocator (it keeps them cached), so a kernel that reads
+    memory nobody wrote sees `byte`.  Small pool: blocks of <= 1 MB carved from 2 MB segments; large pool: split blocks."""
+    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(64)]
+    large = [torch.full((256 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(4)]
+    torch.cuda.synchronize()
+    del small, large
+    for nbytes in (4096, 8 << 20):  # later blocks of both pools really start out filled
+        probe = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
+        del probe
+
+
+if os.environ.get("G2PC_TARGET_POISON") is not None:
+    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
+outputs = {}
 sc = synth.make_scene(1500, seed=31, sh_degree=3)
 d = {k: v.to(dev) for k, v in sc.items()}
 G = gh.Gaussians(d["xyz"], d["scales"], d["rots"], d["colours"], d["opacities"], shs=d["shs"])
@@ -31,9 +54,17 @@ for rtype in ("python", "cuda"):
     R.flush()
     mc = R.gaussian_max_contribution
     assert float(mc.max()) > 0
+    outputs[rtype + "_max_contribution"] = mc
+    outputs[rtype + "_colours"] = R.get_gaussian_colours()
+    if rtype == "cuda":
+        outputs["cuda_total_contribution"] = R.gaussian_total_contribution
+        outputs["cuda_min_surface_distance"] = R.gaussian_min_surface_distance
 G.colours = G.colours * 255
 idx = G.fused_cull(max_contribution=mc, visibility_threshold=0.01)
 G.validate_covariances()
 pts, cols, nrm = g2p.generate_pointcloud(G, 20000, quiet=True)
 torch.cuda.synchronize()
+if os.environ.get("G2PC_TARGET_OUT"):
+    outputs.update(cull_index=idx, points=pts, point_colours=cols, point_normals=nrm)
+    np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
 print("SANITIZER_TARGET_OK", pts.shape[0], idx.shape[0])

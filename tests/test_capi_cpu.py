@@ -40,15 +40,15 @@ def test_missing_library_fails_loudly(tmp_path):
         capi.load(str(tmp_path / "nope.so"))
 
 
-def test_sass_is_sm100a(lib):
-    """The shipped library carries sm_100a code (no PTX-JIT fallback to another arch)."""
+def test_sass_is_sm90a(lib):
+    """The shipped library carries sm_90a code (no PTX-JIT fallback to another arch)."""
     import shutil
     import subprocess
     from g2pc import capi
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     out = subprocess.run(["cuobjdump", "-lelf", capi.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_product_never_imports_the_oracle():

@@ -1,5 +1,6 @@
-"""CPU: the thin host-side loaders (3dgs-to-pc_b200/gauss_dataloader.py, transform_dataloader.py) — self-consistency and,
-when /root/reference is present, equality with the reference's own parsers on generated COLMAP / transforms.json files."""
+"""CPU: the thin host-side loaders (3dgs-to-pc_b200/gauss_dataloader.py, transform_dataloader.py) — self-consistency and
+equality with what the reference's own parsers read from the same generated COLMAP / transforms.json files (golden
+transforms_ref, tests/golden/make_golden.py)."""
 import json
 import os
 import struct
@@ -7,6 +8,8 @@ import struct
 import numpy as np
 import pytest
 import torch
+
+from util import GOLDEN
 
 
 def write_gaussian_ply(path, sc, sh_degree=3):
@@ -115,19 +118,17 @@ def test_transform_loaders_match_reference(tmp_path, kind):
     else:
         path = str(tmp_path / kind)
         _write_colmap(path, cams, binary=(kind == "colmap_bin"))
+    ref = np.load(os.path.join(GOLDEN, "transforms_ref.npz"))
     for skip in (0, 2):
         tr, ik = td.load_transform_data(path, skip_rate=skip)
         assert len(tr) >= 1 and set(tr.keys()) <= set(ik.keys())
         for k, m in tr.items():
             assert np.asarray(m).shape == (4, 4)
-        from oracle import ref_shim
-        if ref_shim.available():
-            ref = ref_shim.load()
-            rtr, rik = ref.transform_dataloader.load_transform_data(path, skip_rate=skip)
-            assert list(rtr.keys()) == list(tr.keys())
-            for k in tr:
-                assert np.allclose(np.asarray(tr[k], dtype=np.float64), np.asarray(rtr[k], dtype=np.float64), atol=1e-12)
-                assert [float(v) for v in ik[k]] == [float(v) for v in rik[k]]
+        key = f"{kind}_{skip}"
+        assert list(tr.keys()) == [str(v) for v in ref[key + "_names"]]
+        for i, k in enumerate(tr):
+            assert np.allclose(np.asarray(tr[k], dtype=np.float64), ref[key + "_matrices"][i], atol=1e-12)
+            assert [float(v) for v in ik[k]] == [float(v) for v in ref[key + "_intrinsics"][i]]
     if kind == "json":
         tr, ik = td.load_transform_data(path)
         assert np.allclose(np.asarray(tr["frame_0003"]), cams[3].numpy())
