@@ -87,6 +87,43 @@ __device__ __forceinline__ float3 draw_eps(uint32_t gid, uint32_t sample, uint32
     return make_float3(ra * ca, ra * sa, rb * cb);
 }
 
+// Eigenvalues of a symmetric 3x3 (row-major f32, off-diagonal pairs averaged like a general solver sees them),
+// trigonometric closed form in f64, returned ASCENDING.  Used by g2pc_eigvals_sym3 (s1_cov.cu) and the magnitudes
+// kernel (s8_cull.cu).  A diagonal matrix (p1 == 0: identity / axis-aligned quaternions) takes the diagonal as is, and
+// l1 = 3q - l0 - l2 may round past a nearly equal neighbour, so the three values are sorted before they are returned.
+__device__ __forceinline__ void g2pc_eig3_sym(const float* S, double& lo, double& mid, double& hi) {
+    const double a00 = S[0], a11 = S[4], a22 = S[8];
+    const double a01 = 0.5 * ((double)S[1] + (double)S[3]);
+    const double a02 = 0.5 * ((double)S[2] + (double)S[6]);
+    const double a12 = 0.5 * ((double)S[5] + (double)S[7]);
+    const double p1 = a01 * a01 + a02 * a02 + a12 * a12;
+    const double q = (a00 + a11 + a22) / 3.0;
+    double l0, l1, l2;
+    if (p1 == 0.0) {
+        l0 = a00; l1 = a11; l2 = a22;
+    } else {
+        const double d0 = a00 - q, d1 = a11 - q, d2 = a22 - q;
+        const double p2 = d0 * d0 + d1 * d1 + d2 * d2 + 2.0 * p1;
+        const double p = sqrt(p2 / 6.0);
+        const double ip = 1.0 / p;
+        const double b00 = d0 * ip, b11 = d1 * ip, b22 = d2 * ip;
+        const double b01 = a01 * ip, b02 = a02 * ip, b12 = a12 * ip;
+        double r = 0.5 * (b00 * (b11 * b22 - b12 * b12) - b01 * (b01 * b22 - b12 * b02) +
+                          b02 * (b01 * b12 - b11 * b02));
+        r = r < -1.0 ? -1.0 : (r > 1.0 ? 1.0 : r);
+        const double phi = acos(r) / 3.0;
+        l0 = q + 2.0 * p * cos(phi);
+        l2 = q + 2.0 * p * cos(phi + 2.0943951023931953);
+        l1 = 3.0 * q - l0 - l2;
+    }
+    // three-element sorting network
+    double t;
+    if (l0 > l1) { t = l0; l0 = l1; l1 = t; }
+    if (l1 > l2) { t = l1; l1 = l2; l2 = t; }
+    if (l0 > l1) { t = l0; l0 = l1; l1 = t; }
+    lo = l0; mid = l1; hi = l2;
+}
+
 // x = mu + L*eps with L lower-triangular (l00,l10,l11,l20,l21,l22); the SAME expression is used by the
 // count pass (explicit Mahalanobis) and the emit pass, so both see bit-identical positions.
 __device__ __forceinline__ float3 mvn_point(const float3 mu, float l00, float l10, float l11, float l20,

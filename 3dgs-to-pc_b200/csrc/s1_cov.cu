@@ -117,35 +117,11 @@ __global__ void __launch_bounds__(256) eigvals_sym3_kernel(const float* __restri
     for (int k = threadIdx.x; k < cnt * 9; k += 256) tile[k] = cov[base * 9 + k];
     __syncthreads();
     if (threadIdx.x >= cnt) return;
-    const float* S = tile + threadIdx.x * 9;
-    // symmetrise like a general eigen-solver sees it: use the average of the off-diagonal pairs
-    const double a00 = S[0], a11 = S[4], a22 = S[8];
-    const double a01 = 0.5 * ((double)S[1] + (double)S[3]);
-    const double a02 = 0.5 * ((double)S[2] + (double)S[6]);
-    const double a12 = 0.5 * ((double)S[5] + (double)S[7]);
-    const double p1 = a01 * a01 + a02 * a02 + a12 * a12;
-    const double q = (a00 + a11 + a22) / 3.0;
-    double l0, l1, l2;
-    if (p1 == 0.0) {
-        l0 = a00; l1 = a11; l2 = a22;
-    } else {
-        const double d0 = a00 - q, d1 = a11 - q, d2 = a22 - q;
-        const double p2 = d0 * d0 + d1 * d1 + d2 * d2 + 2.0 * p1;
-        const double p = sqrt(p2 / 6.0);
-        const double ip = 1.0 / p;
-        const double b00 = d0 * ip, b11 = d1 * ip, b22 = d2 * ip;
-        const double b01 = a01 * ip, b02 = a02 * ip, b12 = a12 * ip;
-        double r = 0.5 * (b00 * (b11 * b22 - b12 * b12) - b01 * (b01 * b22 - b12 * b02) +
-                          b02 * (b01 * b12 - b11 * b02));
-        r = r < -1.0 ? -1.0 : (r > 1.0 ? 1.0 : r);
-        const double phi = acos(r) / 3.0;
-        l0 = q + 2.0 * p * cos(phi);
-        l2 = q + 2.0 * p * cos(phi + 2.0943951023931953);
-        l1 = 3.0 * q - l0 - l2;
-    }
+    double lo, mid, hi;
+    g2pc_eig3_sym(tile + threadIdx.x * 9, lo, mid, hi);
     // ascending order, rounded to f32 (the reference's eigvals are f32: gauss_handler.py:112,259)
     float* o = eig + (base + threadIdx.x) * 3;
-    o[0] = (float)l2; o[1] = (float)l1; o[2] = (float)l0;
+    o[0] = (float)lo; o[1] = (float)mid; o[2] = (float)hi;
 }
 
 }  // namespace

@@ -3,8 +3,10 @@ seeded scenes.  Inputs are regenerated from the seeds by g2pc.synth, so only out
 
     G2PC_REFERENCE_ROOT=<reference checkout> python tests/golden/make_golden.py          CPU vectors, through
                                                                                          oracle/ref_shim.py
-    python tests/golden/make_golden.py --gpu        tiles_ref.npz: the reference's CUDA rasterizer (compiled into
-                                                    oracle/_ref by oracle/build_ref.py), run on an H100
+    python tests/golden/make_golden.py --gpu        tiles_ref.npz, tiles_edge.npz: the reference's CUDA rasterizer
+                                                    (compiled into oracle/_ref by oracle/build_ref.py), run on an H100
+    --edge                                          only the edge-scene vectors (colour_edge.npz, or tiles_edge.npz
+                                                    with --gpu)
 """
 import os
 import sys
@@ -148,6 +150,80 @@ def make_transforms(name="transforms_ref"):
     print(name, sorted(out))
 
 
+def _edge_scenes():
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import edge_scenes
+    return edge_scenes.golden_scenes()
+
+
+def make_colour_edge(name="colour_edge"):
+    """GaussPythonRenderer of the reference on the edge scenes (inside, huge, ties, opacity), tile parameters pinned to
+    (60, 60000), every camera at its native size: images, accumulated max contributions and colours per scene."""
+    ref = ref_shim.load()
+    out = {}
+    for key, (sc, cams, intr) in _edge_scenes().items():
+        with ref_shim.cpu_redirect(pinned_tiles=(60, 60000)):
+            G = ref.gauss_handler.Gaussians(sc["xyz"].clone(), sc["scales"].clone(), sc["rots"].clone(),
+                                            sc["colours"].clone(), sc["opacities"].clone())
+            R = ref.gauss_render.get_renderer("python", G.xyz, torch.unsqueeze(torch.clone(G.opacities), 1), G.colours,
+                                              G.covariances, visible_gaussian_threshold=0.05)
+            imgs = []
+            for c2w, k in zip(cams, intr):
+                cam = ref.camera_handler.get_camera("python", c2w.clone(), k, colour_resolution=int(k[0]))
+                img, _, _, _ = R(cam)
+                imgs.append(img.numpy().astype(np.float32))
+            out[f"{key}_cov"] = G.covariances.numpy()
+            out[f"{key}_images"] = np.stack(imgs)
+            out[f"{key}_max_contribution"] = R.gaussian_max_contribution.numpy()
+            out[f"{key}_colours"] = R.gaussian_colours.numpy()
+        print(name, key, out[f"{key}_images"].shape, "seen", int((out[f"{key}_max_contribution"] > 0).sum()))
+    np.savez_compressed(os.path.join(HERE, name + ".npz"), **out)
+
+
+def make_tiles_edge(name="tiles_edge"):
+    """The reference's CUDA rasterizer (surface distance on) on the edge scenes, camera matrices from
+    oracle.render_cuda.RasterSettings at native size: per camera radii and full colour / depth images, accumulated max /
+    total contributions and minimum surface distances per scene."""
+    from oracle import gaussians as og, render_cuda as orc
+    C = _reference_C()
+    dev = "cuda:0"
+    out = {}
+    for key, (sc, cams, intr) in _edge_scenes().items():
+        cov = og.build_covariance(sc["scales"], sc["rots"])
+        cov6 = cov.reshape(-1, 9)[:, [0, 1, 2, 4, 5, 8]].float().to(dev)
+        xyz, col = sc["xyz"].float().to(dev), sc["colours"].float().to(dev)
+        opa = sc["opacities"].float().unsqueeze(1).to(dev)
+        n = xyz.shape[0]
+        kmax = torch.zeros(n, device=dev)
+        ktot = torch.zeros(n, device=dev)
+        kdist = torch.full((n,), torch.finfo(torch.float).max, device=dev)
+        empty = torch.Tensor([])
+        radii, imgs, deps = [], [], []
+        for c2w, k in zip(cams, intr):
+            rs = orc.RasterSettings(c2w, k)
+            H, W = rs.image_height, rs.image_width
+            mask = torch.ones(H * W, dtype=torch.int32, device=dev)
+            o = C.rasterize_gaussians(torch.as_tensor(rs.bg, device=dev), xyz, col, opa, empty, empty, 1.0, cov6,
+                                      rs.viewmatrix.to(dev), rs.projmatrix.to(dev), rs.tanfovx, rs.tanfovy, H, W, empty,
+                                      3, rs.campos.to(dev), mask, False, False, True, True)
+            _, colour, depth, r, _, _, _, _, contrib, surf, _ = o
+            upd = contrib > kmax
+            kmax[upd] = contrib[upd]
+            ktot += contrib
+            kdist = torch.minimum(kdist, surf)
+            radii.append(r.cpu().numpy().astype(np.int32))
+            imgs.append(colour.cpu().numpy())
+            deps.append(depth[0].cpu().numpy())
+        out[f"{key}_radii"] = np.stack(radii)
+        out[f"{key}_images"] = np.stack(imgs)
+        out[f"{key}_depths"] = np.stack(deps)
+        out[f"{key}_max_contribution"] = kmax.cpu().numpy()
+        out[f"{key}_total_contribution"] = ktot.cpu().numpy()
+        out[f"{key}_min_surface_distance"] = kdist.cpu().numpy()
+        print(name, key, out[f"{key}_images"].shape, "seen", int((kmax > 0).sum()))
+    np.savez_compressed(os.path.join(HERE, name + ".npz"), gpu=np.array(torch.cuda.get_device_name(0)), **out)
+
+
 TILES_REF = dict(n=8000, scene_seed=1253, ncams=4, res=720, pixels=1024, pixel_seed=7)
 
 
@@ -213,13 +289,18 @@ def make_tiles_ref(name="tiles_ref"):
 
 if __name__ == "__main__":
     torch.manual_seed(0)
+    edge_only = "--edge" in sys.argv  # only the edge-scene vectors (colour_edge, or tiles_edge with --gpu)
     if "--gpu" in sys.argv:
-        make_tiles_ref()
+        if not edge_only:
+            make_tiles_ref()
+        make_tiles_edge()
         raise SystemExit(0)
-    make_sh()
-    make_live_small()
-    make_transforms()
-    for name, args in SAMPLING_CASES.items():
-        make_sampling(name, *args)
-    for name, args in COLOUR_CASES.items():
-        make_colour(name, *args)
+    if not edge_only:
+        make_sh()
+        make_live_small()
+        make_transforms()
+        for name, args in SAMPLING_CASES.items():
+            make_sampling(name, *args)
+        for name, args in COLOUR_CASES.items():
+            make_colour(name, *args)
+    make_colour_edge()

@@ -223,3 +223,45 @@ def test_cli_default_flags_and_surface_distance(lib, tmp_path):
     assert abs(v2.shape[0] - 30000) < 300
     with pytest.raises(AttributeError):
         g2p.config_parser(["--input_path", ply, "--transform_path", tj, "--generate_mesh"])
+
+
+@pytest.mark.parametrize("scene", ["inside", "huge", "ties", "opacity"])
+def test_tiles_vs_reference_extension_on_edge_scenes(lib, scene):
+    """Kernels against the unmodified reference rasterizer on the edge scenes of tests/edge_scenes.py (golden tiles_edge,
+    computed on an H100 by tests/golden/make_golden.py --gpu): radii, images, depths, accumulated contributions and
+    surface distances.  The reference under-reports maxima run-dependently (see test_tiles_vs_reference_extension), so
+    contributions are compared one-sidedly; its exact depth ties follow its radix sort, as the kernels' do."""
+    import os
+    import camera_handler as ch
+    from edge_scenes import golden_scenes
+    from g2pc.rasterizer import GaussianRasterizer
+    from oracle import gaussians as og
+    from util import GOLDEN
+    path = os.path.join(GOLDEN, "tiles_edge.npz")
+    g = np.load(path)
+    sc, cams, intr = golden_scenes()[scene]
+    cov = og.build_covariance(sc["scales"], sc["rots"])
+    d = scene_to(sc, DEV)
+    R = GaussianRasterizer(d["xyz"], None, d["opacities"], colors_precomp=d["colours"].float(), cov3D_precomp=cov.to(DEV),
+                           calculate_surface_distance=True)
+    n = sc["xyz"].shape[0]
+    rflips, worst, off_px = 0, 0.0, 0
+    for i, (c2w, k) in enumerate(zip(cams, intr)):
+        img, radii, _, dep = R(ch.get_camera("cuda", c2w.to(DEV), k))
+        rflips += int((radii.cpu().numpy() != g[f"{scene}_radii"][i]).sum())
+        e = np.abs(img.cpu().numpy() - g[f"{scene}_images"][i])
+        worst = max(worst, float(e.max()))
+        off_px += int((e > 2e-4).sum())
+        assert float(e.max()) < 5e-3, f"camera {i}: image max diff {e.max():.2e}"
+        ed = np.abs(dep.cpu().numpy()[0] - g[f"{scene}_depths"][i])
+        assert int((ed > 1e-3).sum()) <= max(2, int(2e-3 * ed.size)), f"camera {i}: depth"
+    assert rflips <= max(1, int(3e-4 * n * len(cams))), f"{rflips} radius flips"
+    assert off_px <= max(3, int(2e-3 * img.numel() * len(cams))), f"{off_px} image values off by > 2e-4"
+    km, rm = R.gaussian_max_contribution.cpu().numpy(), g[f"{scene}_max_contribution"]
+    below = int((km < rm - 1e-4).sum())
+    assert below <= max(1, int(2e-4 * n)), f"{below} maxima below the reference's"
+    kd, rd = R.gaussian_min_surface_distance.cpu().numpy(), g[f"{scene}_min_surface_distance"]
+    cover = int(((kd < 3e38) != (rd < 3e38)).sum())
+    assert cover <= max(2, int(1e-3 * n)), f"{cover} surface distances defined on one side only"
+    print(f"[vs reference ext, edge {scene}] image max diff {worst:.2e} ({off_px} values > 2e-4), radius flips "
+          f"{rflips}, maxima below the reference's {below}, surface-distance coverage differs {cover}")
