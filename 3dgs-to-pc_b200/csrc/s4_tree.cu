@@ -17,13 +17,15 @@
 //                           sets the sticky POISON word: every later kernel of this and the following frames becomes a
 //                           no-op until the host has read the header, fixed the sizes and replayed.
 //   3. g2pc_multisplit      stable one-pass-per-chunk multisplit of the depth-ordered stream into the leaves' lists:
-//        count    CTA c takes 256 consecutive sorted entries and counts its instances per leaf (shared-memory histogram)
+//        count    CTA c takes E = S x C consecutive sorted entries (2 sub-steps of C = 256 at C3) and counts its
+//                 instances per leaf (shared-memory histogram)
 //        scan     per leaf, exclusive prefix over the chunks (+ the leaf's list offset)          -> matrix[c][leaf]
-//        scatter  CTA c marks bit (leaf, k) for every instance in a shared-memory bit matrix (order-free atomicOr); an
-//                 instance's place is matrix[c][leaf] + the set bits of its leaf before bit k (popc): the lists come out
-//                 depth-ordered without any sort of the ~7 N instances (the round-1 path emitted (leaf, id) pairs and
-//                 ran a 2-pass 20 M-pair radix sort per camera).  Splats that cover many tiles are walked by the whole
-//                 warp (colour_common.cuh warp_for_each_node).
+//        scatter  CTA c walks its sub-steps in order, starting from row c of the matrix; per sub-step it marks bit
+//                 (leaf, k) for every instance in a shared-memory bit matrix (order-free atomicOr); an instance's place
+//                 is the leaf's running offset + the set bits of its leaf before bit k (popc), then the offsets move past
+//                 the sub-step: the lists come out depth-ordered without any sort of the ~7 N instances (the round-1
+//                 path emitted (leaf, id) pairs and ran a 2-pass 20 M-pair radix sort per camera).  Splats that cover
+//                 many tiles are walked by the whole warp (colour_common.cuh warp_for_each_node).
 #include <cub/cub.cuh>
 #include "colour_common.cuh"
 
@@ -225,7 +227,7 @@ __global__ void __launch_bounds__(TB) tree_kernel(const TreeParams p) {
     if (threadIdx.x == 0) {
         const int cap_over = (inst_total > p.inst_capacity || (long long)pix_base > p.pix_capacity ||
                               (long long)p.ms_chunks * (long long)nl > p.matrix_capacity || inst_total > 0x7FFFFFFFll)
-                             // (ms_chunks = rows the multisplit needs: chunks + segments, g2pc_multisplit_rows)
+                             // (ms_chunks = rows the multisplit needs: one per chunk, g2pc_multisplit_rows)
                                  ? 1 : 0;
         p.header[G2PC_HDR_NUM_LEAVES] = leaf_base;
         p.header[G2PC_HDR_TOTAL_INST] = (int32_t)(inst_total & 0xFFFFFFFFll);
@@ -250,6 +252,7 @@ struct MsParams {
     int64_t n;
     const float4* proj;
     int32_t width, height;
+    float inv_width, inv_height;  // 1 / width, 1 / height (IEEE division on the host: no division subroutine on the device)
     QtMeta meta;
     QtTables tab;
     int32_t n1;
@@ -266,6 +269,7 @@ struct MsParams {
     int32_t base_clean;    // the base level has no dropped / degenerate node: membership = the packed range, no table look-ups
     uint32_t clean_mask;   // the same, per level
     int32_t grid_w;        // > 0: flat tile grid (s7_tiles.cu): leaf = iy * grid_w + ix, the packed range is the tile rect
+    int32_t steps;         // sub-steps of C entries per chunk (ms_steps)
 };
 
 // f(leaf, owner_lane, owner_gid) for every leaf the lane's entry overlaps; warp-cooperative (all 32 lanes must call).
@@ -320,7 +324,7 @@ __device__ __forceinline__ void for_each_leaf(const MsParams& p, const QtTables&
         const float4 q2 = __ldg(p.proj + 3 * (int64_t)gid + 2);
         gaussian_rect(q0.x, q0.y, q2.z, p.width, p.height, x0, x1, y0, y1);
     }
-    const float isx0 = 1.0f / (float)p.width, isy0 = 1.0f / (float)p.height;
+    const float isx0 = p.inv_width, isy0 = p.inv_height;
     for (int l = lb + 1; l < p.meta.num_levels; ++l) {  // (uniform)
         if (!((p.level_mask >> l) & 1u)) continue;
         const int ol = (1 << l) - 1;
@@ -352,6 +356,14 @@ __device__ __forceinline__ void for_each_leaf(const MsParams& p, const QtTables&
     }
 }
 
+// The sorted stream is cut into chunks of E = steps x C consecutive entries, one CTA per chunk; a CTA walks its chunk in
+// `steps` sub-steps of C entries (one per thread), in stream order.  The per-chunk set-up (tables, node->leaf map, one
+// matrix row) is paid once per E entries, and the matrix (chunks x leaves) stays small enough to live in L2 (C3: 5.9 k
+// rows x 1024 leaves, 24 MB).
+__device__ __forceinline__ unsigned long long ms_entry(const MsParams& p, int64_t k) {
+    return k < p.n ? p.val_sorted[k] : (unsigned long long)G2PC_RANGE_EMPTY << 32;
+}
+
 // shared memory of the count / scatter kernels: [6 * n1 table ints][4^base node->leaf ints][payload]
 __device__ __forceinline__ int32_t* ms_load_common(const MsParams& p, int32_t* smem, QtTables& T) {
     if (p.grid_w > 0) { T = p.tab; return smem; }  // tile grid: nothing to stage
@@ -368,11 +380,13 @@ __device__ __forceinline__ int32_t* ms_load_common(const MsParams& p, int32_t* s
     return s_leaf;
 }
 
-// count:   matrix[c][leaf] = instances of `leaf` in chunk c (one CTA per chunk of C sorted entries)
-// scan:    per leaf, exclusive prefix over the chunks + the leaf's list offset (three small kernels, 32 x 32 tiles)
-// scatter: position = matrix[c][leaf] + rank inside the chunk (bit matrix)
+// count:   matrix[c][leaf] = instances of `leaf` in chunk c (one shared-memory histogram over the chunk's sub-steps)
+// scan:    per leaf, exclusive prefix over the chunks + the leaf's list offset (one kernel, 32 leaves per CTA)
+// scatter: position = running offset of the leaf + rank inside the sub-step (bit matrix)
+// (minimum CTAs per SM in the launch bounds: with the thread count alone ptxas held both kernels to 40-48 registers and
+// spilled; 1024 / C and 768 / C leave them 61 and 80 registers, no spill, and the scatter still fits 3 CTAs per SM at C = 256)
 template <int C>
-__global__ void __launch_bounds__(C) ms_count_kernel(const MsParams p) {
+__global__ void __launch_bounds__(C, 1024 / C) ms_count_kernel(const MsParams p) {
     extern __shared__ int32_t smem_ms[];
     if (g2pc_frame_skipped(p.fail, p.frame)) return;
     const int nl = p.header[G2PC_HDR_NUM_LEAVES];
@@ -381,88 +395,59 @@ __global__ void __launch_bounds__(C) ms_count_kernel(const MsParams p) {
     uint32_t* s_hist = reinterpret_cast<uint32_t*>(s_leaf + (p.grid_w > 0 ? 0 : (1 << (2 * p.base_level))));
     for (int i = threadIdx.x; i < nl; i += C) s_hist[i] = 0u;
     __syncthreads();
-    const int64_t k = (int64_t)blockIdx.x * C + threadIdx.x;
-    unsigned long long v = (unsigned long long)G2PC_RANGE_EMPTY << 32;
-    if (k < p.n) v = p.val_sorted[k];
-    for_each_leaf(p, T, s_leaf, (uint32_t)(v >> 32), (uint32_t)v,
-                  [&](int leaf, int, uint32_t) { atomicAdd(s_hist + leaf, 1u); });
+    // no barrier between the sub-steps: the warps only add to the histogram
+    const int64_t k0 = (int64_t)blockIdx.x * p.steps * C;
+    for (int s = 0; s < p.steps; ++s) {
+        const int64_t b = k0 + (int64_t)s * C;
+        if (b >= p.n) break;  // (uniform)
+        const unsigned long long v = ms_entry(p, b + threadIdx.x);
+        for_each_leaf(p, T, s_leaf, (uint32_t)(v >> 32), (uint32_t)v,
+                      [&](int leaf, int, uint32_t) { atomicAdd(s_hist + leaf, 1u); });
+    }
     __syncthreads();
     uint32_t* row = p.matrix + (int64_t)blockIdx.x * nl;
     for (int i = threadIdx.x; i < nl; i += C) row[i] = s_hist[i];
 }
 
-// Column-wise exclusive scan of matrix (rows x num_leaves) in three steps over tiles of 1024 rows x 32 leaves:
-//   partial: tile sums -> tile_sum[tile_row][leaf];  blocks: per leaf, scan of the tile sums + the leaf's list offset;
-//   apply: every tile rewrites its rows as running offsets.
-constexpr int SCAN_ROWS = 1024;  // rows per tile (32 per thread)
-__global__ void __launch_bounds__(1024) ms_scan_partial_kernel(const MsParams p, int32_t rows) {
+// Column-wise exclusive scan of matrix (rows x num_leaves), rewritten in place as absolute list offsets.  CTA = 32
+// leaves x 32 row bands: each thread sums its band of one column, the bands' sums are scanned in shared memory, then each
+// thread rewrites its band as running offsets.  The whole matrix is a few MB and was just written: L2 traffic only.
+constexpr int SCAN_BATCH = 8;  // matrix loads in flight per thread
+__global__ void __launch_bounds__(1024) ms_scan_kernel(const MsParams p, int32_t rows) {
     __shared__ uint32_t s_sum[32][33];
     if (g2pc_frame_skipped(p.fail, p.frame)) return;
     const int nl = p.header[G2PC_HDR_NUM_LEAVES];
+    if (blockIdx.x * 32 >= nl) return;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int leaf = blockIdx.x * 32 + tx;
-    if (blockIdx.x * 32 >= nl) return;
-    const int r0 = blockIdx.y * SCAN_ROWS + ty * 32;
+    const int band = (rows + 31) / 32;
+    const int r0 = min(rows, ty * band), r1 = min(rows, r0 + band);
+    uint32_t* col = p.matrix + leaf;
     uint32_t sum = 0;
     if (leaf < nl) {
 #pragma unroll 8
-        for (int r = r0; r < min(rows, r0 + 32); ++r) sum += p.matrix[(int64_t)r * nl + leaf];
+        for (int r = r0; r < r1; ++r) sum += col[(int64_t)r * nl];
     }
     s_sum[ty][tx] = sum;
     __syncthreads();
-    if (ty == 0 && leaf < nl) {
-        uint32_t t = 0;
-#pragma unroll
-        for (int s = 0; s < 32; ++s) t += s_sum[s][tx];
-        uint32_t* tile_sum = p.matrix + (int64_t)rows * nl;  // appended behind the rows
-        tile_sum[(int64_t)blockIdx.y * nl + leaf] = t;
-    }
-}
-
-__global__ void __launch_bounds__(256) ms_scan_blocks_kernel(const MsParams p, int32_t rows, int32_t tiles) {
-    if (g2pc_frame_skipped(p.fail, p.frame)) return;
-    const int nl = p.header[G2PC_HDR_NUM_LEAVES];
-    const int leaf = blockIdx.x * 256 + threadIdx.x;
     if (leaf >= nl) return;
-    uint32_t* tile_sum = p.matrix + (int64_t)rows * nl;
     uint32_t run = (uint32_t)p.leaves[leaf].inst_begin;
-    for (int t = 0; t < tiles; ++t) {
-        const uint32_t v = tile_sum[(int64_t)t * nl + leaf];
-        tile_sum[(int64_t)t * nl + leaf] = run;
-        run += v;
-    }
-}
-
-__global__ void __launch_bounds__(1024) ms_scan_apply_kernel(const MsParams p, int32_t rows) {
-    __shared__ uint32_t s_sum[32][33];
-    if (g2pc_frame_skipped(p.fail, p.frame)) return;
-    const int nl = p.header[G2PC_HDR_NUM_LEAVES];
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    const int leaf = blockIdx.x * 32 + tx;
-    if (blockIdx.x * 32 >= nl) return;
-    const int r0 = blockIdx.y * SCAN_ROWS + ty * 32, r1 = min(rows, r0 + 32);
-    uint32_t v[32];
-    uint32_t sum = 0;
-#pragma unroll
-    for (int q = 0; q < 32; ++q) {
-        v[q] = (leaf < nl && r0 + q < r1) ? p.matrix[(int64_t)(r0 + q) * nl + leaf] : 0u;
-        sum += v[q];
-    }
-    s_sum[ty][tx] = sum;
-    __syncthreads();
-    if (leaf >= nl) return;
-    const uint32_t* tile_sum = p.matrix + (int64_t)rows * nl;
-    uint32_t run = tile_sum[(int64_t)blockIdx.y * nl + leaf];
     for (int s = 0; s < ty; ++s) run += s_sum[s][tx];
+    for (int r = r0; r < r1; r += SCAN_BATCH) {
+        // load a batch before storing any of it (the stores would otherwise serialise the loads behind them)
+        uint32_t c[SCAN_BATCH];
 #pragma unroll
-    for (int q = 0; q < 32; ++q) {
-        if (r0 + q < r1) p.matrix[(int64_t)(r0 + q) * nl + leaf] = run;
-        run += v[q];
+        for (int q = 0; q < SCAN_BATCH; ++q) c[q] = r + q < r1 ? col[(int64_t)(r + q) * nl] : 0u;
+#pragma unroll
+        for (int q = 0; q < SCAN_BATCH; ++q) {
+            if (r + q < r1) col[(int64_t)(r + q) * nl] = run;
+            run += c[q];
+        }
     }
 }
 
 template <int C>
-__global__ void __launch_bounds__(C) ms_scatter_kernel(const MsParams p) {
+__global__ void __launch_bounds__(C, 768 / C) ms_scatter_kernel(const MsParams p) {
     extern __shared__ int32_t smem_ms[];
     if (g2pc_frame_skipped(p.fail, p.frame)) return;
     const int nl = p.header[G2PC_HDR_NUM_LEAVES];
@@ -484,25 +469,60 @@ __global__ void __launch_bounds__(C) ms_scatter_kernel(const MsParams p) {
         }
     }
     __syncthreads();
-    const int w = threadIdx.x >> 5;  // the warp = the 32-entry group of the chunk
+    const int w = threadIdx.x >> 5;  // the warp = the 32-entry group of the sub-step
     uint32_t* mybits = s_bits + w * nl;
-    const int64_t k = (int64_t)blockIdx.x * C + threadIdx.x;
-    unsigned long long v = (unsigned long long)G2PC_RANGE_EMPTY << 32;
-    if (k < p.n) v = p.val_sorted[k];
-    const uint32_t range = (uint32_t)(v >> 32), gid = (uint32_t)v;
-    // 1. mark (leaf, k) in the bit matrix: order-free
-    for_each_leaf(p, T, s_leaf, range, gid, [&](int leaf, int owner, uint32_t) { atomicOr(mybits + leaf, 1u << owner); });
-    __syncthreads();
-    // 2. every instance finds its place: the chunk's offset for the leaf, the instances of the same leaf in earlier
-    //    32-entry groups of the chunk, then the earlier lanes of its own group (bit order = depth order)
-    for_each_leaf(p, T, s_leaf, range, gid, [&](int leaf, int owner, uint32_t og) {
-        uint32_t pos = s_row[leaf] + (uint32_t)__popc(mybits[leaf] & ((1u << owner) - 1u));
-        for (int w2 = 0; w2 < w; ++w2) pos += (uint32_t)__popc(s_bits[w2 * nl + leaf]);
-        p.inst_gid[pos] = og;
-    });
+    const int64_t k0 = (int64_t)blockIdx.x * p.steps * C;
+    unsigned long long v = ms_entry(p, k0 + threadIdx.x);
+    for (int s = 0; s < p.steps; ++s) {
+        const int64_t b = k0 + (int64_t)s * C;
+        if (b >= p.n) break;  // (uniform)
+        const bool more = s + 1 < p.steps && b + C < p.n;
+        const uint32_t range = (uint32_t)(v >> 32), gid = (uint32_t)v;
+        // 1. mark (leaf, k) in the bit matrix: order-free
+        for_each_leaf(p, T, s_leaf, range, gid, [&](int leaf, int owner, uint32_t) { atomicOr(mybits + leaf, 1u << owner); });
+        __syncthreads();
+        const unsigned long long vn = more ? ms_entry(p, b + C + threadIdx.x) : 0ull;  // next sub-step, in flight early
+        // 2. every instance finds its place: the running offset of the leaf, the instances of the same leaf in earlier
+        //    32-entry groups of the sub-step, then the earlier lanes of its own group (bit order = depth order)
+        for_each_leaf(p, T, s_leaf, range, gid, [&](int leaf, int owner, uint32_t og) {
+            uint32_t pos = s_row[leaf] + (uint32_t)__popc(mybits[leaf] & ((1u << owner) - 1u));
+            for (int w2 = 0; w2 < w; ++w2) pos += (uint32_t)__popc(s_bits[w2 * nl + leaf]);
+            p.inst_gid[pos] = og;
+        });
+        if (!more) break;
+        __syncthreads();
+        // 3. move every leaf's offset past this sub-step's instances and clear the bit matrix for the next sub-step
+        for (int i = threadIdx.x; i < nl; i += C) {
+            uint32_t cnt = 0;
+#pragma unroll
+            for (int w2 = 0; w2 < WORDS; ++w2) {
+                cnt += (uint32_t)__popc(s_bits[w2 * nl + i]);
+                s_bits[w2 * nl + i] = 0u;
+            }
+            s_row[i] += cnt;
+        }
+        __syncthreads();
+        v = vn;
+    }
 }
 
 size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Sub-steps per chunk for n entries: as many as keep about MS_TARGET_CTAS chunks, ~10 waves of the 3 scatter CTAs an SM
+// of an H100 SXM (132 SMs) holds at C = 256.  Measured at 3 M Gaussians / 1280x720 (count + scatter per camera, H100
+// 80GB HBM3 at 400 W): 1 sub-step 565 us, 2 sub-steps (~4 k chunks) 522 us, 7 sub-steps (~1.5 k chunks) 601 us — longer
+// chunks save set-up but leave the waves unbalanced.  C3 (C = 256): 2 sub-steps, E = 512, 5860 chunks.
+constexpr int64_t MS_TARGET_CTAS = 4096;
+constexpr int64_t MS_MAX_STEPS = 32;
+int32_t ms_steps(int64_t n, int C) {
+    const int64_t s = n / ((int64_t)C * MS_TARGET_CTAS);
+    return (int32_t)(s < 1 ? 1 : (s > MS_MAX_STEPS ? MS_MAX_STEPS : s));
+}
+
+int32_t ms_chunks(int64_t n, int C) {
+    const int64_t e = (int64_t)C * ms_steps(n, C);
+    return (int32_t)((n + e - 1) / e);
+}
 
 template <int C>
 int launch_multisplit(const MsParams& p, int32_t chunks, cudaStream_t st) {
@@ -519,13 +539,7 @@ int launch_multisplit(const MsParams& p, int32_t chunks, cudaStream_t st) {
         G2PC_CUDA(cudaFuncSetAttribute(ms_scatter_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_scatter));
     ms_count_kernel<C><<<(unsigned)chunks, C, smem_count, st>>>(p);
     G2PC_CHECK_LAUNCH();
-    const int tiles = (chunks + SCAN_ROWS - 1) / SCAN_ROWS;
-    const dim3 sgrid((unsigned)((p.leaf_cap + 31) / 32), (unsigned)tiles);
-    ms_scan_partial_kernel<<<sgrid, 1024, 0, st>>>(p, chunks);
-    G2PC_CHECK_LAUNCH();
-    ms_scan_blocks_kernel<<<(unsigned)((p.leaf_cap + 255) / 256), 256, 0, st>>>(p, chunks, tiles);
-    G2PC_CHECK_LAUNCH();
-    ms_scan_apply_kernel<<<sgrid, 1024, 0, st>>>(p, chunks);
+    ms_scan_kernel<<<(unsigned)((p.leaf_cap + 31) / 32), 1024, 0, st>>>(p, chunks);
     G2PC_CHECK_LAUNCH();
     ms_scatter_kernel<C><<<(unsigned)chunks, C, smem_scatter, st>>>(p);
     G2PC_CHECK_LAUNCH();
@@ -585,7 +599,7 @@ extern "C" int g2pc_depth_sort(const uint32_t* depth_key, const uint64_t* val, i
 }
 
 extern "C" int32_t g2pc_multisplit_chunk(int32_t leaf_cap) {
-    // entries per chunk: the scatter kernel keeps leaf_cap x (chunk bits + one offset) in shared memory.  Prefer a
+    // entries per sub-step: the scatter kernel keeps leaf_cap x (sub-step bits + one offset) in shared memory.  Prefer a
     // footprint that lets 3 CTAs share an SM (the kernel is a chain of short latency-bound phases: with one resident CTA
     // per SM the 3600-tile grid of the CUDA back-end ran 3.5x slower per instance than the 1024 leaves of the python one)
     const int64_t n = leaf_cap;
@@ -598,11 +612,10 @@ extern "C" int32_t g2pc_multisplit_chunk(int32_t leaf_cap) {
 }
 
 extern "C" int32_t g2pc_multisplit_rows(int64_t n, int32_t leaf_cap) {
-    // matrix rows the multisplit needs for n entries: one per chunk + one per scan tile of 1024 chunks
+    // matrix rows the multisplit needs for n entries: one per chunk of ms_steps x C entries
     const int C = g2pc_multisplit_chunk(leaf_cap);
     if (C <= 0) return 0;
-    const int32_t chunks = (int32_t)((n + C - 1) / C);
-    return chunks + (chunks + SCAN_ROWS - 1) / SCAN_ROWS;
+    return ms_chunks(n, C);
 }
 
 extern "C" int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void* proj, int32_t width, int32_t height,
@@ -620,6 +633,7 @@ extern "C" int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void
     MsParams p;
     p.val_sorted = (const unsigned long long*)val_sorted; p.n = n; p.proj = (const float4*)proj;
     p.width = width; p.height = height;
+    p.inv_width = 1.0f / (float)width; p.inv_height = 1.0f / (float)height;
     p.meta.num_levels = num_levels; p.meta.max_gaussians_per_tile = 0; p.meta.width = width; p.meta.height = height;
     p.n1 = (1 << num_levels) - 1;
     p.tab.xs = tables; p.tab.xe = tables + p.n1; p.tab.xf = tables + 2 * p.n1;
@@ -631,7 +645,8 @@ extern "C" int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void
     p.leaf_cap = leaf_cap; p.grid_w = 0;
     p.base_clean = (int32_t)((clean_mask >> p.base_level) & 1u);
     p.clean_mask = clean_mask;
-    const int32_t chunks = (int32_t)((n + C - 1) / C);
+    p.steps = ms_steps(n, C);
+    const int32_t chunks = ms_chunks(n, C);
     cudaStream_t st = (cudaStream_t)stream;
     if (C == 256) return launch_multisplit<256>(p, chunks, st);
     if (C == 128) return launch_multisplit<128>(p, chunks, st);
@@ -651,7 +666,7 @@ extern "C" int g2pc_multisplit_grid(const uint64_t* val_sorted, int64_t n, int32
     G2PC_CHECK_ARG(C > 0, "too many tiles for the multisplit");
     MsParams p;
     p.val_sorted = (const unsigned long long*)val_sorted; p.n = n; p.proj = nullptr;
-    p.width = 0; p.height = 0;
+    p.width = 0; p.height = 0; p.inv_width = 0.f; p.inv_height = 0.f;
     p.meta.num_levels = 1; p.meta.max_gaussians_per_tile = 0; p.meta.width = 0; p.meta.height = 0;
     p.n1 = 0;
     p.tab.xs = p.tab.xe = p.tab.xf = p.tab.ys = p.tab.ye = p.tab.yf = nullptr;
@@ -659,7 +674,8 @@ extern "C" int g2pc_multisplit_grid(const uint64_t* val_sorted, int64_t n, int32
     p.node_leaf = nullptr; p.header = header; p.fail = fail; p.frame = frame; p.leaves = leaves; p.matrix = matrix;
     p.inst_gid = inst_gid;
     p.leaf_cap = leaf_cap; p.grid_w = grid_w; p.base_clean = 1; p.clean_mask = 1u;
-    const int32_t chunks = (int32_t)((n + C - 1) / C);
+    p.steps = ms_steps(n, C);
+    const int32_t chunks = ms_chunks(n, C);
     cudaStream_t st = (cudaStream_t)stream;
     if (C == 256) return launch_multisplit<256>(p, chunks, st);
     if (C == 128) return launch_multisplit<128>(p, chunks, st);

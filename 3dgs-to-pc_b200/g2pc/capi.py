@@ -122,7 +122,7 @@ LAUNCHES = 0      # number of hand-written g2pc kernels launched since the last 
 TIMING = None     # None, or a dict filled as {entry point name: [(start_event, end_event), ...]}: every launch is
                   # bracketed with CUDA events on the current stream (bench.py)
 # hand-written kernels launched per entry point (default 1); the radix sort inside g2pc_depth_sort is cub's (library)
-_OWN_KERNELS = {"g2pc_multisplit": 5, "g2pc_multisplit_grid": 5, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
+_OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
                 "g2pc_points_per_gaussian": 5}
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",
                 "g2pc_multisplit_rows", "g2pc_blend_set_compact", "g2pc_cull_workspace_bytes", "g2pc_ppg_workspace_bytes",

@@ -171,7 +171,7 @@ class GaussPythonRenderer(FrameQueue):
         if chunk <= 0:
             raise capi.G2pcError(f"the quadtree has more than {cap} leaves: too many for the multisplit tables")
         t["leaf_cap"], t["chunk"] = cap, chunk
-        t["chunks"] = int(self.lib.g2pc_multisplit_rows(self._n, cap))  # matrix rows: chunks + persistent CTAs
+        t["chunks"] = int(self.lib.g2pc_multisplit_rows(self._n, cap))  # matrix rows: one per multisplit chunk
         for ts in t["slots"]:
             ts["leaves"] = torch.zeros((cap, capi.LEAF_WORDS), dtype=torch.int32, device=self.device)
             ts["leaf_order"] = torch.zeros((cap,), dtype=torch.int32, device=self.device)

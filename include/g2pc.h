@@ -242,12 +242,13 @@ int g2pc_build_tree(const int32_t* tables, int32_t num_levels, int32_t max_gauss
                     void* stream);
 
 /* S4c.  Stable multisplit of the depth-ordered stream into the leaves' lists: inst_gid[leaf.inst_begin ..
- * + leaf.inst_count) = Gaussian ids overlapping the leaf, nearest first.  Three kernels (count, scan, scatter) over
- * chunks of C = g2pc_multisplit_chunk(leaf_cap) sorted entries; matrix: g2pc_multisplit_rows(n, leaf_cap) x leaves
- * uint32 scratch (pass that row count as ms_chunks to g2pc_build_tree, which checks the capacity).
+ * + leaf.inst_count) = Gaussian ids overlapping the leaf, nearest first.  Three kernels (count, scan, scatter); one CTA
+ * per chunk of S x C consecutive sorted entries, walked in S sub-steps of C = g2pc_multisplit_chunk(leaf_cap) entries
+ * (S grows with n: a few waves of CTAs on the GPU); matrix: g2pc_multisplit_rows(n, leaf_cap) x leaves uint32 scratch
+ * (pass that row count as ms_chunks to g2pc_build_tree, which checks the capacity).
  * leaf_cap = max_leaves given to g2pc_build_tree. */
-int32_t g2pc_multisplit_chunk(int32_t leaf_cap);
-int32_t g2pc_multisplit_rows(int64_t n, int32_t leaf_cap); /* rows of `matrix` needed (chunks + one per persistent CTA) */
+int32_t g2pc_multisplit_chunk(int32_t leaf_cap);           /* C: entries per sub-step (0: too many leaves) */
+int32_t g2pc_multisplit_rows(int64_t n, int32_t leaf_cap); /* rows of `matrix` needed: one per chunk */
 int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void* proj, int32_t width, int32_t height,
                     const int32_t* tables, int32_t num_levels, uint32_t level_mask, uint32_t clean_mask,
                     const int32_t* node_leaf, const g2pc_leaf_t* leaves, const int32_t* header, const uint32_t* fail,
