@@ -124,6 +124,36 @@ __device__ __forceinline__ void g2pc_eig3_sym(const float* S, double& lo, double
     lo = l0; mid = l1; hi = l2;
 }
 
+// Block-wide exclusive scan for 1024 threads: returns the thread's prefix and sets `total` to the block's sum.  s_warp is
+// 33 ints of shared memory; every thread must call.
+__device__ __forceinline__ int block_scan_1024(int v, int* s_warp, int& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        int w = s_warp[lane];
+        int winc = w;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, winc, o);
+            if (lane >= o) winc += t;
+        }
+        s_warp[lane] = winc - w;            // exclusive prefix of warp totals
+        if (lane == 31) s_warp[32] = winc;  // grand total
+    }
+    __syncthreads();
+    const int res = s_warp[warp] + inc - v;
+    total = s_warp[32];
+    __syncthreads();
+    return res;
+}
+
 // x = mu + L*eps with L lower-triangular (l00,l10,l11,l20,l21,l22); the SAME expression is used by the
 // count pass (explicit Mahalanobis) and the emit pass, so both see bit-identical positions.
 __device__ __forceinline__ float3 mvn_point(const float3 mu, float l00, float l10, float l11, float l20,

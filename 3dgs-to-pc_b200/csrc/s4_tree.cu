@@ -53,37 +53,6 @@ struct TreeParams {
     int32_t nodes_2d;
 };
 
-__device__ __forceinline__ int off2d(int l) { return ((1 << (2 * l)) - 1) / 3; }
-
-// block-wide exclusive scan for TB threads; returns prefix, sets total
-__device__ __forceinline__ int block_scan_1024(int v, int* s_warp, int& total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        int w = s_warp[lane];
-        int winc = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, winc, o);
-            if (lane >= o) winc += t;
-        }
-        s_warp[lane] = winc - w;      // exclusive prefix of warp totals
-        if (lane == 31) s_warp[32] = winc;  // grand total
-    }
-    __syncthreads();
-    const int res = s_warp[warp] + inc - v;
-    total = s_warp[32];
-    __syncthreads();
-    return res;
-}
-
 // key (BFS rank within a level: child rank = 2*xbit + ybit per level, most significant first) -> (ix, iy)
 __device__ __forceinline__ void deinterleave(int key, int level, int& ix, int& iy) {
     ix = 0; iy = 0;
@@ -97,10 +66,7 @@ __global__ void __launch_bounds__(TB) tree_kernel(const TreeParams p) {
     __shared__ int s_warp[33];
     __shared__ int s_flags[2];
     __shared__ unsigned long long s_sort[SORT_CAP];
-    if (g2pc_frame_skipped(p.fail, p.frame)) {  // this or an earlier frame failed: report and do nothing
-        if (threadIdx.x == 0) { p.header[G2PC_HDR_POISON] = (int32_t)*p.fail; p.header[G2PC_HDR_FRAME] = p.frame; }
-        return;
-    }
+    if (g2pc_report_skipped_frame(p.fail, p.frame, p.header)) return;  // this or an earlier frame failed
     const int L = p.meta.num_levels;
     if (threadIdx.x == 0) { s_flags[0] = 0; s_flags[1] = 0; }
     __syncthreads();
@@ -189,38 +155,13 @@ __global__ void __launch_bounds__(TB) tree_kernel(const TreeParams p) {
         pix_base += ta;
     }
     __syncthreads();
-    // launch order for the blend: heaviest leaves first (instances x pixels, ties by index) — bitonic sort in smem
-    if (nl <= SORT_CAP) {
-        int m = 1;
-        while (m < nl) m <<= 1;
-        for (int i = threadIdx.x; i < m; i += TB) {
-            unsigned long long key = ~0ull;
-            if (i < nl) {
-                unsigned long long w = (unsigned long long)p.leaves[i].inst_count *
-                                       (unsigned long long)(p.leaves[i].w * p.leaves[i].h);
-                w = w < (1ull << 44) - 1ull ? w : (1ull << 44) - 1ull;
-                key = (((1ull << 44) - 1ull - w) << 16) | (unsigned long long)i;  // ascending key = descending work
-            }
-            s_sort[i] = key;
-        }
-        __syncthreads();
-        for (int k = 2; k <= m; k <<= 1) {
-            for (int j = k >> 1; j > 0; j >>= 1) {
-                for (int i = threadIdx.x; i < m; i += TB) {
-                    const int ixj = i ^ j;
-                    if (ixj > i) {
-                        const unsigned long long a = s_sort[i], b = s_sort[ixj];
-                        const bool up = (i & k) == 0;
-                        if ((a > b) == up) { s_sort[i] = b; s_sort[ixj] = a; }
-                    }
-                }
-                __syncthreads();
-            }
-        }
-        for (int i = threadIdx.x; i < nl; i += TB) p.leaf_order[i] = (int)(s_sort[i] & 0xFFFFull);
-    } else {
-        for (int i = threadIdx.x; i < nl; i += TB) p.leaf_order[i] = i;
-    }
+    // launch order for the blend: heaviest leaves first (instances x pixels, ties by index)
+    g2pc_launch_order<TB, SORT_CAP>(s_sort, nl, [&](int i) {
+        unsigned long long w = (unsigned long long)p.leaves[i].inst_count *
+                               (unsigned long long)(p.leaves[i].w * p.leaves[i].h);
+        w = w < (1ull << 44) - 1ull ? w : (1ull << 44) - 1ull;
+        return (((1ull << 44) - 1ull - w) << 16) | (unsigned long long)i;  // ascending key = descending work
+    }, 0xFFFFull, p.leaf_order);
     // the counts are consumed: clear them for the next frame's preprocess
     for (int k = threadIdx.x; k < p.nodes_2d; k += TB) p.node_cnt[k] = 0u;
     if (threadIdx.x < G2PC_WORK_COUNTERS) p.work_counters[threadIdx.x] = 0;
@@ -229,17 +170,8 @@ __global__ void __launch_bounds__(TB) tree_kernel(const TreeParams p) {
                               (long long)p.ms_chunks * (long long)nl > p.matrix_capacity || inst_total > 0x7FFFFFFFll)
                              // (ms_chunks = rows the multisplit needs: one per chunk, g2pc_multisplit_rows)
                                  ? 1 : 0;
-        p.header[G2PC_HDR_NUM_LEAVES] = leaf_base;
-        p.header[G2PC_HDR_TOTAL_INST] = (int32_t)(inst_total & 0xFFFFFFFFll);
-        p.header[G2PC_HDR_TOTAL_INST_HI] = (int32_t)(inst_total >> 32);
-        p.header[G2PC_HDR_TOTAL_PIX] = pix_base;
-        p.header[G2PC_HDR_NEED_DEEPER] = s_flags[0];
-        p.header[G2PC_HDR_LEAF_OVERFLOW] = s_flags[1];
-        p.header[G2PC_HDR_CAP_OVERFLOW] = cap_over;
-        p.header[G2PC_HDR_FRAME] = p.frame;
-        if (s_flags[0] | s_flags[1] | cap_over) atomicMin(p.fail, (uint32_t)(p.frame + 1));
-        const uint32_t f = *(volatile uint32_t*)p.fail;
-        p.header[G2PC_HDR_POISON] = f == 0xFFFFFFFFu ? 0 : (int32_t)f;
+        g2pc_write_frame_header(p.header, p.fail, p.frame, leaf_base, inst_total, pix_base, s_flags[0], s_flags[1],
+                                cap_over);
     }
 }
 
@@ -546,6 +478,15 @@ int launch_multisplit(const MsParams& p, int32_t chunks, cudaStream_t st) {
     return G2PC_OK;
 }
 
+// the rest of g2pc_multisplit / g2pc_multisplit_grid once p is filled: sub-steps and chunks for n entries at C per sub-step
+int run_multisplit(MsParams p, int C, cudaStream_t st) {
+    p.steps = ms_steps(p.n, C);
+    const int32_t chunks = ms_chunks(p.n, C);
+    if (C == 256) return launch_multisplit<256>(p, chunks, st);
+    if (C == 128) return launch_multisplit<128>(p, chunks, st);
+    return launch_multisplit<64>(p, chunks, st);
+}
+
 }  // namespace
 
 extern "C" int g2pc_build_tree(const int32_t* tables, int32_t num_levels, int32_t max_gaussians_per_tile,
@@ -561,13 +502,12 @@ extern "C" int g2pc_build_tree(const int32_t* tables, int32_t num_levels, int32_
     p.meta.num_levels = num_levels; p.meta.max_gaussians_per_tile = max_gaussians_per_tile;
     p.meta.width = 0; p.meta.height = 0;
     p.n1 = (1 << num_levels) - 1;
-    p.tab.xs = tables; p.tab.xe = tables + p.n1; p.tab.xf = tables + 2 * p.n1;
-    p.tab.ys = tables + 3 * p.n1; p.tab.ye = tables + 4 * p.n1; p.tab.yf = tables + 5 * p.n1;
+    p.tab = make_tables(tables, p.n1);
     p.node_cnt = node_cnt; p.node_state = node_state; p.node_leaf = node_leaf; p.leaves = leaves;
     p.leaf_order = leaf_order; p.max_leaves = max_leaves;
     p.inst_capacity = inst_capacity; p.pix_capacity = pix_capacity; p.matrix_capacity = matrix_capacity;
     p.ms_chunks = ms_chunks; p.frame = frame; p.header = header; p.fail = fail; p.work_counters = work_counters;
-    p.nodes_2d = ((1 << (2 * num_levels)) - 1) / 3;
+    p.nodes_2d = off2d(num_levels);
     tree_kernel<<<1, TB, 0, (cudaStream_t)stream>>>(p);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
@@ -636,8 +576,7 @@ extern "C" int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void
     p.inv_width = 1.0f / (float)width; p.inv_height = 1.0f / (float)height;
     p.meta.num_levels = num_levels; p.meta.max_gaussians_per_tile = 0; p.meta.width = width; p.meta.height = height;
     p.n1 = (1 << num_levels) - 1;
-    p.tab.xs = tables; p.tab.xe = tables + p.n1; p.tab.xf = tables + 2 * p.n1;
-    p.tab.ys = tables + 3 * p.n1; p.tab.ye = tables + 4 * p.n1; p.tab.yf = tables + 5 * p.n1;
+    p.tab = make_tables(tables, p.n1);
     p.level_mask = level_mask; p.base_level = __builtin_ctz(level_mask);
     G2PC_CHECK_ARG(p.base_level <= G2PC_RANGE_MAX_LEVEL, "first leaf-candidate level too deep");
     p.node_leaf = node_leaf; p.header = header; p.fail = fail; p.frame = frame; p.leaves = leaves; p.matrix = matrix;
@@ -645,12 +584,7 @@ extern "C" int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void
     p.leaf_cap = leaf_cap; p.grid_w = 0;
     p.base_clean = (int32_t)((clean_mask >> p.base_level) & 1u);
     p.clean_mask = clean_mask;
-    p.steps = ms_steps(n, C);
-    const int32_t chunks = ms_chunks(n, C);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (C == 256) return launch_multisplit<256>(p, chunks, st);
-    if (C == 128) return launch_multisplit<128>(p, chunks, st);
-    return launch_multisplit<64>(p, chunks, st);
+    return run_multisplit(p, C, (cudaStream_t)stream);
 }
 
 /* The same multisplit over a flat grid of tiles (s7_tiles.cu): leaf = tile index, the packed range is the tile rect. */
@@ -664,20 +598,12 @@ extern "C" int g2pc_multisplit_grid(const uint64_t* val_sorted, int64_t n, int32
                    "bad tile grid / leaf_cap");
     const int C = g2pc_multisplit_chunk(leaf_cap);
     G2PC_CHECK_ARG(C > 0, "too many tiles for the multisplit");
-    MsParams p;
-    p.val_sorted = (const unsigned long long*)val_sorted; p.n = n; p.proj = nullptr;
-    p.width = 0; p.height = 0; p.inv_width = 0.f; p.inv_height = 0.f;
-    p.meta.num_levels = 1; p.meta.max_gaussians_per_tile = 0; p.meta.width = 0; p.meta.height = 0;
-    p.n1 = 0;
-    p.tab.xs = p.tab.xe = p.tab.xf = p.tab.ys = p.tab.ye = p.tab.yf = nullptr;
-    p.level_mask = 1u; p.base_level = 0;
-    p.node_leaf = nullptr; p.header = header; p.fail = fail; p.frame = frame; p.leaves = leaves; p.matrix = matrix;
+    MsParams p{};  // no projection records, quadtree tables or node -> leaf map: the grid is one level of tiles
+    p.val_sorted = (const unsigned long long*)val_sorted; p.n = n;
+    p.meta.num_levels = 1;
+    p.level_mask = 1u;
+    p.header = header; p.fail = fail; p.frame = frame; p.leaves = leaves; p.matrix = matrix;
     p.inst_gid = inst_gid;
     p.leaf_cap = leaf_cap; p.grid_w = grid_w; p.base_clean = 1; p.clean_mask = 1u;
-    p.steps = ms_steps(n, C);
-    const int32_t chunks = ms_chunks(n, C);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (C == 256) return launch_multisplit<256>(p, chunks, st);
-    if (C == 128) return launch_multisplit<128>(p, chunks, st);
-    return launch_multisplit<64>(p, chunks, st);
+    return run_multisplit(p, C, (cudaStream_t)stream);
 }

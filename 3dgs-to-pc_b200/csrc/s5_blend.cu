@@ -58,12 +58,6 @@ struct BlendParams {
     unsigned long long* stats;
 };
 
-__device__ __forceinline__ float ex2f(float x) {
-    float r;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));  // results below FLT_MIN flush to 0 (see header comment)
-    return r;
-}
-
 // per-lane FP32 on a pixel pair with a scalar operand; the _rn intrinsics keep every op rounded on its own (no FMA
 // contraction), which fixes the results bit for bit
 __device__ __forceinline__ float2 add2(float2 a, float b) { return make_float2(__fadd_rn(a.x, b), __fadd_rn(a.y, b)); }
@@ -75,38 +69,9 @@ __device__ __forceinline__ float2 fma2(float2 a, float2 b, float c) {
     return make_float2(__fmaf_rn(a.x, b.x, c), __fmaf_rn(a.y, b.y, c));
 }
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// one elected thread: arm the barrier with the byte count, then start the 1-D bulk copy global -> shared (TMA engine)
-__device__ __forceinline__ void tma_load_1d(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // earlier generic-proxy reads of dst are ordered before
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
-}
 __device__ __forceinline__ void cp_async4(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
     __shared__ __align__(16) float4 s_q0[2][CH];
@@ -120,10 +85,7 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
     if (g2pc_frame_skipped(p.fail, p.frame)) return;
     const int num_items = p.header[G2PC_HDR_NUM_LEAVES] * p.slabs;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) {
-        mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_init(&s_bar[2], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (tid == 0) id_ring_init(s_bar);
     for (int w = 0; w < BT / 32; ++w) s_best[w][tid] = 0ull;
     uint32_t phase_bits = 0;  // parity of the next completion of each id barrier (bit s)
     const float t_stop = p.t_stop;
@@ -133,10 +95,7 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
     // persistent CTAs: work items (leaf, slab) are handed out heaviest-leaf-first from a global counter, so the tail of
     // the launch is at most one item long
   for (;;) {
-    if (tid == 0) s_item = atomicAdd(p.work_counter, 1);
-    __syncthreads();
-    const int item = s_item;
-    __syncthreads();
+    const int item = next_work_item(p.work_counter, &s_item);
     if (item >= num_items) break;
     const g2pc_leaf_t lf = p.leaves[p.leaf_order[item / p.slabs]];
     const int qpr = (lf.w + 3) >> 2;
@@ -190,16 +149,6 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
     const uint32_t* list = p.inst_gid + (int64_t)lf.inst_begin;  // 16-byte aligned (tree kernel)
 
     // ---- pipeline helpers ------------------------------------------------------------------------------------------
-    auto issue_ids = [&](int c) {  // thread 0 only
-        const int nl = min(CH, cnt - c * CH);
-        const uint32_t bytes = (uint32_t)(((nl + 3) & ~3) * 4);  // whole 16-byte units (the lists are padded)
-        tma_load_1d(&s_gid[c % 3][0], list + (int64_t)c * CH, bytes, &s_bar[c % 3]);
-    };
-    auto wait_ids = [&](int c) {
-        const int s = c % 3;
-        mbar_wait(&s_bar[s], (phase_bits >> s) & 1u);
-        phase_bits ^= 1u << s;
-    };
     auto issue_records = [&](int c) {
         const int nl = min(CH, cnt - c * CH);
         if (tid < nl) {
@@ -215,14 +164,17 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
 
     bool warp_done = false;
     if (nchunks > 0) {
-        if (tid == 0) { issue_ids(0); if (nchunks > 1) issue_ids(1); }
-        wait_ids(0);
+        if (tid == 0) {
+            id_ring_issue(s_gid, s_bar, list, cnt, 0);
+            if (nchunks > 1) id_ring_issue(s_gid, s_bar, list, cnt, 1);
+        }
+        id_ring_wait(s_bar, phase_bits, 0);
         issue_records(0);
     }
     for (int c = 0; c < nchunks; ++c) {
         const int nload = min(CH, cnt - c * CH);
         const bool more = (c + 1 < nchunks);
-        if (more) { wait_ids(c + 1); issue_records(c + 1); }
+        if (more) { id_ring_wait(s_bar, phase_bits, c + 1); issue_records(c + 1); }
         if (more) cp_async_wait<1>(); else cp_async_wait<0>();
         // records of chunk c visible to the CTA; every thread is past the merge of chunk c - 1 (its id buffer is free)
         const bool all_done = __syncthreads_and(warp_done ? 1 : 0);
@@ -230,7 +182,7 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
             if (more) cp_async_wait<0>();  // drain the gather in flight before the buffers are reused by the next item
             break;
         }
-        if (tid == 0 && c + 2 < nchunks) issue_ids(c + 2);
+        if (tid == 0 && c + 2 < nchunks) id_ring_issue(s_gid, s_bar, list, cnt, c + 2);
         const float4* q0s = s_q0[c & 1];
         const float4* q1s = s_q1[c & 1];
         const float2* bs = s_b[c & 1];
@@ -250,8 +202,8 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
                     const float2 dx23 = add2(px23, nmx);
                     const float2 e01 = fma2(dx01, fma2(dx01, q0.z, make_float2(Bq, Bq)), Cq);
                     const float2 e23 = fma2(dx23, fma2(dx23, q0.z, make_float2(Bq, Bq)), Cq);
-                    const float2 a01 = make_float2(fminf(0.99f, ex2f(e01.x)), fminf(0.99f, ex2f(e01.y)));
-                    const float2 a23 = make_float2(fminf(0.99f, ex2f(e23.x)), fminf(0.99f, ex2f(e23.y)));
+                    const float2 a01 = make_float2(fminf(0.99f, ex2_approx(e01.x)), fminf(0.99f, ex2_approx(e01.y)));
+                    const float2 a23 = make_float2(fminf(0.99f, ex2_approx(e23.x)), fminf(0.99f, ex2_approx(e23.y)));
                     const float2 c01 = mul2(T01, a01);
                     const float2 c23 = mul2(T23, a23);
                     Cr01 = fma2(c01, q1.z, Cr01);
@@ -389,16 +341,7 @@ extern "C" int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, 
     p.slabs = p.compact ? (max_leaf_pixels_quads + 4 * 25 - 1) / (4 * 25) + 1 : (max_leaf_pixels_quads + BT - 1) / BT;
     p.work_counter = work_counters;
     p.stats = (unsigned long long*)stats;
-    static int resident = 0;  // persistent grid: every SM filled to the kernel's occupancy (device constant)
-    if (resident == 0) {
-        int dev = 0, sms = 132, per_sm = 8;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, blend_kernel, BT, 0) != cudaSuccess || per_sm < 1)
-            per_sm = 8;
-        resident = sms * per_sm;
-    }
-    blend_kernel<<<(unsigned)resident, BT, 0, (cudaStream_t)stream>>>(p);
+    blend_kernel<<<(unsigned)g2pc_resident_ctas(blend_kernel, BT, 0, 8), BT, 0, (cudaStream_t)stream>>>(p);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }

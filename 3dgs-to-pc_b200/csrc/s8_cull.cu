@@ -73,30 +73,10 @@ __global__ void __launch_bounds__(1024) cull_scan_kernel(int32_t* __restrict__ b
     long long run = 0;
     for (int b0 = 0; b0 < nblocks; b0 += 1024) {
         const int b = b0 + threadIdx.x;
-        const int v = b < nblocks ? block_cnt[b] : 0;
-        int inc = v;
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) s_w[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            int w = s_w[lane], winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, winc, o);
-                if (lane >= o) winc += t;
-            }
-            s_w[lane] = winc - w;
-            if (lane == 31) s_w[32] = winc;
-        }
-        __syncthreads();
-        if (b < nblocks) block_cnt[b] = (int32_t)(run + s_w[warp] + inc - v);
-        run += s_w[32];
-        __syncthreads();
+        int total;
+        const int pre = block_scan_1024(b < nblocks ? block_cnt[b] : 0, s_w, total);
+        if (b < nblocks) block_cnt[b] = (int32_t)(run + pre);
+        run += total;
     }
     if (threadIdx.x == 0) count[0] = run;
 }

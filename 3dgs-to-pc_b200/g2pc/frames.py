@@ -22,11 +22,17 @@ from . import capi, config
 _HDR_POOLS = {}  # device -> free pinned frame headers (cudaHostAlloc is slow: never once per renderer)
 
 
+def total_instances(h):
+    """(Gaussian, tile) instances of a frame, from its header."""
+    return h[capi.HDR_TOTAL_INST] + (h[capi.HDR_TOTAL_INST_HI] << 32)
+
+
 class FrameQueue:
-    """Mixin.  The owner provides: self.device, self._ensure_buffers(camera, slot) (allocate / grow the slot's scratch on
-    the current stream), self._enqueue_front(camera, frame, slot) -> device header tensor,
-    self._enqueue_back(camera, frame, camera_index, slot), self._fix(header_list), self._confirm(header_list) and
-    self._reset_counts() (zero the per-slot tile counters after a failure)."""
+    """Mixin.  The owner sets self.device, self.lib and self._n (Gaussians), calls _init_frames() and provides:
+    self._ensure_buffers(camera, slot) (allocate / grow the slot's scratch on the current stream, the lists through
+    _grow_lists), self._enqueue_front(camera, frame, slot) -> device header tensor,
+    self._enqueue_back(camera, frame, camera_index, slot), self._fix(header_list) and self._confirm(header_list).
+    Per-resolution table sets go in self._tables; each holds per-slot tile counters t["slots"][slot]["node_cnt"]."""
 
     def _init_frames(self):
         self._frame = 0
@@ -38,6 +44,63 @@ class FrameQueue:
         self._streams = [torch.cuda.Stream(device=self.device) for _ in range(self.num_slots)]
         self._fail = torch.full((1,), -1, dtype=torch.int32, device=self.device)  # 0xFFFFFFFF: no frame has failed
         self._prev_done = None
+        # per-frame scratch: one set per slot (frames alternate between the slots); the lists and the multisplit matrix
+        # are sized per resolution (_grow_lists)
+        dev, m = self.device, max(self._n, 1)
+        nbytes = int(self.lib.g2pc_depth_sort_workspace_bytes(m))
+        self._slots = [dict(proj=torch.empty((m, 12), dtype=torch.float32, device=dev),
+                            depth_key=torch.empty((m,), dtype=torch.int32, device=dev),
+                            val=torch.empty((m,), dtype=torch.int64, device=dev),
+                            val_sorted=torch.empty((m,), dtype=torch.int64, device=dev),
+                            depth_ws=torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev),
+                            hdr=torch.zeros((capi.HDR_WORDS,), dtype=torch.int32, device=dev),
+                            work=torch.zeros((capi.WORK_COUNTERS,), dtype=torch.int32, device=dev),
+                            inst_gid=None, matrix=None) for _ in range(self.num_slots)]
+        self._cam_best = torch.zeros((m,), dtype=torch.int64, device=dev)
+        self._stats = torch.zeros((capi.STAT_WORDS,), dtype=torch.int64, device=dev)
+        # (Gaussian, tile) instances the lists hold, grown when a frame does not fit
+        self._inst_cap = max(8 * self._n, 1 << 16)
+        self._tables = {}
+        self._last_slot = 0
+        self.last_stats = {}
+
+    def _grow_lists(self, sl, leaf_cap, rows):
+        """Grow the slot's depth-ordered lists and multisplit matrix (rows x leaf_cap) to the current capacities."""
+        need = self._inst_cap + 4 * leaf_cap + 64  # lists are padded to 16 bytes; slack for the last TMA unit
+        if sl["inst_gid"] is None or sl["inst_gid"].numel() < need:
+            sl["inst_gid"] = torch.empty((need,), dtype=torch.int32, device=self.device)
+        mneed = rows * leaf_cap
+        if sl["matrix"] is None or sl["matrix"].numel() < mneed:
+            sl["matrix"] = torch.empty((max(mneed, 1),), dtype=torch.int32, device=self.device)
+
+    def _depth_sort(self, sl, stream):
+        """Enqueue the depth sort of the (depth key, value) pairs the slot's preprocess wrote."""
+        capi.call("g2pc_depth_sort", capi.ptr(sl["depth_key"]), capi.ptr(sl["val"]), self._n, capi.ptr(sl["val_sorted"]),
+                  capi.ptr(sl["depth_ws"]), sl["depth_ws"].numel(), stream)
+
+    def _grow_inst_cap(self, h):
+        """A frame's (Gaussian, tile) instances did not fit the lists: raise their capacity (the next _launch grows the
+        buffers)."""
+        total = total_instances(h)
+        if total > 0x7FFFFFFF:
+            raise capi.G2pcError(f"{total} (Gaussian, tile) instances in one camera: more than 2^31 - 1")
+        self._inst_cap = max(self._inst_cap, int(1.25 * total) + 1024)
+
+    def _reset_counts(self):
+        """Zero the per-slot tile counters of every table set (a failed frame left its counts behind)."""
+        for t in self._tables.values():
+            for ts in t["slots"]:
+                ts["node_cnt"].zero_()
+
+    def executed_pairs(self):
+        """(pixel, Gaussian) pairs the blend evaluated since construction: the device counts warp iterations, and a warp
+        blends 32 x 4 pixels."""
+        self.flush()
+        return int(self._stats[capi.STAT_WARP_GAUSSIANS].item()) * 128
+
+    def get_gaussian_colours(self):
+        self.flush()
+        return self.gaussian_colours * 255
 
     def _launch(self, frame, camera, camera_index):
         slot = frame % self.num_slots

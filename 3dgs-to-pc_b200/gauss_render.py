@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from g2pc import capi, config, quadtree
-from g2pc.frames import FrameQueue
+from g2pc.frames import FrameQueue, total_instances
 
 # SH constants kept for API parity with the reference module (gauss_render.py:9-38)
 C0 = 0.28209479177387814
@@ -81,7 +81,6 @@ class GaussPythonRenderer(FrameQueue):
         self.compose_image = True
         self.async_mode = False
         self.first_frame = None  # optional (n) int32: index of the camera that raised each maximum (g2pc/dist.py)
-        self._tables = {}
         self._extra_levels = 0
         self._n = n
         st = capi.stream_ptr(dev)
@@ -90,29 +89,9 @@ class GaussPythonRenderer(FrameQueue):
         capi.call("g2pc_pack_geometry", capi.ptr(self.means3D), capi.ptr(self.cov3d), capi.ptr(self.opacity), n,
                   capi.ptr(self._geom), st)
         self._init_frames()
-        # per-frame scratch: one set per slot (frames alternate between the slots)
-        m = max(n, 1)
-        nbytes = self.lib.g2pc_depth_sort_workspace_bytes(m)
-        self._slots = [dict(proj=torch.empty((m, 12), dtype=torch.float32, device=dev),
-                            depth_key=torch.empty((m,), dtype=torch.int32, device=dev),
-                            val=torch.empty((m,), dtype=torch.int64, device=dev),
-                            val_sorted=torch.empty((m,), dtype=torch.int64, device=dev),
-                            depth_ws=torch.empty((max(int(nbytes), 1),), dtype=torch.uint8, device=dev),
-                            hdr=torch.zeros((capi.HDR_WORDS,), dtype=torch.int32, device=dev),
-                            work=torch.zeros((capi.WORK_COUNTERS,), dtype=torch.int32, device=dev),
-                            inst_gid=None, matrix=None) for _ in range(self.num_slots)]
-        self._cam_best = torch.zeros((m,), dtype=torch.int64, device=dev)
-        self._stats = torch.zeros((capi.STAT_WORDS,), dtype=torch.int64, device=dev)
         self._leaf_colour = None
-        self._inst_cap = max(8 * n, 1 << 16)
-        self._last_slot = 0
-        self.last_stats = {}
 
-    # ---- getters (gauss_render.py:237-264) -----------------------------------------------------------------
-    def get_gaussian_colours(self):
-        self.flush()
-        return self.gaussian_colours * 255
-
+    # ---- getters (gauss_render.py:237-264; get_gaussian_colours in FrameQueue) -------------------------------------
     def get_gaussians_above_contribution_threshold(self, contribution_threshold):
         self.flush()
         return self.gaussian_max_contribution > contribution_threshold
@@ -128,11 +107,6 @@ class GaussPythonRenderer(FrameQueue):
         # the python back-end of the reference reports the MAX contribution here (gauss_render.py:261-264)
         self.flush()
         return self.gaussian_max_contribution
-
-    def executed_pairs(self):
-        """(pixel, Gaussian) pairs the blend kernel evaluated since construction (device counter)."""
-        self.flush()
-        return int(self._stats[capi.STAT_WARP_GAUSSIANS].item()) * 128
 
     # ---- per-resolution tables ---------------------------------------------------------------------------------
     def _get_tables(self, W, H):
@@ -199,21 +173,12 @@ class GaussPythonRenderer(FrameQueue):
         c.height = camera.image_height
         return c
 
-    def _buffers(self, t, sl):
-        """(Re)allocate the slot's frame buffers for the current capacities."""
-        dev = self.device
-        need = self._inst_cap + 4 * t["leaf_cap"] + 64  # lists are padded to 16 bytes; slack for the last TMA unit
-        if sl["inst_gid"] is None or sl["inst_gid"].numel() < need:
-            sl["inst_gid"] = torch.empty((need,), dtype=torch.int32, device=dev)
-        if self._leaf_colour is None or self._leaf_colour.numel() < 3 * t["pix_cap"]:
-            self._leaf_colour = torch.empty((3 * t["pix_cap"],), dtype=torch.float32, device=dev)
-        mneed = t["chunks"] * t["leaf_cap"]
-        if sl["matrix"] is None or sl["matrix"].numel() < mneed:
-            sl["matrix"] = torch.empty((max(mneed, 1),), dtype=torch.int32, device=dev)
-
     def _ensure_buffers(self, camera, slot):
+        """(Re)allocate the slot's frame buffers for the current capacities."""
         t = self._get_tables(int(camera.image_width), int(camera.image_height))
-        self._buffers(t, self._slots[slot])
+        self._grow_lists(self._slots[slot], t["leaf_cap"], t["chunks"])
+        if self._leaf_colour is None or self._leaf_colour.numel() < 3 * t["pix_cap"]:
+            self._leaf_colour = torch.empty((3 * t["pix_cap"],), dtype=torch.float32, device=self.device)
 
     def _enqueue_front(self, camera, frame, slot):
         """Projection, depth sort, tile table and per-tile lists of one camera, asynchronously on the current stream."""
@@ -229,8 +194,7 @@ class GaussPythonRenderer(FrameQueue):
                   ctypes.byref(cam), capi.ptr(t["tables"]), capi.ptr(t["luts"]), qt.num_levels, t["level_mask"],
                   t["clean_mask"], capi.ptr(sl["proj"]),
                   capi.ptr(ts["node_cnt"]), capi.ptr(sl["depth_key"]), capi.ptr(sl["val"]), st)
-        capi.call("g2pc_depth_sort", capi.ptr(sl["depth_key"]), capi.ptr(sl["val"]), n, capi.ptr(sl["val_sorted"]),
-                  capi.ptr(sl["depth_ws"]), sl["depth_ws"].numel(), st)
+        self._depth_sort(sl, st)
         capi.call("g2pc_build_tree", capi.ptr(t["tables"]), qt.num_levels, qt.max_gaussians_per_tile,
                   capi.ptr(ts["node_cnt"]), capi.ptr(ts["node_state"]), capi.ptr(ts["node_leaf"]), capi.ptr(ts["leaves"]),
                   capi.ptr(ts["leaf_order"]), t["leaf_cap"], self._inst_cap, t["pix_cap"], sl["matrix"].numel(),
@@ -278,7 +242,7 @@ class GaussPythonRenderer(FrameQueue):
     def _confirm(self, h):
         t = self._last_tables
         self.last_stats = dict(num_leaves=h[capi.HDR_NUM_LEAVES],
-                               total_instances=h[capi.HDR_TOTAL_INST] + (h[capi.HDR_TOTAL_INST_HI] << 32),
+                               total_instances=total_instances(h),
                                total_leaf_pixels=h[capi.HDR_TOTAL_PIX], levels=t["qt"].num_levels, frame=h[capi.HDR_FRAME])
 
     def _fix(self, h):
@@ -299,18 +263,10 @@ class GaussPythonRenderer(FrameQueue):
                 raise capi.G2pcError("leaf table overflow")
             self._set_leaf_cap(t, max(2 * t["leaf_cap"], int(1.25 * h[capi.HDR_NUM_LEAVES])))
         elif h[capi.HDR_CAP_OVERFLOW]:
-            total = h[capi.HDR_TOTAL_INST] + (h[capi.HDR_TOTAL_INST_HI] << 32)
-            if total > 0x7FFFFFFF:
-                raise capi.G2pcError(f"{total} (Gaussian, tile) instances in one camera: more than 2^31 - 1")
-            self._inst_cap = max(self._inst_cap, int(1.25 * total) + 1024)
+            self._grow_inst_cap(h)
             t["pix_cap"] = max(t["pix_cap"], int(1.25 * h[capi.HDR_TOTAL_PIX]) + 1024)
         else:
             raise capi.G2pcError("poisoned frame header without a cause")
-
-    def _reset_counts(self):
-        for tt in self._tables.values():
-            for ts in tt["slots"]:
-                ts["node_cnt"].zero_()
 
     # ---- introspection for the parity tests ---------------------------------------------------------------------
     def debug_last_camera(self):

@@ -11,7 +11,8 @@
  *   - every pointer is a DEVICE pointer unless the name ends in `_host`; the caller owns all memory,
  *     including scratch (sizes come from the *_bytes query functions or are stated in the comment);
  *   - every call is asynchronous on `stream` (a cudaStream_t passed as void*); no allocation, no host
- *     synchronisation and no global mutable state inside the library;
+ *     synchronisation and no global mutable state inside the library, except the blend footprint switch
+ *     set by g2pc_blend_set_compact;
  *   - return value: 0 = G2PC_OK, otherwise an error code; g2pc_last_error() gives a thread-local message;
  *   - no C++ exception crosses the ABI.
  */
