@@ -317,14 +317,14 @@ static int g_blend_compact = 1;
 extern "C" void g2pc_blend_set_compact(int on) { g_blend_compact = on ? 1 : 0; }
 
 extern "C" int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header,
-                          const uint32_t* fail, int32_t frame, int32_t max_leaf_pixels_quads, const uint32_t* inst_gid,
-                          const void* proj,
+                          const uint32_t* fail, int32_t frame, int32_t max_leaf_width, int32_t max_leaf_height,
+                          const uint32_t* inst_gid, const void* proj,
                           uint64_t* cam_best, const float* max_contrib, float* leaf_colour, uint32_t* owner,
                           int32_t width, int32_t height, float background, float t_stop, int32_t* work_counters,
                           uint64_t* stats, void* stream) {
     G2PC_CHECK_ARG(leaves && leaf_order && header && fail && inst_gid && proj && cam_best && max_contrib && leaf_colour &&
                        owner && work_counters, "null pointer");
-    G2PC_CHECK_ARG(max_leaf_pixels_quads >= 1, "max_leaf_pixels_quads < 1");
+    G2PC_CHECK_ARG(max_leaf_width >= 1 && max_leaf_height >= 1, "max_leaf_width / max_leaf_height < 1");
     G2PC_CHECK_ARG(t_stop >= 0.0f && t_stop < 1.0f, "t_stop must be in [0, 1)");
     G2PC_CHECK_ARG(((uintptr_t)inst_gid & 15) == 0, "inst_gid must be 16-byte aligned (TMA bulk copies)");
     BlendParams p;
@@ -336,9 +336,17 @@ extern "C" int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, 
     p.W = width; p.H = height; p.bg = background;
     p.t_stop = t_stop > 1.17549435e-38f ? t_stop : 1.17549435e-38f;
     p.compact = g_blend_compact;
-    // slabs: CTAs per leaf.  Row strips: ceil(quads / 128).  Blocks: a leaf of max_tile_size has at most
-    // ceil(qpr / 5) x ceil(h / 6) blocks of <= 32 quads; the caller's bound is quads = ceil(w / 4) * h <= 15 * h.
-    p.slabs = p.compact ? (max_leaf_pixels_quads + 4 * 25 - 1) / (4 * 25) + 1 : (max_leaf_pixels_quads + BT - 1) / BT;
+    // slabs: work items (CTA-sized parts) per leaf.  Row strips: ceil(quads / 128), quads = ceil(max_w / 4) * max_h.
+    // Blocks: 4 per item.  A leaf within max_w x max_h has at most ceil(ceil(max_w / 4) / 5) blocks across (the count
+    // grows with the width) and at most ceil(max_h / 6) down (a block has >= 6 rows).  ceil(quads / 100) + 1 items are
+    // enough for leaves up to 160 px wide and are kept there (C3: 10 items for 60 x 60 leaves); wider, shorter leaves
+    // get the count their blocks need.
+    const int64_t qpr = (max_leaf_width + 3) / 4, quads = qpr * max_leaf_height;
+    const int64_t blocks = (qpr + 4) / 5 * (((int64_t)max_leaf_height + 5) / 6);
+    const int64_t kept = (quads + 4 * 25 - 1) / (4 * 25) + 1, need = (blocks + 3) / 4;
+    const int64_t slabs = p.compact ? (need > kept ? need : kept) : (quads + BT - 1) / BT;
+    G2PC_CHECK_ARG(slabs <= 0x7FFFFFFF, "max_leaf_width x max_leaf_height too large");
+    p.slabs = (int32_t)slabs;
     p.work_counter = work_counters;
     p.stats = (unsigned long long*)stats;
     blend_kernel<<<(unsigned)g2pc_resident_ctas(blend_kernel, BT, 0, 8), BT, 0, (cudaStream_t)stream>>>(p);

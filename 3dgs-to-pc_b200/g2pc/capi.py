@@ -52,8 +52,9 @@ SIGNATURES = {
     "g2pc_multisplit_rows": ([_i64, _i32], ctypes.c_int32),
     "g2pc_multisplit": ([_c_void_p, _i64, _c_void_p, _i32, _i32, _c_void_p, _i32, _u32, _u32, _c_void_p, _c_void_p,
                          _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
-    "g2pc_blend": ([_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
-                    _c_void_p, _c_void_p, _i32, _i32, _f32, _f32, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
+    "g2pc_blend": ([_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i32, _c_void_p, _c_void_p, _c_void_p,
+                    _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _f32, _f32, _c_void_p, _c_void_p, _c_void_p],
+                   ctypes.c_int),
     "g2pc_blend_set_compact": ([ctypes.c_int], None),
     "g2pc_accumulate": ([_c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i32, _c_void_p], ctypes.c_int),
     "g2pc_tiles_preprocess": ([_c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i32, _i64, _c_void_p, _c_void_p, _c_void_p,

@@ -134,7 +134,7 @@ class GaussPythonRenderer(FrameQueue):
                      owner=torch.zeros((W * H,), dtype=torch.int32, device=dev),
                      image=torch.ones((H, W, 3), dtype=torch.float32, device=dev),
                      leaf_cap=0, pix_cap=int(1.25 * W * H) + 4096,
-                     max_quads=int(((min(self.max_tile_size, W) + 3) // 4) * min(self.max_tile_size, H)))
+                     max_leaf=(int(min(self.max_tile_size, W)), int(min(self.max_tile_size, H))))
             self._set_leaf_cap(t, min(qt.nodes_2d, 2 * (4 ** base)))
             self._tables[key] = t
         return t
@@ -215,7 +215,7 @@ class GaussPythonRenderer(FrameQueue):
         sl, ts = self._slots[slot], t["slots"][slot]
         bg = 1.0 if self.white_bkgd else 0.0
         capi.call("g2pc_blend", capi.ptr(ts["leaves"]), capi.ptr(ts["leaf_order"]), capi.ptr(sl["hdr"]),
-                  capi.ptr(self._fail), frame, t["max_quads"], capi.ptr(sl["inst_gid"]), capi.ptr(sl["proj"]),
+                  capi.ptr(self._fail), frame, *t["max_leaf"], capi.ptr(sl["inst_gid"]), capi.ptr(sl["proj"]),
                   capi.ptr(self._cam_best), capi.ptr(self.gaussian_max_contribution), capi.ptr(self._leaf_colour),
                   capi.ptr(t["owner"]), W, H, bg, float(self.t_stop), capi.ptr(sl["work"]), capi.ptr(self._stats), st)
         capi.call("g2pc_accumulate", capi.ptr(self._cam_best), capi.ptr(self._leaf_colour), n,

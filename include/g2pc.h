@@ -258,7 +258,8 @@ int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void* proj, int
 
 /* S5.  Front-to-back blend of every leaf (gauss_render.py:337-369) + per-Gaussian maximum contribution / arg-max pixel
  * (:371-385) published as cam_best[g] = max((bits(contribution) << 32) | ~leaf_pixel_index).
- * The leaf count comes from `header` (device).  max_leaf_pixels_quads: upper bound of ceil(w/4)*h over the leaves.
+ * The leaf count comes from `header` (device).  max_leaf_width / max_leaf_height: upper bounds of the leaves' w and h
+ * (every leaf fits in max_leaf_width x max_leaf_height); they size the split of a leaf into work items.
  * max_contrib (n) f32: the running maxima of the earlier cameras (read-only here; contributions that cannot beat
  * them skip the bookkeeping).  leaf_colour: (pix_capacity,3) f32.  owner: uint32 per image pixel (zero on entry):
  * 1 + index of the last leaf pixel covering it.  work_counters: cleared by g2pc_build_tree (persistent CTAs pull
@@ -268,7 +269,8 @@ int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void* proj, int
  * contributions that underflow are dropped: the strict-parity setting); the reference's CUDA back-end stops each pixel
  * at T < 1e-4 (forward.cu:415).  stats: G2PC_STAT_WORDS uint64 or NULL. */
 int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header, const uint32_t* fail,
-               int32_t frame, int32_t max_leaf_pixels_quads, const uint32_t* inst_gid, const void* proj, uint64_t* cam_best,
+               int32_t frame, int32_t max_leaf_width, int32_t max_leaf_height, const uint32_t* inst_gid, const void* proj,
+               uint64_t* cam_best,
                const float* max_contrib, float* leaf_colour, uint32_t* owner, int32_t width, int32_t height,
                float background, float t_stop, int32_t* work_counters, uint64_t* stats, void* stream);
 

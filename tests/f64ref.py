@@ -253,11 +253,12 @@ def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True):
                 **counts)
 
 
-def leaf_blend(r0, c0, w, h, ids, proj):
+def leaf_blend(r0, c0, w, h, ids, proj, bg=1.0, transmittance=False):
     """gauss_render.py:337-369 for one quadtree leaf in f64, fed the kernel's records (python back-end layout:
     {mx, my, K c00, K (c01 + c10)} {K c11, log2 o, r, g} {b, depth, radius, valid}) and its depth-ordered list `ids`:
-    alpha = min(0.99, o exp(power)), contribution T alpha, T *= 1 - alpha, white background.  Returns (colour
-    (h*w, 3), contribution (h*w, len(ids))) with pixels row-major over the leaf."""
+    alpha = min(0.99, o exp(power)), contribution T alpha, T *= 1 - alpha, background `bg` (white by default).
+    Returns (colour (h*w, 3), contribution (h*w, len(ids))) with pixels row-major over the leaf, and the final
+    transmittance (h*w,) as a third value when `transmittance` is set."""
     ys, xs = np.meshgrid(np.arange(r0, r0 + h), np.arange(c0, c0 + w), indexing="ij")
     px, py = xs.reshape(-1).astype(np.float64), ys.reshape(-1).astype(np.float64)
     P = proj[ids].astype(np.float64)
@@ -272,4 +273,6 @@ def leaf_blend(r0, c0, w, h, ids, proj):
         contrib[:, j] = c
         col += c[:, None] * P[j, 6:9][None, :]
         T = T * (1.0 - alpha)
-    return col + T[:, None], contrib
+    if transmittance:
+        return col + bg * T[:, None], contrib, T
+    return col + bg * T[:, None], contrib
