@@ -1,0 +1,433 @@
+// s9_clean.cu — statistical outlier removal of the finished point cloud (--clean_pointcloud): exact k-nearest-neighbour
+// mean distances and the keep mask.
+//
+// Reference semantics restated (not copied):
+//   gauss_to_pc.py:743-759   the clean runs once on the whole cloud after generation
+//   mesh_handler.py:89-94    clean_point_cloud -> Open3D PointCloud::RemoveStatisticalOutliers(nb_neighbors=20, std_ratio)
+// avg[i] = (sum of sqrt(d2) over the k smallest d2 of point i, self included, ascending) / min(k, n), d2 in float64 as
+// (dx*dx + dy*dy) + dz*dz of the upcast float32 coordinates; keep[i] = avg[i] > 0 && avg[i] < mean + std_ratio * std.
+//
+// Index: an implicit linear octree.  Every point gets a 126-bit Morton key: 42 bits per axis over a cube of power-of-two
+// edge E that holds the bounding box, split into two 63-bit words (hi = the top 21 bits of each axis, lo = the low 21).
+// Two stable cub radix sorts (lo first, then hi) order the points by the full key, so every octree cell at every level
+// 0..42 is one contiguous range of the sorted array.  Exact duplicates share their key and sit next to each other.
+//
+// Query (one thread per sorted point, so a warp holds 32 spatial neighbours): the WIN = 2*K_MAX sorted neighbours around
+// the query are scanned first, which gives a tight k-th distance at once and answers a query with >= k exact copies
+// (k-th distance 0) without any further work.  Then a stackless walk of the octree in Morton order: a cell whose box is
+// not nearer than the current k-th distance is skipped without touching memory; otherwise its range is found by
+// galloping search from the previous position, and it is scanned if it holds <= LEAF_T points (or is a 42-bit cell),
+// else entered.  The k smallest d2 live in registers; indices are not needed (only the multiset of distances matters).
+// Box distances are lowered by a margin of E * 2^-48, which covers the rounding of the quantisation and of the distance
+// arithmetic, so a cell is skipped only when no point in it can enter the list: the result is exact.
+#include <cub/cub.cuh>
+#include "common.cuh"
+
+namespace {
+
+typedef unsigned __int128 u128;
+
+constexpr int K_MAX = G2PC_SOR_K_MAX;
+constexpr int WIN = 2 * K_MAX;     // a run of >= k exact copies through the query always lies K_MAX deep in the window
+constexpr int LEAF_T = 32;         // a cell with at most this many points is scanned, a larger one is entered
+constexpr int QBITS = 42;          // quantisation bits per axis (deepest octree level)
+constexpr int QB = 128;            // query threads per CTA
+constexpr int BB = 256;            // bounding-box / key / gather threads per CTA
+constexpr int BOX_PER_CTA = BB * 8;
+constexpr uint64_t MASK21 = (1ull << 21) - 1;
+constexpr uint64_t KEY_NONFINITE = (1ull << 63) - 1;  // non-finite points sort last and are nobody's neighbour
+
+struct Frame {
+    double lo[3];   // bounding-box minimum (finite points)
+    double scale;   // 2^42 / E
+    double edge;    // E: power of two >= the largest bounding-box extent
+    double margin;  // E * 2^-48
+};
+
+__host__ __device__ __forceinline__ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+__device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
+
+// 21-bit integer -> every third bit of 63
+__device__ __forceinline__ uint64_t spread3(uint64_t v) {
+    v &= MASK21;
+    v = (v | v << 32) & 0x001f00000000ffffull;
+    v = (v | v << 16) & 0x001f0000ff0000ffull;
+    v = (v | v << 8) & 0x100f00f00f00f00full;
+    v = (v | v << 4) & 0x10c30c30c30c30c3ull;
+    v = (v | v << 2) & 0x1249249249249249ull;
+    return v;
+}
+
+__device__ __forceinline__ uint64_t morton63(uint64_t x, uint64_t y, uint64_t z) {
+    return spread3(x) << 2 | spread3(y) << 1 | spread3(z);
+}
+
+// 126-bit key of the 42-bit cell coordinates (x, y, z)
+__device__ __forceinline__ u128 key126(uint64_t x, uint64_t y, uint64_t z) {
+    return (u128)morton63(x >> 21, y >> 21, z >> 21) << 63 | morton63(x & MASK21, y & MASK21, z & MASK21);
+}
+
+// per-CTA min / max of the finite coordinates: part[6 * b ..] = (min x, min y, min z, max x, max y, max z)
+__global__ void __launch_bounds__(BB) bbox_kernel(const float* __restrict__ xyz, int64_t n, float* __restrict__ part) {
+    __shared__ float s[6][BB / 32];
+    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+    const int64_t base = (int64_t)blockIdx.x * BOX_PER_CTA;
+    for (int r = 0; r < BOX_PER_CTA / BB; ++r) {
+        const int64_t i = base + r * BB + threadIdx.x;
+        if (i >= n) break;
+        const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
+        if (!finite3(x, y, z)) continue;
+        mn[0] = fminf(mn[0], x); mn[1] = fminf(mn[1], y); mn[2] = fminf(mn[2], z);
+        mx[0] = fmaxf(mx[0], x); mx[1] = fmaxf(mx[1], y); mx[2] = fmaxf(mx[2], z);
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
+            mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
+        }
+    }
+    if ((threadIdx.x & 31) == 0) {
+        for (int a = 0; a < 3; ++a) { s[a][threadIdx.x >> 5] = mn[a]; s[3 + a][threadIdx.x >> 5] = mx[a]; }
+    }
+    __syncthreads();
+    if (threadIdx.x < 6) {
+        float v = s[threadIdx.x][0];
+        for (int w = 1; w < BB / 32; ++w) v = threadIdx.x < 3 ? fminf(v, s[threadIdx.x][w]) : fmaxf(v, s[threadIdx.x][w]);
+        part[6 * blockIdx.x + threadIdx.x] = v;
+    }
+}
+
+// one thread: fold the per-CTA boxes into the quantisation frame
+__global__ void frame_kernel(const float* __restrict__ part, int nb, Frame* __restrict__ fr) {
+    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+    for (int b = 0; b < nb; ++b)
+        for (int a = 0; a < 3; ++a) { mn[a] = fminf(mn[a], part[6 * b + a]); mx[a] = fmaxf(mx[a], part[6 * b + 3 + a]); }
+    Frame f;
+    double ext = 0.0;
+    if (mn[0] <= mx[0]) {
+        for (int a = 0; a < 3; ++a) { f.lo[a] = mn[a]; ext = fmax(ext, (double)mx[a] - (double)mn[a]); }
+    } else {  // no finite point
+        f.lo[0] = f.lo[1] = f.lo[2] = 0.0;
+    }
+    int e = 0;
+    if (ext > 0.0) frexp(ext, &e);  // ext < 2^e
+    f.edge = ldexp(1.0, e);
+    f.scale = ldexp(1.0, QBITS - e);
+    f.margin = ldexp(1.0, e - 48);
+    *fr = f;
+}
+
+// hi / lo key words per input row, idx = row; non-finite rows get KEY_NONFINITE and are counted in status[0]
+__global__ void __launch_bounds__(BB) key_kernel(const float* __restrict__ xyz, int64_t n, const Frame* __restrict__ fr,
+                                                 uint64_t* __restrict__ hi, uint64_t* __restrict__ lo,
+                                                 uint32_t* __restrict__ idx, int32_t* __restrict__ status) {
+    const int64_t i = (int64_t)blockIdx.x * BB + threadIdx.x;
+    if (i >= n) return;
+    const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
+    idx[i] = (uint32_t)i;
+    if (!finite3(x, y, z)) {
+        hi[i] = KEY_NONFINITE; lo[i] = KEY_NONFINITE;
+        atomicAdd(status, 1);
+        return;
+    }
+    const double top = 4398046511103.0;  // 2^42 - 1
+    uint64_t q[3];
+    const float c[3] = {x, y, z};
+    for (int a = 0; a < 3; ++a) {
+        const double u = ((double)c[a] - fr->lo[a]) * fr->scale;
+        q[a] = (uint64_t)fmin(fmax(u, 0.0), top);
+    }
+    hi[i] = morton63(q[0] >> 21, q[1] >> 21, q[2] >> 21);
+    lo[i] = morton63(q[0] & MASK21, q[1] & MASK21, q[2] & MASK21);
+}
+
+__global__ void __launch_bounds__(BB) gather_u64_kernel(const uint64_t* __restrict__ src, const uint32_t* __restrict__ idx,
+                                                        int64_t n, uint64_t* __restrict__ dst) {
+    const int64_t j = (int64_t)blockIdx.x * BB + threadIdx.x;
+    if (j < n) dst[j] = src[idx[j]];
+}
+
+// sorted index -> (lo, hi) key pair and the point as float4
+__global__ void __launch_bounds__(BB) gather_sorted_kernel(const uint64_t* __restrict__ hi_sorted,
+                                                           const uint64_t* __restrict__ lo, const uint32_t* __restrict__ idx,
+                                                           const float* __restrict__ xyz, int64_t n,
+                                                           ulonglong2* __restrict__ keys, float4* __restrict__ pts) {
+    const int64_t j = (int64_t)blockIdx.x * BB + threadIdx.x;
+    if (j >= n) return;
+    const uint32_t i = idx[j];
+    keys[j] = make_ulonglong2(lo[i], hi_sorted[j]);
+    pts[j] = make_float4(xyz[3 * (int64_t)i], xyz[3 * (int64_t)i + 1], xyz[3 * (int64_t)i + 2], 0.f);
+}
+
+__device__ __forceinline__ u128 key_at(const ulonglong2* __restrict__ keys, int j) {
+    const ulonglong2 v = keys[j];
+    return (u128)v.y << 63 | v.x;
+}
+
+// first j in [a, n) with key(j) >= K (n if none): galloping from a, then bisection
+__device__ __forceinline__ int lower_bound_from(const ulonglong2* __restrict__ keys, int a, int n, u128 K) {
+    if (a >= n || key_at(keys, a) >= K) return a;
+    int lo = a, hi, step = 1;  // key(lo) < K
+    for (;;) {
+        if (step >= n - lo) { hi = n; break; }
+        hi = lo + step;
+        if (key_at(keys, hi) >= K) break;
+        lo = hi;
+        step <<= 1;
+    }
+    while (hi - lo > 1) {
+        const int mid = lo + ((hi - lo) >> 1);
+        if (key_at(keys, mid) < K) lo = mid; else hi = mid;
+    }
+    return hi;
+}
+
+// best[] holds the k smallest d2 ascending in its LAST k slots (the others are -inf), so the k-th distance is always
+// best[K_MAX - 1] and every index below is a compile-time constant (the list stays in registers)
+__device__ __forceinline__ void consider(double (&best)[K_MAX], const float4 q, const float4 p) {
+    const double dx = __dsub_rn((double)q.x, (double)p.x), dy = __dsub_rn((double)q.y, (double)p.y),
+                 dz = __dsub_rn((double)q.z, (double)p.z);
+    const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+    if (d2 < best[K_MAX - 1]) {  // insert, dropping the largest: new[j] = max(old[j-1], min(old[j], d2))
+#pragma unroll
+        for (int j = K_MAX - 1; j > 0; --j) best[j] = fmax(best[j - 1], fmin(best[j], d2));
+        best[0] = fmin(best[0], d2);
+    }
+}
+
+__device__ __forceinline__ void scan_range(double (&best)[K_MAX], const float4 q, const float4* __restrict__ pts, int j0,
+                                           int j1) {
+    for (int j = j0; j < j1; ++j) consider(best, q, pts[j]);
+}
+
+// distance of the shifted query s from the cell [c*w, (c+1)*w] along one axis, lowered by the margin
+__device__ __forceinline__ double axis_gap(double s, uint64_t c, double w, double margin) {
+    const double lo = (double)c * w, hi = (double)(c + 1) * w;
+    const double g = fmax(fmax(lo - s, s - hi), 0.0);
+    return fmax(g - margin, 0.0);
+}
+
+__global__ void __launch_bounds__(QB) knn_kernel(const ulonglong2* __restrict__ keys, const float4* __restrict__ pts,
+                                                 const uint32_t* __restrict__ order, const Frame* __restrict__ frp, int n,
+                                                 int k, double* __restrict__ avg) {
+    const int t = blockIdx.x * QB + threadIdx.x;
+    if (t >= n) return;
+    const float4 q = pts[t];
+    if (!finite3(q.x, q.y, q.z)) { avg[order[t]] = __longlong_as_double(0x7ff8000000000000ll); return; }
+    const Frame fr = *frp;
+    const int kp = k < n ? k : n;
+    double best[K_MAX];
+#pragma unroll
+    for (int j = 0; j < K_MAX; ++j) best[j] = j >= K_MAX - kp ? INFINITY : -INFINITY;
+
+    const int W = n < WIN ? n : WIN;
+    int w0 = t - WIN / 2;
+    w0 = w0 < 0 ? 0 : (w0 > n - W ? n - W : w0);
+    const int w1 = w0 + W;
+    scan_range(best, q, pts, w0, w1);
+
+    // the same shifted frame as the quantisation
+    const double sx = (double)q.x - fr.lo[0], sy = (double)q.y - fr.lo[1], sz = (double)q.z - fr.lo[2];
+    int L = 1, a = 0;
+    uint64_t cx = 0, cy = 0, cz = 0;
+    double w = fr.edge * 0.5;  // cell edge at level L
+    for (;;) {
+        const double gx = axis_gap(sx, cx, w, fr.margin), gy = axis_gap(sy, cy, w, fr.margin),
+                     gz = axis_gap(sz, cz, w, fr.margin);
+        if (gx * gx + gy * gy + gz * gz < best[K_MAX - 1]) {
+            const int sh = QBITS - L;
+            const u128 start = key126(cx << sh, cy << sh, cz << sh);
+            const int a0 = lower_bound_from(keys, a, n, start);
+            const int b0 = lower_bound_from(keys, a0, n, start + ((u128)1 << (3 * sh)));
+            if (b0 - a0 > LEAF_T && L < QBITS) {  // enter: first child
+                ++L; cx <<= 1; cy <<= 1; cz <<= 1; w *= 0.5; a = a0;
+                continue;
+            }
+            scan_range(best, q, pts, a0, b0 < w0 ? b0 : w0);
+            scan_range(best, q, pts, a0 > w1 ? a0 : w1, b0);
+            a = b0;
+        }
+        // next cell in Morton order: climb out of finished last children, then step to the next sibling
+        while (L > 0 && (cx & cy & cz & 1)) { cx >>= 1; cy >>= 1; cz >>= 1; --L; w *= 2.0; }
+        if (L == 0) break;
+        const uint32_t d = (uint32_t)((cx & 1) << 2 | (cy & 1) << 1 | (cz & 1)) + 1;
+        cx = (cx & ~1ull) | (d >> 2); cy = (cy & ~1ull) | ((d >> 1) & 1); cz = (cz & ~1ull) | (d & 1);
+    }
+
+    double s = 0.0;
+#pragma unroll
+    for (int j = 0; j < K_MAX; ++j)
+        if (j >= K_MAX - kp) s = __dadd_rn(s, sqrt(best[j]));
+    avg[order[t]] = s / (double)kp;
+}
+
+// ---- statistics and keep mask ------------------------------------------------------------------------------------
+constexpr int SB = 256;
+constexpr int SOR_PER_CTA = SB * 8;
+
+// pass 0: per-CTA sum of avg over avg > 0;  pass 1: of (avg - mean)^2 over avg > 0.  Fixed order: bit-identical re-runs.
+template <int PASS>
+__global__ void __launch_bounds__(SB) sor_partial_kernel(const double* __restrict__ avg, int64_t n,
+                                                         const double* __restrict__ stats, double* __restrict__ partial) {
+    __shared__ double s_w[SB / 32];
+    const double mean = PASS == 1 ? stats[0] : 0.0;
+    const int64_t base = (int64_t)blockIdx.x * SOR_PER_CTA;
+    double v = 0.0;
+    for (int r = 0; r < SOR_PER_CTA / SB; ++r) {
+        const int64_t i = base + r * SB + threadIdx.x;
+        if (i >= n) break;
+        const double x = avg[i];
+        if (x > 0.0) v = __dadd_rn(v, PASS == 0 ? x : __dmul_rn(x - mean, x - mean));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double tot = 0.0;
+        for (int w = 0; w < SB / 32; ++w) tot = __dadd_rn(tot, s_w[w]);
+        partial[blockIdx.x] = tot;
+    }
+}
+
+// one CTA: fixed-order sum of the partials; pass 0 -> stats[0] = mean, pass 1 -> stats[1] = std, stats[2] = threshold.
+// Every point has a neighbour (itself), so the count of valid distances is n.
+template <int PASS>
+__global__ void __launch_bounds__(1024) sor_finish_kernel(const double* __restrict__ partial, int nb, int64_t n,
+                                                          double std_ratio, double* __restrict__ stats) {
+    __shared__ double s[1024];
+    double t = 0.0;
+    for (int i = threadIdx.x; i < nb; i += 1024) t = __dadd_rn(t, partial[i]);
+    s[threadIdx.x] = t;
+    __syncthreads();
+    for (int o = 512; o > 0; o >>= 1) {
+        if (threadIdx.x < o) s[threadIdx.x] = __dadd_rn(s[threadIdx.x], s[threadIdx.x + o]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        if (PASS == 0) {
+            stats[0] = s[0] / (double)n;
+        } else {
+            const double sd = sqrt(s[0] / (double)(n - 1));  // n == 1: 0 / 0 = NaN, nothing is kept
+            stats[1] = sd;
+            stats[2] = __dadd_rn(stats[0], __dmul_rn(std_ratio, sd));
+        }
+    }
+}
+
+__global__ void __launch_bounds__(SB) sor_keep_kernel(const double* __restrict__ avg, int64_t n,
+                                                      const double* __restrict__ stats, uint8_t* __restrict__ keep) {
+    const int64_t i = (int64_t)blockIdx.x * SB + threadIdx.x;
+    if (i >= n) return;
+    const double x = avg[i];
+    keep[i] = (x > 0.0 && x < stats[2]) ? 1 : 0;
+}
+
+// workspace layout of g2pc_knn_mean_dist
+struct KnnLayout {
+    size_t frame, part, hi, lo, keys, idx_a, idx_b, pts, tmp, tmp_bytes, total;
+};
+
+KnnLayout knn_layout(int64_t n) {
+    KnnLayout l;
+    size_t sort_b = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, n, 0, 63);
+    const size_t nb = (size_t)((n + BOX_PER_CTA - 1) / BOX_PER_CTA);
+    const size_t un = (size_t)n;
+    size_t o = 0;
+    l.frame = o; o += align256(sizeof(Frame));
+    l.part = o; o += align256(nb * 6 * sizeof(float));
+    l.hi = o; o += align256(un * 8);
+    l.lo = o; o += align256(un * 8);
+    l.keys = o; o += 2 * align256(un * 8);  // first the two 8n-byte sort buffers, then the (lo, hi) key pairs
+    l.idx_a = o; o += align256(un * 4);
+    l.idx_b = o; o += align256(un * 4);
+    l.pts = o; o += align256(un * 16);
+    l.tmp = o; l.tmp_bytes = align256(sort_b); o += l.tmp_bytes;
+    l.total = o;
+    return l;
+}
+
+}  // namespace
+
+extern "C" int64_t g2pc_knn_workspace_bytes(int64_t n) { return n <= 0 ? 0 : (int64_t)knn_layout(n).total; }
+
+extern "C" int g2pc_knn_mean_dist(const float* xyz, int64_t n, int32_t k, double* avg, int32_t* status, void* workspace,
+                                  int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(n >= 0, "n < 0");
+    G2PC_CHECK_ARG(n < 0x7FFFFFFFll, "n must fit int32 indices");
+    G2PC_CHECK_ARG(k >= 1 && k <= K_MAX, "k must be in 1..G2PC_SOR_K_MAX");
+    G2PC_CHECK_ARG(status, "null status");
+    cudaStream_t st = (cudaStream_t)stream;
+    G2PC_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+    if (n == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(xyz && avg && workspace, "null pointer");
+    const KnnLayout l = knn_layout(n);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.total, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    char* ws = (char*)workspace;
+    Frame* fr = (Frame*)(ws + l.frame);
+    float* part = (float*)(ws + l.part);
+    uint64_t* hi = (uint64_t*)(ws + l.hi);
+    uint64_t* lo = (uint64_t*)(ws + l.lo);
+    uint64_t* lo_by_lo = (uint64_t*)(ws + l.keys);               // sort 1 output keys
+    uint64_t* hi_by_lo = (uint64_t*)(ws + l.keys + align256((size_t)n * 8));  // hi gathered in that order
+    uint64_t* hi_sorted = hi;                                      // sort 2 output keys (hi is dead by then)
+    ulonglong2* keys = (ulonglong2*)(ws + l.keys);
+    uint32_t* idx_a = (uint32_t*)(ws + l.idx_a);
+    uint32_t* idx_b = (uint32_t*)(ws + l.idx_b);
+    float4* pts = (float4*)(ws + l.pts);
+    void* tmp = ws + l.tmp;
+    const int nbox = (int)((n + BOX_PER_CTA - 1) / BOX_PER_CTA);
+    const unsigned g = (unsigned)((n + BB - 1) / BB);
+
+    bbox_kernel<<<nbox, BB, 0, st>>>(xyz, n, part);
+    G2PC_CHECK_LAUNCH();
+    frame_kernel<<<1, 1, 0, st>>>(part, nbox, fr);
+    G2PC_CHECK_LAUNCH();
+    key_kernel<<<g, BB, 0, st>>>(xyz, n, fr, hi, lo, idx_a, status);
+    G2PC_CHECK_LAUNCH();
+    size_t b = l.tmp_bytes;
+    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, lo, lo_by_lo, idx_a, idx_b, n, 0, 63, st));
+    gather_u64_kernel<<<g, BB, 0, st>>>(hi, idx_b, n, hi_by_lo);
+    G2PC_CHECK_LAUNCH();
+    b = l.tmp_bytes;  // stable: points with equal hi keep their lo order
+    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, hi_by_lo, hi_sorted, idx_b, idx_a, n, 0, 63, st));
+    gather_sorted_kernel<<<g, BB, 0, st>>>(hi_sorted, lo, idx_a, xyz, n, keys, pts);
+    G2PC_CHECK_LAUNCH();
+    knn_kernel<<<(unsigned)((n + QB - 1) / QB), QB, 0, st>>>(keys, pts, idx_a, fr, (int)n, k, avg);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_sor_workspace_bytes(int64_t n) {
+    return (int64_t)(((n + SOR_PER_CTA - 1) / SOR_PER_CTA + 1) * sizeof(double));
+}
+
+extern "C" int g2pc_sor_mask(const double* avg, int64_t n, double std_ratio, uint8_t* keep, double* stats,
+                             void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(n >= 0, "n < 0");
+    G2PC_CHECK_ARG(std_ratio > 0.0, "std_ratio must be > 0");
+    if (n == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(avg && keep && stats && workspace, "null pointer");
+    G2PC_CHECK_ARG(workspace_bytes >= g2pc_sor_workspace_bytes(n), "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 7) == 0, "workspace must be 8-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int nb = (int)((n + SOR_PER_CTA - 1) / SOR_PER_CTA);
+    double* partial = (double*)workspace;
+    sor_partial_kernel<0><<<nb, SB, 0, st>>>(avg, n, stats, partial);
+    G2PC_CHECK_LAUNCH();
+    sor_finish_kernel<0><<<1, 1024, 0, st>>>(partial, nb, n, std_ratio, stats);
+    G2PC_CHECK_LAUNCH();
+    sor_partial_kernel<1><<<nb, SB, 0, st>>>(avg, n, stats, partial);
+    G2PC_CHECK_LAUNCH();
+    sor_finish_kernel<1><<<1, 1024, 0, st>>>(partial, nb, n, std_ratio, stats);
+    G2PC_CHECK_LAUNCH();
+    sor_keep_kernel<<<(unsigned)((n + SB - 1) / SB), SB, 0, st>>>(avg, n, stats, keep);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}

@@ -155,6 +155,28 @@ int64_t g2pc_ppg_workspace_bytes(int64_t n);
 int g2pc_points_per_gaussian(const float* cov, const float* contrib, int64_t n, double num_points, double* magnitudes,
                              int32_t* ppg, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- N5: statistical outlier removal of the point cloud (s9_clean.cu, --clean_pointcloud) ------------------------ */
+/* Replaces Open3D's PointCloud::remove_statistical_outlier(nb_neighbors=20, std_ratio) behind the reference's
+ * mesh_handler.clean_point_cloud (mesh_handler.py:89-94, called at gauss_to_pc.py:743-759).  Compact the cloud with
+ * keep as the extra_mask of g2pc_cull_select, then g2pc_gather_rows. */
+#define G2PC_SOR_K_MAX 32 /* largest nb_neighbors */
+
+/* avg (n float64) = mean of the sqrt of the k' = min(k, n) smallest squared distances of every point to the cloud (the
+ * point itself included, d2 = (dx*dx + dy*dy) + dz*dz in float64 of the float32 coordinates, summed in ascending order):
+ * exact, not approximate.  xyz (n,3) f32; 1 <= k <= G2PC_SOR_K_MAX.  status: one int32, set to the number of points with a
+ * non-finite coordinate (their avg is NaN and they are nobody's neighbour).  workspace: g2pc_knn_workspace_bytes(n),
+ * 256-byte aligned. */
+int64_t g2pc_knn_workspace_bytes(int64_t n);
+int g2pc_knn_mean_dist(const float* xyz, int64_t n, int32_t k, double* avg, int32_t* status, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+/* stats (3 float64): mean = (sum of avg over avg > 0) / n, std = sqrt((sum of (avg - mean)^2 over avg > 0) / (n - 1)),
+ * threshold = mean + std_ratio * std, each sum reduced in a fixed order (bit-identical re-runs); keep (n uint8) =
+ * avg > 0 && avg < threshold.  std_ratio > 0.  workspace: g2pc_sor_workspace_bytes(n), 8-byte aligned.  n == 0 writes
+ * nothing. */
+int64_t g2pc_sor_workspace_bytes(int64_t n);
+int g2pc_sor_mask(const double* avg, int64_t n, double std_ratio, uint8_t* keep, double* stats, void* workspace,
+                  int64_t workspace_bytes, void* stream);
+
 /* ---- S3-S6: colour stage, renderer_type=python semantics (gauss_render.py:101-465) ------------------------------ */
 /* Replaces GaussPythonRenderer.__call__/render (gauss_render.py:266-465) and — as the native op boundary — the role
  * of _C.rasterize_gaussians (rasterize_points.cu:36-145) in the per-camera loop of gauss_to_pc.py:437-454.

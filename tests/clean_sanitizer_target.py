@@ -1,0 +1,47 @@
+"""Tiny statistical-outlier clean, meant to be executed under compute-sanitizer (tests/test_clean_gpu.py): memcheck and
+racecheck over the k-NN index build, the query kernel, the statistics and the compaction.
+
+Without the sanitizer (the test runs it directly when the tool does not support the GPU):
+  G2PC_TARGET_POISON=<byte>   every block PyTorch's caching allocator hands out afterwards starts filled with <byte>
+  G2PC_TARGET_OUT=<file.npz>  every output of the run is saved there, for bit-for-bit comparison between runs"""
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "3dgs-to-pc_b200"))
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from g2pc import outliers  # noqa: E402
+
+dev = "cuda:0"
+
+
+def poison_allocator(byte):
+    """Fill and release blocks of both pools of the caching allocator (it keeps them cached), so a kernel that reads
+    memory nobody wrote sees `byte`."""
+    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(64)]
+    large = [torch.full((64 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(4)]
+    torch.cuda.synchronize()
+    del small, large
+    for nbytes in (4096, 8 << 20):
+        probe = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
+        del probe
+
+
+if os.environ.get("G2PC_TARGET_POISON") is not None:
+    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
+rng = np.random.default_rng(3)
+p = np.concatenate([rng.random((3000, 3)), np.repeat(rng.random((1, 3)), 25, 0), [[40.0, 40.0, 40.0]],
+                    0.5 + 1e-6 * rng.random((500, 3))]).astype(np.float32)
+xyz = torch.from_numpy(p).to(dev)
+cols = torch.from_numpy(rng.uniform(-10, 300, p.shape).astype(np.float32)).to(dev)
+nrm = torch.from_numpy(rng.normal(size=p.shape).astype(np.float32)).to(dev)
+pts, c, n, dbg = outliers.remove_statistical_outliers(xyz, cols, nrm, 20, 3.0, return_debug=True)
+torch.cuda.synchronize()
+if os.environ.get("G2PC_TARGET_OUT"):
+    outputs = dict(points=pts, colours=c, normals=n, **dbg)
+    np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
+print("CLEAN_TARGET_OK", pts.shape[0])

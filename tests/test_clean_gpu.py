@@ -1,0 +1,347 @@
+"""GPU: statistical outlier removal (--clean_pointcloud, g2pc_knn_mean_dist + g2pc_sor_mask + the cull compaction)
+against the float64 restatement of Open3D's rule (f64ref_outliers.statistical_outliers).
+
+The per-point mean distances are exact: the kernel evaluates the same float64 operations in the same order as the
+oracle, so they must be bit-identical.  The cloud statistics are reduced in a fixed order on the device and
+sequentially in the oracle, so they agree to 1e-12 relative; a point whose avg lies within 1e-12 * threshold of the
+threshold may then be kept by one and not the other (counted and printed; none are expected)."""
+import os
+import shutil
+import subprocess
+import sys
+import time
+import zlib
+
+import numpy as np
+import pytest
+import torch
+
+import f64ref_outliers
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda:0"
+HERE = os.path.dirname(os.path.abspath(__file__))
+TARGET = os.path.join(HERE, "clean_sanitizer_target.py")
+K_MAX = 32
+BAND = 1e-12
+
+
+def _sampled_cloud(n_gaussians, num_points, seed):
+    """Point cloud of a synthetic scene sampled the way the CLI does with --no_render_colours."""
+    import gauss_to_pc as g2p
+    from g2pc import sampler, synth
+    sc = {k: v.to(DEV) for k, v in synth.make_scene(n_gaussians, seed=seed).items()}
+    st = g2p.GaussPointCloudSettings(
+        renderer_type="python", num_points=num_points, prioritise_visible_gaussians=True, mahalanobis_distance_std=2.0,
+        camera_skip_rate=0, render_colours=False, min_opacity=0.0, bounding_box_min=None, bounding_box_max=None,
+        calculate_normals=True, cull_large_percentage=0.0, remove_unrendered_gaussians=True, colour_resolution=None,
+        max_sh_degree=3, exact_num_points=False, visibility_threshold=0.05, surface_distance_std=None,
+        generate_mesh=False, quiet=True, device=DEV)
+    sampler.reset_call_counter(0)
+    pc, _ = g2p.convert_gaussians_to_pc(sc["xyz"], sc["scales"], sc["rots"], sc["colours"].clone() * 255,
+                                        sc["opacities"], sc["shs"], None, None, None, st)
+    return pc
+
+
+def _scene(name, rng):
+    u = lambda n, lo=0.0, hi=1.0: rng.uniform(lo, hi, (n, 3)).astype(np.float32)
+    if name == "sampled":
+        return _sampled_cloud(60_000, 200_000, seed=71).points.cpu().numpy()
+    if name == "cube":
+        return u(100_000)
+    if name == "plane":
+        p = u(100_000, -2.0, 2.0)
+        p[:, 2] = np.float32(0.5) + rng.normal(0, 1e-6, p.shape[0]).astype(np.float32)
+        return p
+    if name == "dense_sparse":
+        return np.concatenate([np.float32(0.3) + u(50_000, 0.0, 1e-4), u(5_000)])
+    if name == "isolated":
+        return np.concatenate([u(20_000), np.float32([[1e3, 1e3, 1e3], [-1e3, 0, 0], [0, 1e3, -1e3], [2e3, 2e3, 2e3]])])
+    if name == "far_clusters":
+        centres = np.float32([[1e4, 1e4, 1e4], [-1e4, 1e4, -1e4], [1e4, -1e4, 0], [-1e4, -1e4, -1e4]])
+        return np.concatenate([c + u(5_000, 0.0, 1e-3) for c in centres]).astype(np.float32)
+    if name == "dup_runs":
+        parts = [u(3_000)]
+        for r in (18, 19, 20, 21, 30, 31, 32, 33, 40):
+            parts += [np.repeat(u(1), r, 0), u(7)]
+        p = np.concatenate(parts)
+        return p[rng.permutation(p.shape[0])]
+    if name == "lattice":  # every point on an octree cell boundary
+        g = np.arange(32, dtype=np.float32)
+        return np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3)
+    if name.startswith("small"):
+        return u(int(name[5:]))
+    raise KeyError(name)
+
+
+SCENES = ["sampled", "cube", "plane", "dense_sparse", "isolated", "far_clusters", "dup_runs", "lattice", "small1",
+          "small5", "small19", "small31"]
+
+
+def _avg(p, k):
+    from g2pc import outliers
+    xyz = torch.from_numpy(np.ascontiguousarray(p, dtype=np.float32)).to(DEV)
+    avg, status = outliers.mean_distances(xyz, k)
+    assert int(status.item()) == 0
+    return avg.cpu().numpy()
+
+
+def _same(a, b):
+    """Bit-for-bit equality as a plain bool (keeps pytest from diffing megabytes of bytes on a failure)."""
+    return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
+
+
+def _ulps(a, b):
+    ia, ib = a.view(np.int64), b.view(np.int64)
+    return np.abs(ia - ib)
+
+
+@pytest.mark.parametrize("k", [1, 2, 20, K_MAX])
+@pytest.mark.parametrize("scene", SCENES)
+def test_mean_distances_bit_identical(lib, scene, k):
+    rng = np.random.default_rng(zlib.crc32(f"{scene}/{k}".encode()))
+    p = _scene(scene, rng)
+    got = _avg(p, k)
+    want = f64ref_outliers.knn_mean_distances(p, k)
+    diff = got.tobytes() != want.tobytes()
+    if diff:
+        bad = np.nonzero(got != want)[0]
+        print(f"[{scene} k={k}] {bad.size} of {p.shape[0]} differ, max {_ulps(got, want).max()} ulp; first "
+              f"{bad[:5]} got {got[bad[:5]]} want {want[bad[:5]]}")
+    assert not diff
+
+
+def _check_keep(keep, avg, thr, tag):
+    rule = (avg > 0) & (avg < thr)
+    band = np.abs(avg - thr) <= BAND * abs(thr)
+    off = (keep != rule) & ~band
+    print(f"[{tag}] kept {int(keep.sum())} of {avg.size}; {int(band.sum())} point(s) within the threshold band")
+    assert not off.any(), f"{int(off.sum())} keep decisions differ outside the band"
+
+
+@pytest.mark.parametrize("scene", ["sampled", "isolated", "dup_runs", "small1", "small5"])
+def test_statistics_and_keep_mask(lib, scene):
+    from g2pc import outliers
+    p = _scene(scene, np.random.default_rng(3))
+    avg_o, keep_o, (mean, std, thr) = f64ref_outliers.statistical_outliers(p, 20, 10.0)
+    xyz = torch.from_numpy(p).to(DEV)
+    avg, _ = outliers.mean_distances(xyz, 20)
+    keep, stats = outliers.sor_mask(avg, 10.0)
+    s = stats.cpu().numpy()
+    if p.shape[0] == 1:
+        assert s[0] == 0.0 and np.isnan(s[1]) and np.isnan(s[2]) and int(keep.sum()) == 0
+        return
+    for got, want in zip(s, (mean, std, thr)):
+        assert abs(got - want) <= 1e-12 * abs(want), (s, (mean, std, thr))
+    _check_keep(keep.cpu().numpy().astype(bool), avg_o, thr, scene)
+
+
+def test_output_rows(lib):
+    from g2pc import outliers
+    rng = np.random.default_rng(8)
+    p = np.concatenate([rng.random((20_000, 3)), rng.uniform(5, 50, (40, 3))]).astype(np.float32)
+    n = p.shape[0]
+    cols = torch.from_numpy(rng.uniform(-60.0, 320.0, (n, 3)).astype(np.float32)).to(DEV)
+    cols[:3] = torch.tensor([[-0.5, 255.0, 255.9], [0.99, 254.99, 1e9], [-1e9, 0.0, 128.5]], device=DEV)
+    nrm = torch.from_numpy(rng.normal(size=(n, 3)).astype(np.float32)).to(DEV)
+    xyz = torch.from_numpy(p).to(DEV)
+    pts, c, nn, dbg = outliers.remove_statistical_outliers(xyz, cols, nrm, 20, 3.0, return_debug=True)
+    _, keep_o, _ = f64ref_outliers.statistical_outliers(p, 20, 3.0)
+    keep = dbg["keep"].cpu().numpy().astype(bool)
+    assert np.array_equal(keep, keep_o) and not keep[20_000:].all()
+    assert pts.dtype == torch.float32 and _same(pts.cpu().numpy(), p[keep])
+    want_c = np.clip(cols.cpu().numpy(), 0, 255).astype(np.int32)[keep]
+    assert c.dtype == torch.int32 and np.array_equal(c.cpu().numpy(), want_c)
+    assert _same(nn.cpu().numpy(), nrm.cpu().numpy()[keep])
+    pts2, c2, nn2 = outliers.remove_statistical_outliers(xyz, None, None, 20, 3.0)
+    assert c2 is None and nn2 is None and torch.equal(pts2, pts)
+    import mesh_handler
+    pts3, c3, nn3 = mesh_handler.clean_point_cloud(xyz, cols, None, std_ratio=3.0)
+    assert nn3 is None and torch.equal(pts3, pts) and torch.equal(c3, c)
+    # an empty cloud comes back empty
+    e = torch.zeros((0, 3), device=DEV)
+    pe, ce, ne = outliers.remove_statistical_outliers(e, e, None)
+    assert pe.shape == (0, 3) and ce.shape == (0, 3) and ce.dtype == torch.int32 and ne is None
+
+
+def poison_allocator(byte):
+    """Fill and release blocks of both pools of PyTorch's caching allocator (it keeps them cached), so any memory a
+    kernel reads without writing it first holds `byte`.  Blocks the allocator serves from elsewhere (a free tail of a
+    segment that still holds a live tensor, or a fresh cudaMalloc) are not poisoned: this run checks that a clean on
+    reused memory repeats bit for bit; the small sanitizer target, poisoned before its first allocation, checks reads
+    of unwritten memory."""
+    torch.cuda.empty_cache()
+    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=DEV) for _ in range(64)]
+    large = [torch.full((1 << 30,), byte, dtype=torch.uint8, device=DEV) for _ in range(4)]
+    torch.cuda.synchronize()
+    del small, large
+    for nbytes in (4096, 8 << 20):
+        probe = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
+        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
+        del probe
+
+
+def _clean_to_host(xyz, cols, nrm):
+    from g2pc import outliers
+    out = outliers.remove_statistical_outliers(xyz, cols, nrm, 20, 10.0, return_debug=True)
+    return [t.cpu().numpy() for t in out[:3]] + [out[3][k].cpu().numpy() for k in ("avg", "stats", "keep")]
+
+
+def test_scale_c3_cloud(lib):
+    """A 10 M-point cloud sampled like C3: avg on a 20 k subset bit-identical to the oracle over all 10 M points, the
+    statistics recomputed on the host from the kernel's avg, the keep rule, and three bit-identical runs (the last one
+    on poisoned allocator memory)."""
+    pc = _sampled_cloud(3_000_000, 10_000_000, seed=1236)
+    host = [t.cpu() for t in (pc.points, pc.colours, pc.normals)]
+    n = host[0].shape[0]
+    assert n > 9_000_000
+    runs = [_clean_to_host(pc.points, pc.colours, pc.normals) for _ in range(2)]
+    del pc
+    poison_allocator(0x5A)
+    runs.append(_clean_to_host(*[t.to(DEV) for t in host]))
+    for r in runs[1:]:
+        for a, b in zip(runs[0], r):
+            assert _same(a, b)
+    pts, _, _, avg, s, keep = runs[0]
+    keep = keep.astype(bool)
+    p = host[0].numpy()
+    sub = np.random.default_rng(4).choice(n, 20_000, replace=False)
+    want = f64ref_outliers.knn_mean_distances(p, 20, query=sub)
+    assert _same(avg[sub], want), f"{int((avg[sub] != want).sum())} of 20000 differ"
+    mean, std, thr = f64ref_outliers.sor_statistics(avg, 10.0)
+    for got, w in zip(s, (mean, std, thr)):
+        assert abs(got - w) <= 1e-12 * abs(w), (s, (mean, std, thr))
+    _check_keep(keep, avg, thr, "10M")
+    assert _same(pts, p[keep])
+
+
+@pytest.mark.parametrize("case", ["copies", "tiny_cube"])
+def test_bounded_work(lib, case):
+    """Degenerate clouds finish within 10 s (a bound on the work, not a performance claim)."""
+    from g2pc import outliers
+    rng = np.random.default_rng(12)
+    sparse = rng.uniform(-1.0, 1.0, (1000, 3)).astype(np.float32)
+    if case == "copies":
+        dense = np.repeat(np.float32([[0.25, -0.5, 0.125]]), 1_000_000, 0)
+    else:
+        dense = (np.float32(0.1) + rng.uniform(0, 1e-5, (1_000_000, 3))).astype(np.float32)
+    p = np.concatenate([dense, sparse])
+    xyz = torch.from_numpy(p).to(DEV)
+    outliers.remove_statistical_outliers(xyz[:1000], None, None)  # warm-up
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    _, _, _, dbg = outliers.remove_statistical_outliers(xyz, None, None, return_debug=True)
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    print(f"[{case}] clean of {p.shape[0]} points: {dt:.3f} s")
+    assert dt < 10.0
+    avg = dbg["avg"].cpu().numpy()
+    if case == "copies":
+        assert (avg[:1_000_000] == 0).all() and not dbg["keep"].cpu().numpy()[:1_000_000].any()
+        # the k nearest of a scattered point hold at most k copies: the oracle over 20 copies + the sparse points
+        want = f64ref_outliers.knn_mean_distances(np.concatenate([dense[:20], sparse]), 20)[20:]
+        assert _same(avg[1_000_000:], want)
+    else:
+        sub = np.concatenate([np.arange(0, 1_000_000, 997), np.arange(1_000_000, p.shape[0])])
+        want = f64ref_outliers.knn_mean_distances(p, 20, query=sub)
+        assert _same(avg[sub], want)
+
+
+def test_cli_clean(lib, tmp_path):
+    """g2p.main with and without --clean_pointcloud on the same scene and seed: the cleaned PLY's records are the
+    uncleaned PLY's records selected by the oracle's keep mask; --no_calculate_normals writes no normal properties."""
+    import gauss_dataloader as gd
+    import gauss_to_pc as g2p
+    from g2pc import sampler, synth
+    from test_io_cpu import write_gaussian_ply
+    sc = synth.make_scene(20_000, seed=23, sh_degree=3)
+    ply = str(tmp_path / "scene.ply")
+    write_gaussian_ply(ply, sc)
+    outs = {}
+    for tag, extra in (("raw", []), ("clean", ["--clean_pointcloud"]), ("raw_nn", ["--no_calculate_normals"]),
+                       ("clean_nn", ["--no_calculate_normals", "--clean_pointcloud"])):
+        outs[tag] = str(tmp_path / f"{tag}.ply")
+        sampler.reset_call_counter(0)
+        g2p.main(["--input_path", ply, "--output_path", outs[tag], "--num_points", "150000", "--no_render_colours",
+                  "--quiet"] + extra)
+    for raw, clean in (("raw", "clean"), ("raw_nn", "clean_nn")):
+        v, c = gd.read_ply_vertices(outs[raw]), gd.read_ply_vertices(outs[clean])
+        assert v.dtype == c.dtype
+        p = np.stack([v["x"], v["y"], v["z"]], 1)
+        avg, keep, (_, _, thr) = f64ref_outliers.statistical_outliers(p, 20, 10.0)
+        assert int((np.abs(avg - thr) <= BAND * thr).sum()) == 0
+        assert 0 < int(keep.sum()) < p.shape[0] or keep.all()
+        assert _same(c, v[keep])
+    with open(outs["clean_nn"], "rb") as f:
+        head = f.read(400).split(b"end_header")[0]
+    assert b"nx" not in head and b"red" in head
+    with open(outs["clean"], "rb") as f:
+        assert b"property float nx" in f.read(400)
+
+
+def test_errors(lib):
+    from g2pc import capi, outliers
+    p = torch.rand((100, 3), device=DEV)
+    with pytest.raises(capi.G2pcError):
+        outliers.remove_statistical_outliers(p.cpu(), None, None)
+    for bad in (float("nan"), float("inf"), -float("inf")):
+        q = p.clone()
+        q[17, 1] = bad
+        with pytest.raises(capi.G2pcError, match="non-finite"):
+            outliers.remove_statistical_outliers(q, None, None)
+    for k in (0, -1, K_MAX + 1):
+        with pytest.raises(capi.G2pcError):
+            outliers.remove_statistical_outliers(p, None, None, nb_neighbors=k)
+    for r in (0.0, -1.0, float("nan")):
+        with pytest.raises(capi.G2pcError):
+            outliers.remove_statistical_outliers(p, None, None, std_ratio=r)
+    with pytest.raises(capi.G2pcError):
+        outliers.remove_statistical_outliers(p.double(), None, None)
+    with pytest.raises(capi.G2pcError):  # the C ABI refuses k above the cap on its own
+        capi.call("g2pc_knn_mean_dist", capi.ptr(p), 100, K_MAX + 1, None, None, None, 0, capi.stream_ptr(DEV))
+
+
+def _sanitizer():
+    return shutil.which("compute-sanitizer") or (
+        "/usr/local/cuda/bin/compute-sanitizer" if os.path.exists("/usr/local/cuda/bin/compute-sanitizer") else None)
+
+
+def _run_target(env_extra, out):
+    env = dict(os.environ, G2PC_TARGET_OUT=str(out), **env_extra)
+    r = subprocess.run([sys.executable, TARGET], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env,
+                       timeout=600)
+    assert r.returncode == 0 and "CLEAN_TARGET_OK" in r.stdout, r.stdout[-3000:]
+    with np.load(out) as z:
+        return {k: z[k] for k in z.files}
+
+
+def _check_from_outputs(tmp_path):
+    runs = [_run_target({"G2PC_TARGET_POISON": b, "CUDA_LAUNCH_BLOCKING": "1"}, tmp_path / f"fill_{b}.npz")
+            for b in ("0x00", "0xff", "0x5a")]
+    for other in runs[1:]:
+        assert sorted(other) == sorted(runs[0])
+        for k in runs[0]:
+            assert _same(other[k], runs[0][k]), k
+
+
+@pytest.mark.parametrize("tool", ["memcheck", "racecheck"])
+def test_clean_under_compute_sanitizer(lib, tool, tmp_path):
+    exe = _sanitizer()
+    if exe is None:
+        _check_from_outputs(tmp_path)
+        return
+    cmd = [exe, "--tool", tool, "--kernel-name", "kns=_GLOBAL__N_"] + \
+          (["--report-api-errors", "no"] if tool == "memcheck" else []) + ["--print-limit", "5", sys.executable, TARGET]
+    try:
+        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
+    except subprocess.TimeoutExpired:
+        pytest.skip("compute-sanitizer run exceeded 10 minutes on this box")
+    if "Error: Device not supported" in r.stdout:
+        _check_from_outputs(tmp_path)
+        return
+    tail = r.stdout[-3000:]
+    assert "CLEAN_TARGET_OK" in r.stdout, tail
+    if tool == "racecheck":
+        assert "RACECHECK SUMMARY: 0 hazards displayed (0 errors, 0 warnings)" in r.stdout, tail
+    else:
+        assert "ERROR SUMMARY: 0 errors" in r.stdout, tail
