@@ -1,0 +1,1272 @@
+// s10_mesh.cu — Poisson surface reconstruction of an oriented point cloud (N6): splat, multigrid solve, iso-value,
+// marching tetrahedra, per-vertex density / colour gathers, density trim, Laplacian smoothing and vertex normals.
+//
+// Reference semantics restated (not copied): mesh_handler.py:23-40 generate_mesh = Open3D statistical outlier removal,
+// create_from_point_cloud_poisson(depth), removal of the vertices below the 10 % density quantile, Laplacian smoothing.
+// The rules below are this project's own (Open3D's octree solver is not restated); DESIGN.md §2 writes them down and
+// tests/f64ref_mesh.py restates them in float64.
+//
+// Grid: R = 2^depth nodes per axis at the cell centres origin + (i + 1/2) h of a cube of edge L = 1.1 x the largest
+// extent, centred on the bounding box; node index (k R + j) R + i.  Every point has a dual cell i0 (the 2x2x2 nodes
+// around it) and trilinear weights w = (wx * wy) * wz.  B (int64) is the central-difference divergence of the splatted
+// normals in units of 2^-32: exact integer atomics, so re-runs are bit-identical.  The solve works on float32 grids with
+// the right-hand side b = (B - mean B) * h * 2^-33 formed on the fly from B (no float copy of b is stored).
+// All float64 expressions that a test compares bit for bit are written with __d*_rn intrinsics: no FMA contraction.
+#include <cub/cub.cuh>
+#include "common.cuh"
+
+namespace {
+
+constexpr int MB = 256;                         // threads per CTA of the per-point / per-cell kernels
+constexpr int RED_BLOCKS = 1024;                // fixed partition of every float64 reduction: bit-identical re-runs
+constexpr int NPT = 4;                          // lattice nodes per thread in the extraction kernels
+constexpr int NODES_PER_CTA = MB * NPT;
+constexpr int BOX_PER_CTA = MB * 8;
+constexpr int COARSE_SWEEPS = 100;              // red-black sweeps of the 4^3 coarsest level
+constexpr uint32_t CELL_NONE = 0x7FFFFFFFu;     // dual cell of a point that was not splatted (sorts last)
+constexpr double TWO32 = 4294967296.0;
+
+// frame words (float64, device): written by g2pc_mesh_splat
+enum { FR_ORIGIN = 0, FR_H = 3, FR_L = 4, FR_MEANB = 5, FR_EXTENT = 6, FR_R = 7 };
+
+__host__ __device__ __forceinline__ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+__device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
+
+struct PointCell {
+    int i0[3];
+    double f[3];
+};
+
+// u = (p - origin) / h - 1/2, i0 = clamp(floor(u), 0, R - 2), f = clamp(u - i0, 0, 1)
+__device__ __forceinline__ PointCell point_cell(const float* __restrict__ xyz, int64_t i, const double* __restrict__ fr,
+                                                int R) {
+    PointCell c;
+    const double h = fr[FR_H];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const double u = __dsub_rn(__ddiv_rn(__dsub_rn((double)xyz[3 * i + a], fr[FR_ORIGIN + a]), h), 0.5);
+        const double fl = fmin(fmax(floor(u), 0.0), (double)(R - 2));
+        c.i0[a] = (int)fl;
+        c.f[a] = fmin(fmax(__dsub_rn(u, fl), 0.0), 1.0);
+    }
+    return c;
+}
+
+// weight of dual-cell corner o (bit 0 = x): (wx * wy) * wz with w = f on the upper side, 1 - f on the lower
+__device__ __forceinline__ double corner_weight(const PointCell& c, int o) {
+    double w[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) w[a] = (o >> a) & 1 ? c.f[a] : __dsub_rn(1.0, c.f[a]);
+    return __dmul_rn(__dmul_rn(w[0], w[1]), w[2]);
+}
+
+__device__ __forceinline__ uint32_t cell_id(const PointCell& c, int R) {
+    return ((uint32_t)c.i0[2] * (uint32_t)(R - 1) + (uint32_t)c.i0[1]) * (uint32_t)(R - 1) + (uint32_t)c.i0[0];
+}
+
+__device__ __forceinline__ double node_coord(const double* __restrict__ fr, int a, int i) {
+    return __dadd_rn(fr[FR_ORIGIN + a], __dmul_rn((double)i + 0.5, fr[FR_H]));
+}
+
+// ---- fixed-order float64 reductions -----------------------------------------------------------------------------
+__device__ __forceinline__ double block_sum(double v, double* s_w) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double t = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t = __dadd_rn(t, s_w[w]);
+    return t;  // valid in thread 0
+}
+
+// one CTA of 1024 threads: out[slot] = sum of RED_BLOCKS partials (x scale), in a fixed order
+__global__ void __launch_bounds__(1024) finish_kernel(const double* __restrict__ partial, double scale,
+                                                      double* __restrict__ out) {
+    __shared__ double s[1024];
+    s[threadIdx.x] = threadIdx.x < RED_BLOCKS ? partial[threadIdx.x] : 0.0;
+    __syncthreads();
+    for (int o = 512; o > 0; o >>= 1) {
+        if (threadIdx.x < o) s[threadIdx.x] = __dadd_rn(s[threadIdx.x], s[threadIdx.x + o]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *out = __dmul_rn(s[0], scale);
+}
+
+// ---- splat ------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(MB) bbox_kernel(const float* __restrict__ xyz, int64_t n, float* __restrict__ part) {
+    __shared__ float s[6][MB / 32];
+    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+    const int64_t base = (int64_t)blockIdx.x * BOX_PER_CTA;
+    for (int r = 0; r < BOX_PER_CTA / MB; ++r) {
+        const int64_t i = base + r * MB + threadIdx.x;
+        if (i >= n) break;
+        const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
+        if (!finite3(x, y, z)) continue;
+        mn[0] = fminf(mn[0], x); mn[1] = fminf(mn[1], y); mn[2] = fminf(mn[2], z);
+        mx[0] = fmaxf(mx[0], x); mx[1] = fmaxf(mx[1], y); mx[2] = fmaxf(mx[2], z);
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
+            mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
+        }
+    }
+    if ((threadIdx.x & 31) == 0)
+        for (int a = 0; a < 3; ++a) { s[a][threadIdx.x >> 5] = mn[a]; s[3 + a][threadIdx.x >> 5] = mx[a]; }
+    __syncthreads();
+    if (threadIdx.x < 6) {
+        float v = s[threadIdx.x][0];
+        for (int w = 1; w < MB / 32; ++w) v = threadIdx.x < 3 ? fminf(v, s[threadIdx.x][w]) : fmaxf(v, s[threadIdx.x][w]);
+        part[6 * blockIdx.x + threadIdx.x] = v;
+    }
+}
+
+// one thread: L = 1.1 * largest extent, origin = centre - L / 2, h = L / R (h = 0 when no finite point / zero extent)
+__global__ void frame_kernel(const float* __restrict__ part, int nb, int R, double* __restrict__ fr) {
+    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+    for (int b = 0; b < nb; ++b)
+        for (int a = 0; a < 3; ++a) { mn[a] = fminf(mn[a], part[6 * b + a]); mx[a] = fmaxf(mx[a], part[6 * b + 3 + a]); }
+    double ext = 0.0;
+    const bool any = mn[0] <= mx[0];
+    if (any)
+        for (int a = 0; a < 3; ++a) ext = fmax(ext, __dsub_rn((double)mx[a], (double)mn[a]));
+    const double L = __dmul_rn(1.1, ext);
+    for (int a = 0; a < 3; ++a)
+        fr[FR_ORIGIN + a] = any ? __dsub_rn(__dmul_rn(__dadd_rn((double)mn[a], (double)mx[a]), 0.5), __dmul_rn(L, 0.5))
+                                : 0.0;
+    fr[FR_H] = __ddiv_rn(L, (double)R);
+    fr[FR_L] = L;
+    fr[FR_MEANB] = 0.0;
+    fr[FR_EXTENT] = ext;
+    fr[FR_R] = (double)R;
+}
+
+// per point: skip zero / non-finite normals (status[0]) and non-finite points (status[1]); otherwise every (node c,
+// axis a) of the dual cell adds q = llrint(w * n_a * 2^32) to B[c - e_a] and subtracts it from B[c + e_a]
+template <typename NT>
+__global__ void __launch_bounds__(MB) splat_kernel(const float* __restrict__ xyz, const NT* __restrict__ nrm, int64_t n,
+                                                   int R, const double* __restrict__ fr,
+                                                   unsigned long long* __restrict__ B, uint32_t* __restrict__ cell,
+                                                   int32_t* __restrict__ status) {
+    const int64_t i = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (i >= n) return;
+    cell[i] = CELL_NONE;
+    if (!finite3(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2])) { atomicAdd(&status[1], 1); return; }
+    if (!(fr[FR_H] > 0.0)) return;
+    const double nx = (double)nrm[3 * i], ny = (double)nrm[3 * i + 1], nz = (double)nrm[3 * i + 2];
+    const double s = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(nx, nx), __dmul_rn(ny, ny)), __dmul_rn(nz, nz)));
+    if (!(s > 0.0) || !isfinite(s)) { atomicAdd(&status[0], 1); return; }
+    const double nh[3] = {__ddiv_rn(nx, s), __ddiv_rn(ny, s), __ddiv_rn(nz, s)};
+    const PointCell c = point_cell(xyz, i, fr, R);
+    cell[i] = cell_id(c, R);
+    const int64_t stride[3] = {1, R, (int64_t)R * R};
+    for (int o = 0; o < 8; ++o) {
+        const double w = corner_weight(c, o);
+        const int cc[3] = {c.i0[0] + (o & 1), c.i0[1] + ((o >> 1) & 1), c.i0[2] + (o >> 2)};
+        const int64_t node = ((int64_t)cc[2] * R + cc[1]) * R + cc[0];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const long long q = llrint(__dmul_rn(__dmul_rn(w, nh[a]), TWO32));
+            if (q == 0) continue;
+            if (cc[a] > 0) atomicAdd(&B[node - stride[a]], (unsigned long long)q);
+            if (cc[a] < R - 1) atomicAdd(&B[node + stride[a]], (unsigned long long)(-q));
+        }
+    }
+}
+
+// exact int64 sum of B (wrap-around arithmetic: the total is exact whenever it fits int64)
+__global__ void __launch_bounds__(MB) sum_b_kernel(const long long* __restrict__ B, int64_t cells,
+                                                   unsigned long long* __restrict__ total) {
+    unsigned long long v = 0;
+    for (int64_t i = (int64_t)blockIdx.x * MB + threadIdx.x; i < cells; i += (int64_t)gridDim.x * MB)
+        v += (unsigned long long)B[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(total, v);
+}
+
+__global__ void mean_b_kernel(const unsigned long long* __restrict__ total, int64_t cells, double* __restrict__ fr) {
+    fr[FR_MEANB] = __ddiv_rn((double)(long long)*total, (double)cells);
+}
+
+// ---- multigrid ---------------------------------------------------------------------------------------------------
+// right-hand side of a level: the finest reads B, the coarser ones their float grid
+struct Rhs {
+    const long long* B;
+    const float* f;
+    const double* fr;
+    __device__ __forceinline__ float operator()(int64_t i) const {
+        if (f) return f[i];
+        return (float)__dmul_rn(__dsub_rn((double)B[i], fr[FR_MEANB]), __dmul_rn(fr[FR_H], 0x1p-33));
+    }
+};
+
+// sum of the in-grid neighbours of (i, j, k) and their count (a mirrored ghost equals the cell itself)
+template <typename T>
+__device__ __forceinline__ T neighbour_sum(const float* __restrict__ chi, int n, int i, int j, int k, int64_t c, int& cnt) {
+    const int64_t nn = (int64_t)n * n;
+    T s = 0;
+    cnt = 0;
+    if (i > 0) { s += (T)chi[c - 1]; ++cnt; }
+    if (i < n - 1) { s += (T)chi[c + 1]; ++cnt; }
+    if (j > 0) { s += (T)chi[c - n]; ++cnt; }
+    if (j < n - 1) { s += (T)chi[c + n]; ++cnt; }
+    if (k > 0) { s += (T)chi[c - nn]; ++cnt; }
+    if (k < n - 1) { s += (T)chi[c + nn]; ++cnt; }
+    return s;
+}
+
+// b - (sum of neighbours - 6 chi) with mirrored ghosts = b - (sum of in-grid neighbours - count * chi), in float64
+__device__ __forceinline__ double residual(const float* __restrict__ chi, const Rhs& rhs, int n, int i, int j, int k) {
+    const int64_t c = ((int64_t)k * n + j) * n + i;
+    int cnt;
+    const double s = neighbour_sum<double>(chi, n, i, j, k, c, cnt);
+    return (double)rhs(c) - (s - (double)cnt * (double)chi[c]);
+}
+
+// one colour of a red-black Gauss-Seidel sweep: cells with (i + j + k) % 2 == colour
+__global__ void __launch_bounds__(MB) rb_smooth_kernel(float* __restrict__ chi, Rhs rhs, int n, int colour) {
+    const int64_t t = (int64_t)blockIdx.x * MB + threadIdx.x;
+    const int half = n >> 1;
+    if (t >= (int64_t)n * n * half) return;
+    const int64_t row = t / half;
+    const int j = (int)(row % n), k = (int)(row / n);
+    const int i = 2 * (int)(t % half) + ((j + k + colour) & 1);
+    const int64_t c = ((int64_t)k * n + j) * n + i;
+    int cnt;
+    const float s = neighbour_sum<float>(chi, n, i, j, k, c, cnt);
+    chi[c] = (s - rhs(c)) / (float)cnt;
+}
+
+// coarse right-hand side = 4 x the mean of the 8 fine residuals (the stencil is not scaled by 1/h^2)
+__global__ void __launch_bounds__(MB) restrict_kernel(const float* __restrict__ chi, Rhs rhs, int n,
+                                                      float* __restrict__ rc) {
+    const int nc = n >> 1;
+    const int64_t t = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (t >= (int64_t)nc * nc * nc) return;
+    const int I = (int)(t % nc), J = (int)((t / nc) % nc), K = (int)(t / ((int64_t)nc * nc));
+    double s = 0.0;
+    for (int o = 0; o < 8; ++o) s += residual(chi, rhs, n, 2 * I + (o & 1), 2 * J + ((o >> 1) & 1), 2 * K + (o >> 2));
+    rc[t] = (float)(0.5 * s);
+}
+
+// fine += trilinear (cell-centred: 3/4, 1/4 per axis, clamped at the faces) interpolation of the coarse correction
+__global__ void __launch_bounds__(MB) prolong_kernel(float* __restrict__ chi, int n, const float* __restrict__ ec) {
+    const int64_t t = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (t >= (int64_t)n * n * n) return;
+    const int nc = n >> 1;
+    const int p[3] = {(int)(t % n), (int)((t / n) % n), (int)(t / ((int64_t)n * n))};
+    int lo[3], hi[3];
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = p[a] >> 1;
+        const int q = lo[a] + ((p[a] & 1) ? 1 : -1);
+        hi[a] = q < 0 ? 0 : (q > nc - 1 ? nc - 1 : q);
+    }
+    float e = 0.f;
+    for (int o = 0; o < 8; ++o) {
+        const int x = (o & 1) ? hi[0] : lo[0], y = (o & 2) ? hi[1] : lo[1], z = (o & 4) ? hi[2] : lo[2];
+        const float w = ((o & 1) ? 0.25f : 0.75f) * ((o & 2) ? 0.25f : 0.75f) * ((o & 4) ? 0.25f : 0.75f);
+        e += w * ec[((int64_t)z * nc + y) * nc + x];
+    }
+    chi[t] += e;
+}
+
+// the 4^3 coarsest level in one CTA: right-hand side made mean-free, then red-black sweeps from the current chi
+__global__ void __launch_bounds__(64) coarse_kernel(float* __restrict__ chi, Rhs rhs) {
+    __shared__ float x[64], b[64];
+    __shared__ float mean;
+    const int t = threadIdx.x;
+    x[t] = chi[t];
+    b[t] = rhs(t);
+    __syncthreads();
+    if (t == 0) {
+        double s = 0.0;
+        for (int q = 0; q < 64; ++q) s += b[q];
+        mean = (float)(s / 64.0);
+    }
+    __syncthreads();
+    b[t] -= mean;
+    const int i = t & 3, j = (t >> 2) & 3, k = t >> 4;
+    __syncthreads();
+    for (int it = 0; it < COARSE_SWEEPS; ++it) {
+        for (int colour = 0; colour < 2; ++colour) {
+            if (((i + j + k) & 1) == colour) {
+                int cnt;
+                const float s = neighbour_sum<float>(x, 4, i, j, k, t, cnt);
+                x[t] = (s - b[t]) / (float)cnt;
+            }
+            __syncthreads();
+        }
+    }
+    chi[t] = x[t];
+}
+
+// MODE 0: partial sums of r^2 at the finest level; 1: of b^2; 2: of chi
+template <int MODE>
+__global__ void __launch_bounds__(MB) grid_partial_kernel(const float* __restrict__ chi, Rhs rhs, int n,
+                                                          double* __restrict__ partial) {
+    __shared__ double s_w[MB / 32];
+    const int64_t cells = (int64_t)n * n * n;
+    double v = 0.0;
+    for (int64_t t = (int64_t)blockIdx.x * MB + threadIdx.x; t < cells; t += (int64_t)RED_BLOCKS * MB) {
+        if (MODE == 0) {
+            const double r = residual(chi, rhs, n, (int)(t % n), (int)((t / n) % n), (int)(t / ((int64_t)n * n)));
+            v = __dadd_rn(v, __dmul_rn(r, r));
+        } else if (MODE == 1) {
+            const double b = (double)rhs(t);
+            v = __dadd_rn(v, __dmul_rn(b, b));
+        } else {
+            v = __dadd_rn(v, (double)chi[t]);
+        }
+    }
+    const double tot = block_sum(v, s_w);
+    if (threadIdx.x == 0) partial[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(MB) shift_kernel(float* __restrict__ chi, int64_t cells, const double* __restrict__ mean) {
+    const int64_t t = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (t < cells) chi[t] = (float)__dsub_rn((double)chi[t], *mean);
+}
+
+// iso: partial sums of (trilinear chi at the point) and of the count over the splatted points
+__global__ void __launch_bounds__(MB) iso_partial_kernel(const float* __restrict__ xyz, const uint32_t* __restrict__ cell,
+                                                         int64_t n, const double* __restrict__ fr, int R,
+                                                         const float* __restrict__ chi, double* __restrict__ partial) {
+    __shared__ double s_w[MB / 32];
+    double v = 0.0, cnt = 0.0;
+    for (int64_t i = (int64_t)blockIdx.x * MB + threadIdx.x; i < n; i += (int64_t)RED_BLOCKS * MB) {
+        if (cell[i] == CELL_NONE) continue;
+        const PointCell c = point_cell(xyz, i, fr, R);
+        double x = 0.0;
+        for (int o = 0; o < 8; ++o) {
+            const int64_t node = ((int64_t)(c.i0[2] + (o >> 2)) * R + c.i0[1] + ((o >> 1) & 1)) * R + c.i0[0] + (o & 1);
+            x = __dadd_rn(x, __dmul_rn(corner_weight(c, o), (double)chi[node]));
+        }
+        v = __dadd_rn(v, x);
+        cnt += 1.0;
+    }
+    const double tv = block_sum(v, s_w);
+    __syncthreads();
+    const double tc = block_sum(cnt, s_w);
+    if (threadIdx.x == 0) { partial[blockIdx.x] = tv; partial[RED_BLOCKS + blockIdx.x] = tc; }
+}
+
+__global__ void iso_div_kernel(double* __restrict__ iso2) {
+    iso2[1] = iso2[2] > 0.0 ? __ddiv_rn(iso2[1], iso2[2]) : 0.0;
+}
+
+// ---- marching tetrahedra --------------------------------------------------------------------------------------------
+// inside / in-grid bits of the 8 corners P + {0,1}^3 (bit o: x = o & 1, y = o >> 1 & 1, z = o >> 2)
+struct Cube {
+    uint32_t inside, valid;
+};
+
+__device__ __forceinline__ Cube load_cube(const float* __restrict__ chi, int R, int i, int j, int k, double iso) {
+    Cube c{0u, 0u};
+#pragma unroll
+    for (int o = 0; o < 8; ++o) {
+        const int x = i + (o & 1), y = j + ((o >> 1) & 1), z = k + (o >> 2);
+        if (x < R && y < R && z < R) {
+            c.valid |= 1u << o;
+            if ((double)chi[((int64_t)z * R + y) * R + x] < iso) c.inside |= 1u << o;
+        }
+    }
+    return c;
+}
+
+// bit d (1..7) set iff the lattice edge (P, P + d) exists and crosses the surface
+__device__ __forceinline__ uint32_t cross_mask(Cube c) {
+    uint32_t m = 0;
+    const uint32_t in0 = c.inside & 1u;
+#pragma unroll
+    for (int d = 1; d < 8; ++d)
+        if (((c.valid >> d) & 1u) && ((c.inside >> d) & 1u) != in0) m |= 1u << d;
+    return m;
+}
+
+// corner (bitmask) q of Kuhn tetrahedron p: 0, e_a, e_a + e_b, 1 for the p-th axis permutation (a, b, c) in
+// lexicographic order
+__device__ __forceinline__ int tet_corner(int p, int q) {
+    const int a = p >> 1;
+    const int r0 = a == 0 ? 1 : 0, r1 = a == 2 ? 1 : 2;
+    const int b = (p & 1) ? r1 : r0;
+    return q == 0 ? 0 : (q == 1 ? 1 << a : (q == 2 ? (1 << a) | (1 << b) : 7));
+}
+
+__device__ __forceinline__ int tet_triangle_count(int p, uint32_t inside) {
+    int ni = 0;
+    for (int q = 0; q < 4; ++q) ni += (inside >> tet_corner(p, q)) & 1;
+    return ni == 2 ? 2 : (ni == 1 || ni == 3 ? 1 : 0);
+}
+
+__device__ __forceinline__ int cube_triangle_count(uint32_t inside) {
+    int t = 0;
+    for (int p = 0; p < 6; ++p) t += tet_triangle_count(p, inside);
+    return t;
+}
+
+// The triangles of tetrahedron p: edges as (lower corner, upper corner) bitmask pairs.  One inside corner I or one
+// outside corner O: one triangle over the three edges of that corner; two and two (inside I0 < I1, outside O0 < O1,
+// tetrahedron-local order): the quad I0O0, I0O1, I1O1, I1O0 split along I0O0-I1O1.  Each triangle is wound
+// counter-clockwise seen from the outside (chi >= iso): the normal of the triangle of the edge midpoints must point from
+// an inside to an outside corner, else its last two edges swap.  Integer arithmetic (doubled midpoints): exact.
+__device__ __forceinline__ int tet_triangles(int p, uint32_t inside, int (&tri)[2][3][2]) {
+    int v[4], I[4], O[4], ni = 0, no = 0;
+    for (int q = 0; q < 4; ++q) {
+        v[q] = tet_corner(p, q);
+        if ((inside >> v[q]) & 1) I[ni++] = q; else O[no++] = q;
+    }
+    int e[2][3][2], nt;  // tetrahedron-local vertex pairs
+    if (ni == 1 || ni == 3) {
+        const int apex = ni == 1 ? I[0] : O[0];
+        const int* other = ni == 1 ? O : I;
+        for (int s = 0; s < 3; ++s) { e[0][s][0] = apex; e[0][s][1] = other[s]; }
+        nt = 1;
+    } else if (ni == 2) {
+        const int q[2][3][2] = {{{I[0], O[0]}, {I[0], O[1]}, {I[1], O[1]}}, {{I[0], O[0]}, {I[1], O[1]}, {I[1], O[0]}}};
+        for (int t = 0; t < 2; ++t)
+            for (int s = 0; s < 3; ++s) { e[t][s][0] = q[t][s][0]; e[t][s][1] = q[t][s][1]; }
+        nt = 2;
+    } else {
+        return 0;
+    }
+    const int din[3] = {v[O[0]] & 1, (v[O[0]] >> 1) & 1, v[O[0]] >> 2};
+    const int dio[3] = {din[0] - (v[I[0]] & 1), din[1] - ((v[I[0]] >> 1) & 1), din[2] - (v[I[0]] >> 2)};
+    for (int t = 0; t < nt; ++t) {
+        int M[3][3];
+        for (int s = 0; s < 3; ++s) {
+            const int a = v[e[t][s][0]], b = v[e[t][s][1]];
+            for (int x = 0; x < 3; ++x) M[s][x] = ((a >> x) & 1) + ((b >> x) & 1);
+        }
+        const int u[3] = {M[1][0] - M[0][0], M[1][1] - M[0][1], M[1][2] - M[0][2]};
+        const int w[3] = {M[2][0] - M[0][0], M[2][1] - M[0][1], M[2][2] - M[0][2]};
+        const int N[3] = {u[1] * w[2] - u[2] * w[1], u[2] * w[0] - u[0] * w[2], u[0] * w[1] - u[1] * w[0]};
+        const bool flip = N[0] * dio[0] + N[1] * dio[1] + N[2] * dio[2] < 0;
+        for (int s = 0; s < 3; ++s) {
+            const int src = flip && s > 0 ? 3 - s : s;
+            const int a = v[e[t][src][0]], b = v[e[t][src][1]];
+            // corners of a tetrahedron are nested bitmasks: the smaller one is the lower end of the lattice edge
+            tri[t][s][0] = a < b ? a : b;
+            tri[t][s][1] = a < b ? b : a;
+        }
+    }
+    return nt;
+}
+
+__device__ __forceinline__ void node_ijk(int64_t node, int R, int& i, int& j, int& k) {
+    i = (int)(node % R);
+    j = (int)((node / R) % R);
+    k = (int)(node / ((int64_t)R * R));
+}
+
+// per CTA (NODES_PER_CTA consecutive nodes): crossed edges and triangles of the cubes whose lowest corner they are
+__global__ void __launch_bounds__(MB) mt_count_kernel(const float* __restrict__ chi, int R, const double* __restrict__ iso2,
+                                                      long long* __restrict__ vblk, long long* __restrict__ tblk) {
+    __shared__ double s_w[MB / 32];
+    const double iso = iso2[1];
+    const int64_t cells = (int64_t)R * R * R;
+    int nv = 0, nt = 0;
+    for (int q = 0; q < NPT; ++q) {
+        const int64_t node = (int64_t)blockIdx.x * NODES_PER_CTA + threadIdx.x * NPT + q;
+        if (node >= cells) break;
+        int i, j, k;
+        node_ijk(node, R, i, j, k);
+        const Cube c = load_cube(chi, R, i, j, k, iso);
+        nv += __popc(cross_mask(c));
+        if (c.valid == 0xFFu) nt += cube_triangle_count(c.inside);
+    }
+    const double sv = block_sum((double)nv, s_w);
+    __syncthreads();
+    const double st = block_sum((double)nt, s_w);
+    if (threadIdx.x == 0) { vblk[blockIdx.x] = (long long)sv; tblk[blockIdx.x] = (long long)st; }
+}
+
+__global__ void totals_kernel(const long long* __restrict__ voff, const long long* __restrict__ toff, int64_t nb,
+                              long long* __restrict__ counts) {
+    counts[0] = voff[nb];
+    counts[1] = toff[nb];
+}
+
+// vertices in ascending edge key (node * 8 + d); node_base[node] = index of the node's first vertex, node_mask[node] =
+// its crossed-edge mask (both read by the triangle pass)
+__global__ void __launch_bounds__(MB) mt_vertex_kernel(const float* __restrict__ chi, int R, const double* __restrict__ fr,
+                                                       const double* __restrict__ iso2, const long long* __restrict__ voff,
+                                                       int32_t* __restrict__ node_base, uint8_t* __restrict__ node_mask,
+                                                       long long* __restrict__ vkey, double* __restrict__ vt,
+                                                       double* __restrict__ vpos) {
+    typedef cub::BlockScan<int, MB> Scan;
+    __shared__ typename Scan::TempStorage tmp;
+    const double iso = iso2[1];
+    const int64_t cells = (int64_t)R * R * R;
+    uint32_t m[NPT];
+    int nv = 0;
+    for (int q = 0; q < NPT; ++q) {
+        const int64_t node = (int64_t)blockIdx.x * NODES_PER_CTA + threadIdx.x * NPT + q;
+        m[q] = 0;
+        if (node >= cells) continue;
+        int i, j, k;
+        node_ijk(node, R, i, j, k);
+        m[q] = cross_mask(load_cube(chi, R, i, j, k, iso));
+        nv += __popc(m[q]);
+    }
+    int pre;
+    Scan(tmp).ExclusiveSum(nv, pre);
+    long long cur = voff[blockIdx.x] + pre;
+    for (int q = 0; q < NPT; ++q) {
+        const int64_t node = (int64_t)blockIdx.x * NODES_PER_CTA + threadIdx.x * NPT + q;
+        if (node >= cells) break;
+        node_base[node] = (int32_t)cur;
+        node_mask[node] = (uint8_t)m[q];
+        if (!m[q]) continue;
+        int i, j, k;
+        node_ijk(node, R, i, j, k);
+        const double ca = (double)chi[node];
+        const double pa[3] = {node_coord(fr, 0, i), node_coord(fr, 1, j), node_coord(fr, 2, k)};
+        for (int d = 1; d < 8; ++d) {
+            if (!((m[q] >> d) & 1u)) continue;
+            const int ib = i + (d & 1), jb = j + ((d >> 1) & 1), kb = k + (d >> 2);
+            const double cb = (double)chi[((int64_t)kb * R + jb) * R + ib];
+            const double t = __ddiv_rn(__dsub_rn(iso, ca), __dsub_rn(cb, ca));
+            const double pb[3] = {node_coord(fr, 0, ib), node_coord(fr, 1, jb), node_coord(fr, 2, kb)};
+            vkey[cur] = node * 8 + d;
+            vt[cur] = t;
+            for (int a = 0; a < 3; ++a) vpos[3 * cur + a] = __dadd_rn(pa[a], __dmul_rn(t, __dsub_rn(pb[a], pa[a])));
+            ++cur;
+        }
+    }
+}
+
+// triangles in ascending (cube, tetrahedron, triangle)
+__global__ void __launch_bounds__(MB) mt_triangle_kernel(const float* __restrict__ chi, int R,
+                                                         const double* __restrict__ iso2, const long long* __restrict__ toff,
+                                                         const int32_t* __restrict__ node_base,
+                                                         const uint8_t* __restrict__ node_mask,
+                                                         int32_t* __restrict__ faces) {
+    typedef cub::BlockScan<int, MB> Scan;
+    __shared__ typename Scan::TempStorage tmp;
+    const double iso = iso2[1];
+    const int64_t cells = (int64_t)R * R * R;
+    uint32_t ins[NPT];
+    int nt = 0;
+    for (int q = 0; q < NPT; ++q) {
+        const int64_t node = (int64_t)blockIdx.x * NODES_PER_CTA + threadIdx.x * NPT + q;
+        ins[q] = 0xFFu;  // no triangles
+        if (node >= cells) continue;
+        int i, j, k;
+        node_ijk(node, R, i, j, k);
+        const Cube c = load_cube(chi, R, i, j, k, iso);
+        if (c.valid != 0xFFu) continue;
+        ins[q] = c.inside;
+        nt += cube_triangle_count(c.inside);
+    }
+    int pre;
+    Scan(tmp).ExclusiveSum(nt, pre);
+    long long cur = toff[blockIdx.x] + pre;
+    for (int q = 0; q < NPT; ++q) {
+        if (ins[q] == 0xFFu || ins[q] == 0u) continue;
+        const int64_t node = (int64_t)blockIdx.x * NODES_PER_CTA + threadIdx.x * NPT + q;
+        for (int p = 0; p < 6; ++p) {
+            int tri[2][3][2];
+            const int n = tet_triangles(p, ins[q], tri);
+            for (int t = 0; t < n; ++t, ++cur) {
+                for (int s = 0; s < 3; ++s) {
+                    const int lo = tri[t][s][0], d = tri[t][s][1] ^ lo;
+                    const int64_t pn = node + (lo & 1) + (int64_t)((lo >> 1) & 1) * R + (int64_t)(lo >> 2) * R * R;
+                    faces[3 * cur + s] = node_base[pn] + __popc(node_mask[pn] & ((1u << d) - 1u));
+                }
+            }
+        }
+    }
+}
+
+// ---- density and colour gathers ------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(MB) iota_kernel(uint32_t* __restrict__ v, int64_t n) {
+    const int64_t i = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (i < n) v[i] = (uint32_t)i;
+}
+
+// first sorted position of every non-empty dual cell (the others stay -1)
+__global__ void __launch_bounds__(MB) cell_start_kernel(const uint32_t* __restrict__ sk, int64_t n,
+                                                        int32_t* __restrict__ start) {
+    const int64_t j = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (j >= n) return;
+    const uint32_t key = sk[j];
+    if (key != CELL_NONE && (j == 0 || sk[j - 1] != key)) start[key] = (int32_t)j;
+}
+
+// W = sum of w, C = sum of w * colour over the points of the 8 dual cells around the node: cells in ascending index,
+// points in ascending input index, sequential float64
+__device__ __forceinline__ void node_sums(int x, int y, int z, int R, const uint32_t* __restrict__ sk,
+                                          const uint32_t* __restrict__ sidx, int64_t n, const int32_t* __restrict__ start,
+                                          const float* __restrict__ xyz, const int32_t* __restrict__ col,
+                                          const double* __restrict__ fr, double& W, double (&C)[3]) {
+    W = 0.0;
+    C[0] = C[1] = C[2] = 0.0;
+    for (int o = 7; o >= 0; --o) {
+        const int cx = x - (o & 1), cy = y - ((o >> 1) & 1), cz = z - (o >> 2);
+        if (cx < 0 || cy < 0 || cz < 0 || cx > R - 2 || cy > R - 2 || cz > R - 2) continue;
+        const uint32_t id = ((uint32_t)cz * (uint32_t)(R - 1) + (uint32_t)cy) * (uint32_t)(R - 1) + (uint32_t)cx;
+        int64_t j = start[id];
+        if (j < 0) continue;
+        for (; j < n && sk[j] == id; ++j) {
+            const uint32_t pi = sidx[j];
+            const double w = corner_weight(point_cell(xyz, pi, fr, R), o);
+            W = __dadd_rn(W, w);
+            if (col)
+                for (int a = 0; a < 3; ++a) C[a] = __dadd_rn(C[a], __dmul_rn(w, (double)col[3 * (int64_t)pi + a]));
+        }
+    }
+}
+
+__global__ void __launch_bounds__(MB) gather_kernel(const long long* __restrict__ vkey, const double* __restrict__ vt,
+                                                    int64_t m, int R, const uint32_t* __restrict__ sk,
+                                                    const uint32_t* __restrict__ sidx, int64_t n,
+                                                    const int32_t* __restrict__ start, const float* __restrict__ xyz,
+                                                    const int32_t* __restrict__ col, const double* __restrict__ fr,
+                                                    double* __restrict__ dens, uint8_t* __restrict__ vcol) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m) return;
+    const long long key = vkey[v];
+    const int64_t node = key >> 3;
+    const int d = (int)(key & 7);
+    int i, j, k;
+    node_ijk(node, R, i, j, k);
+    double Wa, Wb, Ca[3], Cb[3];
+    node_sums(i, j, k, R, sk, sidx, n, start, xyz, col, fr, Wa, Ca);
+    node_sums(i + (d & 1), j + ((d >> 1) & 1), k + (d >> 2), R, sk, sidx, n, start, xyz, col, fr, Wb, Cb);
+    const double t = vt[v], s = __dsub_rn(1.0, t);
+    const double D = __dadd_rn(__dmul_rn(s, Wa), __dmul_rn(t, Wb));
+    dens[v] = D;
+    if (!vcol) return;
+    for (int a = 0; a < 3; ++a) {
+        double c = 0.0;
+        if (D > 0.0) {
+            c = floor(__dadd_rn(__ddiv_rn(__dadd_rn(__dmul_rn(s, Ca[a]), __dmul_rn(t, Cb[a])), D), 0.5));
+            c = fmin(fmax(c, 0.0), 255.0);
+        }
+        vcol[3 * v + a] = (uint8_t)c;
+    }
+}
+
+// ---- density trim -------------------------------------------------------------------------------------------------
+// numpy's default (linear) quantile q = 0.1 of the sorted densities: virtual index (m - 1) * q, then
+// a + (b - a) * g, or b - (b - a) * (1 - g) when g >= 0.5
+__global__ void quantile_kernel(const double* __restrict__ sorted, int64_t m, double* __restrict__ thr) {
+    const double vi = __dmul_rn((double)(m - 1), 0.1);
+    int64_t lo, hi;
+    double g;
+    if (vi >= (double)(m - 1)) {
+        lo = hi = m - 1;
+        g = 0.0;
+    } else {
+        const double fl = floor(vi);
+        lo = (int64_t)fl;
+        hi = lo + 1;
+        g = __dsub_rn(vi, fl);
+    }
+    const double a = sorted[lo], b = sorted[hi], diff = __dsub_rn(b, a);
+    *thr = g >= 0.5 ? __dsub_rn(b, __dmul_rn(diff, __dsub_rn(1.0, g))) : __dadd_rn(a, __dmul_rn(diff, g));
+}
+
+__global__ void __launch_bounds__(MB) keep_kernel(const double* __restrict__ dens, int64_t m,
+                                                  const double* __restrict__ thr, uint8_t* __restrict__ keep,
+                                                  int32_t* __restrict__ flag) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m) return;
+    const int k = dens[v] < *thr ? 0 : 1;
+    keep[v] = (uint8_t)k;
+    flag[v] = k;
+}
+
+__global__ void __launch_bounds__(MB) tri_flag_kernel(const int32_t* __restrict__ faces, int64_t t,
+                                                      const uint8_t* __restrict__ keep, int32_t* __restrict__ flag) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t) return;
+    flag[f] = keep[faces[3 * f]] & keep[faces[3 * f + 1]] & keep[faces[3 * f + 2]];
+}
+
+__global__ void __launch_bounds__(MB) compact_vertices_kernel(const uint8_t* __restrict__ keep,
+                                                              const int32_t* __restrict__ vmap, int64_t m,
+                                                              const double* __restrict__ dens,
+                                                              const double* __restrict__ vpos,
+                                                              const uint8_t* __restrict__ vcol, double* __restrict__ dens_o,
+                                                              double* __restrict__ vpos_o, uint8_t* __restrict__ vcol_o) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m || !keep[v]) return;
+    const int64_t o = vmap[v];
+    dens_o[o] = dens[v];
+    for (int a = 0; a < 3; ++a) vpos_o[3 * o + a] = vpos[3 * v + a];
+    if (vcol)
+        for (int a = 0; a < 3; ++a) vcol_o[3 * o + a] = vcol[3 * v + a];
+}
+
+__global__ void __launch_bounds__(MB) compact_faces_kernel(const int32_t* __restrict__ faces, const int32_t* __restrict__ flag,
+                                                           const int32_t* __restrict__ fmap, int64_t t,
+                                                           const int32_t* __restrict__ vmap, int32_t* __restrict__ faces_o) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t || !flag[f]) return;
+    const int64_t o = fmap[f];
+    for (int s = 0; s < 3; ++s) faces_o[3 * o + s] = vmap[faces[3 * f + s]];
+}
+
+__global__ void trim_counts_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ map, int64_t m,
+                                   const int32_t* __restrict__ tflag, const int32_t* __restrict__ tmap, int64_t t,
+                                   long long* __restrict__ counts) {
+    counts[0] = m ? (long long)map[m - 1] + flag[m - 1] : 0;
+    counts[1] = t ? (long long)tmap[t - 1] + tflag[t - 1] : 0;
+}
+
+// ---- one-ring / incidence lists, smoothing, normals ----------------------------------------------------------------
+// directed one-ring edges (u << 32 | v), both directions of every triangle edge
+__global__ void __launch_bounds__(MB) ring_keys_kernel(const int32_t* __restrict__ faces, int64_t t,
+                                                       unsigned long long* __restrict__ keys) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t) return;
+    for (int s = 0; s < 3; ++s) {
+        const unsigned long long a = (uint32_t)faces[3 * f + s], b = (uint32_t)faces[3 * f + (s + 1) % 3];
+        keys[6 * f + 2 * s] = a << 32 | b;
+        keys[6 * f + 2 * s + 1] = b << 32 | a;
+    }
+}
+
+// incident triangles (v << 32 | triangle)
+__global__ void __launch_bounds__(MB) incidence_keys_kernel(const int32_t* __restrict__ faces, int64_t t,
+                                                            unsigned long long* __restrict__ keys) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t) return;
+    for (int s = 0; s < 3; ++s) keys[3 * f + s] = (unsigned long long)(uint32_t)faces[3 * f + s] << 32 | (uint64_t)f;
+}
+
+// row[v] = first sorted key with high word >= v, for v = 0..m
+__global__ void __launch_bounds__(MB) row_kernel(const unsigned long long* __restrict__ keys, int64_t e, int64_t m,
+                                                 int32_t* __restrict__ row) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v > m) return;
+    const unsigned long long K = (unsigned long long)v << 32;
+    int64_t lo = 0, hi = e;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (keys[mid] < K) lo = mid + 1; else hi = mid;
+    }
+    row[v] = (int32_t)lo;
+}
+
+// one Jacobi step, lambda = 1/2: v + (sum w_j v_j / sum w_j - v) / 2, w_j = 1 / (|v - v_j| + 1e-12), distinct
+// neighbours in ascending index
+__global__ void __launch_bounds__(MB) smooth_kernel(const double* __restrict__ p, int64_t m,
+                                                    const unsigned long long* __restrict__ keys,
+                                                    const int32_t* __restrict__ row, double* __restrict__ q) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m) return;
+    const double x[3] = {p[3 * v], p[3 * v + 1], p[3 * v + 2]};
+    double sw = 0.0, s[3] = {0.0, 0.0, 0.0};
+    const int64_t r0 = row[v], r1 = row[v + 1];
+    for (int64_t j = r0; j < r1; ++j) {
+        if (j > r0 && keys[j] == keys[j - 1]) continue;
+        const int64_t u = (int64_t)(keys[j] & 0xFFFFFFFFull);
+        const double y[3] = {p[3 * u], p[3 * u + 1], p[3 * u + 2]};
+        const double dx = __dsub_rn(x[0], y[0]), dy = __dsub_rn(x[1], y[1]), dz = __dsub_rn(x[2], y[2]);
+        const double dist = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+        const double w = __ddiv_rn(1.0, __dadd_rn(dist, 1e-12));
+        sw = __dadd_rn(sw, w);
+        for (int a = 0; a < 3; ++a) s[a] = __dadd_rn(s[a], __dmul_rn(w, y[a]));
+    }
+    for (int a = 0; a < 3; ++a)
+        q[3 * v + a] = r1 > r0 ? __dadd_rn(x[a], __dmul_rn(0.5, __dsub_rn(__ddiv_rn(s[a], sw), x[a]))) : x[a];
+}
+
+// normal = normalised sum of cross(p1 - p0, p2 - p0) over the incident triangles in ascending order (zero stays zero)
+__global__ void __launch_bounds__(MB) normals_kernel(const double* __restrict__ p, int64_t m,
+                                                     const int32_t* __restrict__ faces,
+                                                     const unsigned long long* __restrict__ keys,
+                                                     const int32_t* __restrict__ row, float* __restrict__ vout,
+                                                     float* __restrict__ nout) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m) return;
+    double n[3] = {0.0, 0.0, 0.0};
+    for (int64_t j = row[v]; j < row[v + 1]; ++j) {
+        const int64_t f = (int64_t)(keys[j] & 0xFFFFFFFFull);
+        const int64_t a = faces[3 * f], b = faces[3 * f + 1], c = faces[3 * f + 2];
+        double u[3], w[3];
+        for (int x = 0; x < 3; ++x) { u[x] = __dsub_rn(p[3 * b + x], p[3 * a + x]); w[x] = __dsub_rn(p[3 * c + x], p[3 * a + x]); }
+        n[0] = __dadd_rn(n[0], __dsub_rn(__dmul_rn(u[1], w[2]), __dmul_rn(u[2], w[1])));
+        n[1] = __dadd_rn(n[1], __dsub_rn(__dmul_rn(u[2], w[0]), __dmul_rn(u[0], w[2])));
+        n[2] = __dadd_rn(n[2], __dsub_rn(__dmul_rn(u[0], w[1]), __dmul_rn(u[1], w[0])));
+    }
+    const double s = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(n[0], n[0]), __dmul_rn(n[1], n[1])), __dmul_rn(n[2], n[2])));
+    for (int x = 0; x < 3; ++x) {
+        nout[3 * v + x] = s > 0.0 ? (float)__ddiv_rn(n[x], s) : 0.f;
+        vout[3 * v + x] = (float)p[3 * v + x];
+    }
+}
+
+unsigned grid_of(int64_t n) { return (unsigned)((n + MB - 1) / MB); }
+
+int64_t cells_of(int depth) { return (int64_t)1 << (3 * depth); }
+
+bool depth_ok(int depth) { return depth >= 2 && depth <= G2PC_MESH_DEPTH_MAX; }
+
+// ---- workspace layouts ----------------------------------------------------------------------------------------------
+struct SplatLayout {
+    size_t part, total, bytes;
+    int nb;
+};
+SplatLayout splat_layout(int64_t n) {
+    SplatLayout l;
+    l.nb = (int)((n + BOX_PER_CTA - 1) / BOX_PER_CTA);
+    size_t o = 0;
+    l.part = o; o += align256((size_t)(l.nb > 0 ? l.nb : 1) * 6 * sizeof(float));
+    l.total = o; o += align256(8);
+    l.bytes = o;
+    return l;
+}
+
+struct SolveLayout {
+    size_t chi[G2PC_MESH_DEPTH_MAX], rhs[G2PC_MESH_DEPTH_MAX], partial, bytes;
+};
+SolveLayout solve_layout(int depth) {
+    SolveLayout l;
+    size_t o = 0;
+    for (int lv = 1; lv <= depth - 2; ++lv) {
+        const size_t c = (size_t)cells_of(depth - lv) * sizeof(float);
+        l.chi[lv] = o; o += align256(c);
+        l.rhs[lv] = o; o += align256(c);
+    }
+    l.partial = o; o += align256(2 * RED_BLOCKS * sizeof(double));
+    l.bytes = o;
+    return l;
+}
+
+struct ExtractLayout {
+    size_t vblk, tblk, voff, toff, tmp, tmp_bytes, bytes;
+    int64_t nb;
+};
+ExtractLayout extract_layout(int depth) {
+    ExtractLayout l;
+    l.nb = (cells_of(depth) + NODES_PER_CTA - 1) / NODES_PER_CTA;
+    const size_t a = align256((size_t)(l.nb + 1) * 8);
+    size_t scan_b = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const long long*)nullptr, (long long*)nullptr, (int)(l.nb + 1));
+    size_t o = 0;
+    l.vblk = o; o += a;
+    l.tblk = o; o += a;
+    l.voff = o; o += a;
+    l.toff = o; o += a;
+    l.tmp = o; l.tmp_bytes = align256(scan_b); o += l.tmp_bytes;
+    l.bytes = o;
+    return l;
+}
+
+struct GatherLayout {
+    size_t keys_a, keys_b, idx_a, idx_b, tmp, tmp_bytes, bytes;
+};
+GatherLayout gather_layout(int64_t n) {
+    GatherLayout l;
+    size_t sort_b = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, 0, 31);
+    const size_t a = align256((size_t)n * 4);
+    size_t o = 0;
+    l.keys_a = o; o += a;
+    l.keys_b = o; o += a;
+    l.idx_a = o; o += a;
+    l.idx_b = o; o += a;
+    l.tmp = o; l.tmp_bytes = align256(sort_b); o += l.tmp_bytes;
+    l.bytes = o;
+    return l;
+}
+
+struct TrimLayout {
+    size_t sorted, thr, vflag, vmap, tflag, tmap, tmp, tmp_bytes, bytes;
+};
+TrimLayout trim_layout(int64_t m, int64_t t) {
+    TrimLayout l;
+    size_t sort_b = 0, scan_v = 0, scan_t = 0;
+    cub::DeviceRadixSort::SortKeys(nullptr, sort_b, (const double*)nullptr, (double*)nullptr, (int)m);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_v, (const int32_t*)nullptr, (int32_t*)nullptr, (int)m);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_t, (const int32_t*)nullptr, (int32_t*)nullptr, (int)t);
+    size_t tb = sort_b > scan_v ? sort_b : scan_v;
+    tb = tb > scan_t ? tb : scan_t;
+    size_t o = 0;
+    l.sorted = o; o += align256((size_t)m * 8);
+    l.thr = o; o += align256(8);
+    l.vflag = o; o += align256((size_t)m * 4);
+    l.vmap = o; o += align256((size_t)m * 4);
+    l.tflag = o; o += align256((size_t)t * 4);
+    l.tmap = o; o += align256((size_t)t * 4);
+    l.tmp = o; l.tmp_bytes = align256(tb); o += l.tmp_bytes;
+    l.bytes = o;
+    return l;
+}
+
+// one-ring (smooth: e = 6t directed edges) or incidence (normals: e = 3t) lists
+struct ListLayout {
+    size_t keys_a, keys_b, row, pos, tmp, tmp_bytes, bytes;
+};
+ListLayout list_layout(int64_t m, int64_t e, bool pos) {
+    ListLayout l;
+    size_t sort_b = 0;
+    cub::DeviceRadixSort::SortKeys(nullptr, sort_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                   (int)e);
+    size_t o = 0;
+    l.keys_a = o; o += align256((size_t)e * 8);
+    l.keys_b = o; o += align256((size_t)e * 8);
+    l.row = o; o += align256((size_t)(m + 1) * 4);
+    l.pos = o; o += pos ? align256((size_t)m * 24) : 0;
+    l.tmp = o; l.tmp_bytes = align256(sort_b); o += l.tmp_bytes;
+    l.bytes = o;
+    return l;
+}
+
+// sort the keys of an e-entry list and bound its rows; returns the sorted buffer
+int build_lists(char* ws, const ListLayout& l, int64_t m, int64_t e, unsigned long long** sorted, cudaStream_t st) {
+    unsigned long long* ka = (unsigned long long*)(ws + l.keys_a);
+    unsigned long long* kb = (unsigned long long*)(ws + l.keys_b);
+    int end_bit = 33;  // the high word holds a vertex index < m <= 2^31
+    while (end_bit < 64 && ((unsigned long long)m >> (end_bit - 32)) != 0) ++end_bit;
+    size_t b = l.tmp_bytes;
+    if (e > 0) G2PC_CUDA(cub::DeviceRadixSort::SortKeys(ws + l.tmp, b, ka, kb, (int)e, 0, end_bit, st));
+    row_kernel<<<grid_of(m + 1), MB, 0, st>>>(kb, e, m, (int32_t*)(ws + l.row));
+    G2PC_CHECK_LAUNCH();
+    *sorted = kb;
+    return G2PC_OK;
+}
+
+}  // namespace
+
+// ---- C ABI -----------------------------------------------------------------------------------------------------------
+extern "C" int64_t g2pc_mesh_splat_workspace_bytes(int64_t n) { return (int64_t)splat_layout(n).bytes; }
+
+extern "C" int g2pc_mesh_splat(const float* xyz, const void* normals, int normal_dtype, int64_t n, int32_t depth,
+                               double* frame, int64_t* B, uint32_t* cell, int32_t* status, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(n >= 0 && n < 0x7FFFFFFFll, "n must be in 0..2^31-2");
+    G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
+    G2PC_CHECK_ARG(normal_dtype == G2PC_F32 || normal_dtype == G2PC_F64, "normals must be float32 or float64");
+    G2PC_CHECK_ARG(frame && B && status && workspace, "null pointer");
+    G2PC_CHECK_ARG(n == 0 || (xyz && normals && cell), "null pointer");
+    const SplatLayout l = splat_layout(n);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    const int R = 1 << depth;
+    const int64_t cells = cells_of(depth);
+    float* part = (float*)(ws + l.part);
+    unsigned long long* total = (unsigned long long*)(ws + l.total);
+    G2PC_CUDA(cudaMemsetAsync(status, 0, 2 * sizeof(int32_t), st));
+    G2PC_CUDA(cudaMemsetAsync(B, 0, (size_t)cells * 8, st));
+    G2PC_CUDA(cudaMemsetAsync(total, 0, 8, st));
+    if (n > 0) {
+        bbox_kernel<<<l.nb, MB, 0, st>>>(xyz, n, part);
+        G2PC_CHECK_LAUNCH();
+    }
+    frame_kernel<<<1, 1, 0, st>>>(part, n > 0 ? l.nb : 0, R, frame);
+    G2PC_CHECK_LAUNCH();
+    if (n > 0) {
+        unsigned long long* Bu = (unsigned long long*)B;
+        if (normal_dtype == G2PC_F32)
+            splat_kernel<float><<<grid_of(n), MB, 0, st>>>(xyz, (const float*)normals, n, R, frame, Bu, cell, status);
+        else
+            splat_kernel<double><<<grid_of(n), MB, 0, st>>>(xyz, (const double*)normals, n, R, frame, Bu, cell, status);
+        G2PC_CHECK_LAUNCH();
+    }
+    sum_b_kernel<<<RED_BLOCKS, MB, 0, st>>>((const long long*)B, cells, total);
+    G2PC_CHECK_LAUNCH();
+    mean_b_kernel<<<1, 1, 0, st>>>(total, cells, frame);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_solve_workspace_bytes(int32_t depth) {
+    return depth_ok(depth) ? (int64_t)solve_layout(depth).bytes : 0;
+}
+
+extern "C" int g2pc_mesh_vcycle(const int64_t* B, const double* frame, int32_t depth, float* chi, int32_t first,
+                                double* norms, void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
+    G2PC_CHECK_ARG(B && frame && chi && norms && workspace, "null pointer");
+    const SolveLayout l = solve_layout(depth);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    const int R = 1 << depth, levels = depth - 2;  // level lv has R >> lv cells per axis; the last one has 4
+    double* partial = (double*)(ws + l.partial);
+    float* lchi[G2PC_MESH_DEPTH_MAX];
+    Rhs lrhs[G2PC_MESH_DEPTH_MAX];
+    lchi[0] = chi;
+    lrhs[0] = Rhs{(const long long*)B, nullptr, frame};
+    for (int lv = 1; lv <= levels; ++lv) {
+        lchi[lv] = (float*)(ws + l.chi[lv]);
+        lrhs[lv] = Rhs{nullptr, (const float*)(ws + l.rhs[lv]), frame};
+    }
+    const Rhs rhs0 = lrhs[0];
+    if (first) {
+        G2PC_CUDA(cudaMemsetAsync(chi, 0, (size_t)cells_of(depth) * 4, st));
+        grid_partial_kernel<1><<<RED_BLOCKS, MB, 0, st>>>(chi, rhs0, R, partial);
+        G2PC_CHECK_LAUNCH();
+        finish_kernel<<<1, 1024, 0, st>>>(partial, 1.0, norms + 1);
+        G2PC_CHECK_LAUNCH();
+    }
+    auto smooth = [&](int lv, int sweeps) -> int {
+        const int n = R >> lv;
+        for (int s = 0; s < sweeps; ++s)
+            for (int colour = 0; colour < 2; ++colour) {
+                rb_smooth_kernel<<<grid_of((int64_t)n * n * (n / 2)), MB, 0, st>>>(lchi[lv], lrhs[lv], n, colour);
+                G2PC_CHECK_LAUNCH();
+            }
+        return G2PC_OK;
+    };
+    for (int lv = 0; lv < levels; ++lv) {
+        const int n = R >> lv, nc = n >> 1;
+        if (smooth(lv, 2)) return G2PC_ERR_CUDA;
+        restrict_kernel<<<grid_of((int64_t)nc * nc * nc), MB, 0, st>>>(lchi[lv], lrhs[lv], n, (float*)lrhs[lv + 1].f);
+        G2PC_CHECK_LAUNCH();
+        G2PC_CUDA(cudaMemsetAsync(lchi[lv + 1], 0, (size_t)nc * nc * nc * 4, st));
+    }
+    coarse_kernel<<<1, 64, 0, st>>>(lchi[levels], lrhs[levels]);
+    G2PC_CHECK_LAUNCH();
+    for (int lv = levels - 1; lv >= 0; --lv) {
+        const int n = R >> lv;
+        prolong_kernel<<<grid_of((int64_t)n * n * n), MB, 0, st>>>(lchi[lv], n, lchi[lv + 1]);
+        G2PC_CHECK_LAUNCH();
+        if (smooth(lv, 2)) return G2PC_ERR_CUDA;
+    }
+    grid_partial_kernel<0><<<RED_BLOCKS, MB, 0, st>>>(chi, rhs0, R, partial);
+    G2PC_CHECK_LAUNCH();
+    finish_kernel<<<1, 1024, 0, st>>>(partial, 1.0, norms);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_iso_workspace_bytes(void) { return (int64_t)align256(2 * RED_BLOCKS * sizeof(double)); }
+
+extern "C" int g2pc_mesh_iso(const float* xyz, const uint32_t* cell, int64_t n, const double* frame, int32_t depth,
+                             float* chi, double* iso, void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(n >= 0 && n < 0x7FFFFFFFll, "n must be in 0..2^31-2");
+    G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
+    G2PC_CHECK_ARG(frame && chi && iso && workspace, "null pointer");
+    G2PC_CHECK_ARG(n == 0 || (xyz && cell), "null pointer");
+    G2PC_CHECK_ARG(workspace_bytes >= g2pc_mesh_iso_workspace_bytes(), "workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    double* partial = (double*)workspace;
+    const int R = 1 << depth;
+    const int64_t cells = cells_of(depth);
+    const Rhs none{nullptr, nullptr, frame};
+    grid_partial_kernel<2><<<RED_BLOCKS, MB, 0, st>>>(chi, none, R, partial);
+    G2PC_CHECK_LAUNCH();
+    finish_kernel<<<1, 1024, 0, st>>>(partial, 1.0 / (double)cells, iso);
+    G2PC_CHECK_LAUNCH();
+    shift_kernel<<<grid_of(cells), MB, 0, st>>>(chi, cells, iso);
+    G2PC_CHECK_LAUNCH();
+    iso_partial_kernel<<<RED_BLOCKS, MB, 0, st>>>(xyz, cell, n, frame, R, chi, partial);
+    G2PC_CHECK_LAUNCH();
+    finish_kernel<<<1, 1024, 0, st>>>(partial, 1.0, iso + 1);
+    G2PC_CHECK_LAUNCH();
+    finish_kernel<<<1, 1024, 0, st>>>(partial + RED_BLOCKS, 1.0, iso + 2);
+    G2PC_CHECK_LAUNCH();
+    iso_div_kernel<<<1, 1, 0, st>>>(iso);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_extract_workspace_bytes(int32_t depth) {
+    return depth_ok(depth) ? (int64_t)extract_layout(depth).bytes : 0;
+}
+
+extern "C" int g2pc_mesh_extract_count(const float* chi, int32_t depth, const double* iso, int64_t* counts,
+                                       void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
+    G2PC_CHECK_ARG(chi && iso && counts && workspace, "null pointer");
+    const ExtractLayout l = extract_layout(depth);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    long long* vblk = (long long*)(ws + l.vblk);
+    long long* tblk = (long long*)(ws + l.tblk);
+    G2PC_CUDA(cudaMemsetAsync(vblk + l.nb, 0, 8, st));
+    G2PC_CUDA(cudaMemsetAsync(tblk + l.nb, 0, 8, st));
+    mt_count_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, 1 << depth, iso, vblk, tblk);
+    G2PC_CHECK_LAUNCH();
+    size_t b = l.tmp_bytes;
+    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, vblk, (long long*)(ws + l.voff), (int)(l.nb + 1), st));
+    b = l.tmp_bytes;
+    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, tblk, (long long*)(ws + l.toff), (int)(l.nb + 1), st));
+    totals_kernel<<<1, 1, 0, st>>>((const long long*)(ws + l.voff), (const long long*)(ws + l.toff), l.nb,
+                                   (long long*)counts);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int g2pc_mesh_extract_emit(const float* chi, int32_t depth, const double* frame, const double* iso,
+                                      void* node_scratch, int64_t node_scratch_bytes, const void* workspace,
+                                      int64_t workspace_bytes, int64_t* vkey, double* vt, double* vpos, int32_t* faces,
+                                      void* stream) {
+    G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
+    G2PC_CHECK_ARG(chi && frame && iso && node_scratch && workspace, "null pointer");
+    const ExtractLayout l = extract_layout(depth);
+    const int64_t cells = cells_of(depth);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(node_scratch_bytes >= 5 * cells, "node scratch too small (5 bytes per node)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const char* ws = (const char*)workspace;
+    int32_t* base = (int32_t*)node_scratch;
+    uint8_t* mask = (uint8_t*)node_scratch + 4 * cells;
+    const int R = 1 << depth;
+    mt_vertex_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, R, frame, iso, (const long long*)(ws + l.voff), base, mask,
+                                                    (long long*)vkey, vt, vpos);
+    G2PC_CHECK_LAUNCH();
+    mt_triangle_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, R, iso, (const long long*)(ws + l.toff), base, mask, faces);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_gather_workspace_bytes(int64_t n) { return (int64_t)gather_layout(n).bytes; }
+
+extern "C" int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const uint32_t* cell, int64_t n,
+                                const double* frame, int32_t depth, const int64_t* vkey, const double* vt, int64_t m,
+                                void* cell_scratch, int64_t cell_scratch_bytes, double* density, uint8_t* vcolours,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(n >= 0 && n < 0x7FFFFFFFll && m >= 0, "bad sizes");
+    G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
+    G2PC_CHECK_ARG(frame && cell_scratch && workspace, "null pointer");
+    const int R = 1 << depth;
+    const int64_t dual = (int64_t)(R - 1) * (R - 1) * (R - 1);
+    G2PC_CHECK_ARG(cell_scratch_bytes >= 4 * dual, "cell scratch too small (4 bytes per dual cell)");
+    const GatherLayout l = gather_layout(n);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    if (m == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(vkey && vt && density && (n == 0 || (xyz && cell)), "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    uint32_t* ka = (uint32_t*)(ws + l.keys_a);
+    uint32_t* kb = (uint32_t*)(ws + l.keys_b);
+    uint32_t* ia = (uint32_t*)(ws + l.idx_a);
+    uint32_t* ib = (uint32_t*)(ws + l.idx_b);
+    int32_t* start = (int32_t*)cell_scratch;
+    G2PC_CUDA(cudaMemsetAsync(start, 0xFF, (size_t)dual * 4, st));
+    if (n > 0) {
+        G2PC_CUDA(cudaMemcpyAsync(ka, cell, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+        iota_kernel<<<grid_of(n), MB, 0, st>>>(ia, n);
+        G2PC_CHECK_LAUNCH();
+        size_t b = l.tmp_bytes;  // stable: a cell's points stay in input order
+        G2PC_CUDA(cub::DeviceRadixSort::SortPairs(ws + l.tmp, b, ka, kb, ia, ib, (int)n, 0, 31, st));
+        cell_start_kernel<<<grid_of(n), MB, 0, st>>>(kb, n, start);
+        G2PC_CHECK_LAUNCH();
+    }
+    gather_kernel<<<grid_of(m), MB, 0, st>>>((const long long*)vkey, vt, m, R, kb, ib, n, start, xyz, colours, frame,
+                                             density, vcolours);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_trim_workspace_bytes(int64_t m, int64_t t) { return (int64_t)trim_layout(m, t).bytes; }
+
+extern "C" int g2pc_mesh_trim(const double* density, const double* vpos, const uint8_t* vcolours, int64_t m,
+                              const int32_t* faces, int64_t t, uint8_t* keep, double* threshold, int64_t* counts,
+                              double* density_out, double* vpos_out, uint8_t* vcolours_out, int32_t* faces_out,
+                              void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(m > 0 && m < 0x7FFFFFFFll && t >= 0 && t < 0x7FFFFFFFll, "need 1..2^31-2 vertices");
+    G2PC_CHECK_ARG(density && vpos && keep && threshold && counts && density_out && vpos_out && workspace,
+                   "null pointer");
+    G2PC_CHECK_ARG(!vcolours == !vcolours_out, "vertex colours need an output");
+    G2PC_CHECK_ARG(t == 0 || (faces && faces_out), "null pointer");
+    const TrimLayout l = trim_layout(m, t);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    double* sorted = (double*)(ws + l.sorted);
+    int32_t* vflag = (int32_t*)(ws + l.vflag);
+    int32_t* vmap = (int32_t*)(ws + l.vmap);
+    int32_t* tflag = (int32_t*)(ws + l.tflag);
+    int32_t* tmap = (int32_t*)(ws + l.tmap);
+    size_t b = l.tmp_bytes;
+    G2PC_CUDA(cub::DeviceRadixSort::SortKeys(ws + l.tmp, b, density, sorted, (int)m, 0, 64, st));
+    quantile_kernel<<<1, 1, 0, st>>>(sorted, m, threshold);
+    G2PC_CHECK_LAUNCH();
+    keep_kernel<<<grid_of(m), MB, 0, st>>>(density, m, threshold, keep, vflag);
+    G2PC_CHECK_LAUNCH();
+    b = l.tmp_bytes;
+    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, vflag, vmap, (int)m, st));
+    if (t > 0) {
+        tri_flag_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, keep, tflag);
+        G2PC_CHECK_LAUNCH();
+        b = l.tmp_bytes;
+        G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, tflag, tmap, (int)t, st));
+        compact_faces_kernel<<<grid_of(t), MB, 0, st>>>(faces, tflag, tmap, t, vmap, faces_out);
+        G2PC_CHECK_LAUNCH();
+    }
+    compact_vertices_kernel<<<grid_of(m), MB, 0, st>>>(keep, vmap, m, density, vpos, vcolours, density_out, vpos_out,
+                                                       vcolours_out);
+    G2PC_CHECK_LAUNCH();
+    trim_counts_kernel<<<1, 1, 0, st>>>(vflag, vmap, m, tflag, tmap, t, (long long*)counts);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_smooth_workspace_bytes(int64_t m, int64_t t) {
+    return (int64_t)list_layout(m, 6 * t, true).bytes;
+}
+
+extern "C" int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, int64_t t, int32_t iterations,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(m >= 0 && m < 0x7FFFFFFFll && t >= 0 && 6 * t < 0x7FFFFFFFll, "bad sizes");
+    G2PC_CHECK_ARG(iterations >= 0, "iterations < 0");
+    if (m == 0 || iterations == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(vpos && workspace && (t == 0 || faces), "null pointer");
+    const ListLayout l = list_layout(m, 6 * t, true);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    if (t > 0) {
+        ring_keys_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, (unsigned long long*)(ws + l.keys_a));
+        G2PC_CHECK_LAUNCH();
+    }
+    unsigned long long* keys;
+    if (build_lists(ws, l, m, 6 * t, &keys, st)) return G2PC_ERR_CUDA;
+    const int32_t* row = (const int32_t*)(ws + l.row);
+    double* other = (double*)(ws + l.pos);
+    double* src = vpos;
+    double* dst = other;
+    for (int it = 0; it < iterations; ++it) {
+        smooth_kernel<<<grid_of(m), MB, 0, st>>>(src, m, keys, row, dst);
+        G2PC_CHECK_LAUNCH();
+        double* x = src; src = dst; dst = x;
+    }
+    if (src != vpos) G2PC_CUDA(cudaMemcpyAsync(vpos, src, (size_t)m * 24, cudaMemcpyDeviceToDevice, st));
+    return G2PC_OK;
+}
+
+extern "C" int64_t g2pc_mesh_normals_workspace_bytes(int64_t m, int64_t t) {
+    return (int64_t)list_layout(m, 3 * t, false).bytes;
+}
+
+extern "C" int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* faces, int64_t t, float* vertices,
+                                 float* normals, void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(m >= 0 && m < 0x7FFFFFFFll && t >= 0 && 3 * t < 0x7FFFFFFFll, "bad sizes");
+    if (m == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(vpos && vertices && normals && workspace && (t == 0 || faces), "null pointer");
+    const ListLayout l = list_layout(m, 3 * t, false);
+    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    if (t > 0) {
+        incidence_keys_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, (unsigned long long*)(ws + l.keys_a));
+        G2PC_CHECK_LAUNCH();
+    }
+    unsigned long long* keys;
+    if (build_lists(ws, l, m, 3 * t, &keys, st)) return G2PC_ERR_CUDA;
+    normals_kernel<<<grid_of(m), MB, 0, st>>>(vpos, m, faces, keys, (const int32_t*)(ws + l.row), vertices, normals);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}

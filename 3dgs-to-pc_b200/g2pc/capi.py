@@ -43,6 +43,30 @@ SIGNATURES = {
     "g2pc_knn_mean_dist": ([_c_void_p, _i64, _i32, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_sor_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_sor_mask": ([_c_void_p, _i64, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_splat_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_mesh_splat": ([_c_void_p, _c_void_p, ctypes.c_int, _i64, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                         _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_solve_workspace_bytes": ([_i32], ctypes.c_int64),
+    "g2pc_mesh_vcycle": ([_c_void_p, _c_void_p, _i32, _c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p],
+                         ctypes.c_int),
+    "g2pc_mesh_iso_workspace_bytes": ([], ctypes.c_int64),
+    "g2pc_mesh_iso": ([_c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
+                      ctypes.c_int),
+    "g2pc_mesh_extract_workspace_bytes": ([_i32], ctypes.c_int64),
+    "g2pc_mesh_extract_count": ([_c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_extract_emit": ([_c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i64, _c_void_p,
+                                _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_gather_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_mesh_gather": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p,
+                          _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_trim_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_mesh_trim": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
+                        _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_smooth_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_mesh_smooth": ([_c_void_p, _i64, _c_void_p, _i64, _i32, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_normals_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_mesh_normals": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
+                          ctypes.c_int),
     "g2pc_points_per_gaussian": ([_c_void_p, _c_void_p, _i64, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _i64,
                                   _c_void_p], ctypes.c_int),
     "g2pc_pack_geometry": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p], ctypes.c_int),
@@ -129,10 +153,16 @@ TIMING = None     # None, or a dict filled as {entry point name: [(start_event, 
 # hand-written kernels launched per entry point (default 1); the radix sorts inside g2pc_depth_sort and
 # g2pc_knn_mean_dist are cub's (library)
 _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
-                "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_sor_mask": 5}
+                "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_sor_mask": 5, "g2pc_mesh_splat": 5,
+                "g2pc_mesh_iso": 7, "g2pc_mesh_extract_count": 2, "g2pc_mesh_extract_emit": 2, "g2pc_mesh_gather": 3,
+                "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3}
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",
                 "g2pc_multisplit_rows", "g2pc_blend_set_compact", "g2pc_cull_workspace_bytes", "g2pc_ppg_workspace_bytes",
-                "g2pc_depth_sort_workspace_bytes", "g2pc_knn_workspace_bytes", "g2pc_sor_workspace_bytes"}
+                "g2pc_depth_sort_workspace_bytes", "g2pc_knn_workspace_bytes", "g2pc_sor_workspace_bytes",
+                "g2pc_mesh_splat_workspace_bytes", "g2pc_mesh_solve_workspace_bytes", "g2pc_mesh_iso_workspace_bytes",
+                "g2pc_mesh_extract_workspace_bytes", "g2pc_mesh_gather_workspace_bytes",
+                "g2pc_mesh_trim_workspace_bytes", "g2pc_mesh_smooth_workspace_bytes",
+                "g2pc_mesh_normals_workspace_bytes"}
 
 
 def call(name, *args):

@@ -1,0 +1,71 @@
+"""Mesh an existing point cloud on the GPU: Poisson reconstruction with a multigrid solve, marching tetrahedra, density
+trim and Laplacian smoothing (g2pc/mesh.py).
+
+    python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10]
+                      [--laplacian_iterations 10] [--quiet]
+
+The cloud must carry normals (nx ny nz), as gauss_to_pc.py writes them by default; its colours (red green blue) are
+carried over to the mesh's vertices.  The normals are used as they are: a mesh faces the way its normals point."""
+import argparse
+import time
+
+import numpy as np
+import torch
+
+import gauss_dataloader
+from g2pc import build, mesh
+
+
+def _depth(s):
+    d = int(s)
+    if not mesh.DEPTH_MIN <= d <= mesh.DEPTH_MAX:
+        raise argparse.ArgumentTypeError(f"must be in {mesh.DEPTH_MIN}..{mesh.DEPTH_MAX}")
+    return d
+
+
+def _iterations(s):
+    i = int(s)
+    if i < 0:
+        raise argparse.ArgumentTypeError("must be >= 0")
+    return i
+
+
+def config_parser(argv=None):
+    p = argparse.ArgumentParser(description="Mesh a point cloud with oriented normals (Poisson reconstruction)")
+    p.add_argument("--input_path", required=True, help="point-cloud PLY with x y z and nx ny nz (red green blue optional)")
+    p.add_argument("--mesh_output_path", default="mesh.ply", help="output mesh PLY")
+    p.add_argument("--poisson_depth", type=_depth, default=10,
+                   help=f"grid of 2^depth nodes per axis, {mesh.DEPTH_MIN}..{mesh.DEPTH_MAX}")
+    p.add_argument("--laplacian_iterations", type=_iterations, default=10, help="Laplacian smoothing steps (0: none)")
+    p.add_argument("--quiet", action="store_true", help="print nothing")
+    return p.parse_args(argv)
+
+
+def load_cloud(path, device="cuda:0"):
+    """(points (n,3) f32, normals (n,3) f32, colours (n,3) f32 or None) of a point-cloud PLY."""
+    v = gauss_dataloader.read_ply_vertices(path)
+    names = v.dtype.names
+    if not all(k in names for k in ("nx", "ny", "nz")):
+        raise ValueError(f"{path} has no normals (nx ny nz): Poisson meshing needs them")
+    col = lambda *k: torch.from_numpy(np.ascontiguousarray(np.stack([v[c] for c in k], 1), dtype=np.float32))
+    colours = col("red", "green", "blue").to(device) if "red" in names else None
+    return col("x", "y", "z").to(device), col("nx", "ny", "nz").to(device), colours
+
+
+def main(argv=None):
+    args = config_parser(argv)
+    build.build()
+    t0 = time.perf_counter()
+    points, normals, colours = load_cloud(args.input_path)
+    if not args.quiet:
+        print(f"Meshing {points.shape[0]} points at depth {args.poisson_depth}")
+    m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations)
+    mesh.write_mesh_ply(args.mesh_output_path, m)
+    if not args.quiet:
+        print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path} "
+              f"in {time.perf_counter() - t0:.2f} s")
+    return m
+
+
+if __name__ == "__main__":
+    main()

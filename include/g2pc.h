@@ -177,6 +177,85 @@ int64_t g2pc_sor_workspace_bytes(int64_t n);
 int g2pc_sor_mask(const double* avg, int64_t n, double std_ratio, uint8_t* keep, double* stats, void* workspace,
                   int64_t workspace_bytes, void* stream);
 
+/* ---- N6: Poisson mesh of an oriented point cloud (s10_mesh.cu, g2pc/mesh.py, mesh_pc.py) ------------------------- */
+/* Replaces Open3D's create_from_point_cloud_poisson + density trim + filter_smooth_laplacian behind the reference's
+ * mesh_handler.generate_mesh (mesh_handler.py:23-40), with this project's own rules (DESIGN.md §2).  Order of calls:
+ * splat -> vcycle (until the residual is small enough) -> iso -> extract_count -> extract_emit -> gather -> trim -> smooth
+ * -> normals.  Grid: R = 2^depth nodes per axis, 2 <= depth <= G2PC_MESH_DEPTH_MAX; node index (k*R + j)*R + i. */
+#define G2PC_MESH_DEPTH_MAX 10
+#define G2PC_MESH_FRAME_WORDS 8 /* float64: origin x y z, h, L, mean of B, largest extent, R */
+
+/* frame (G2PC_MESH_FRAME_WORDS float64): L = 1.1 x the largest extent of the finite points, origin = bounding-box
+ * centre - L/2, h = L/R (h = 0: zero extent, nothing is splatted).  B (R^3 int64, zeroed here): every point with a
+ * usable normal adds llrint(w * n_a / |n| * 2^32) at node - e_a and subtracts it at node + e_a for the 8 trilinear
+ * weights w of its dual cell and the 3 axes a (exact integer atomics).  cell (n uint32): linear index of the point's
+ * dual cell in the (R-1)^3 lattice, 0x7FFFFFFF when it was not splatted.  status (2 int32): points skipped for a zero or
+ * non-finite normal, points with a non-finite coordinate.  normals (n,3) in normal_dtype (G2PC_F32 / G2PC_F64).
+ * workspace: g2pc_mesh_splat_workspace_bytes(n), 256-byte aligned. */
+int64_t g2pc_mesh_splat_workspace_bytes(int64_t n);
+int g2pc_mesh_splat(const float* xyz, const void* normals, int normal_dtype, int64_t n, int32_t depth, double* frame,
+                    int64_t* B, uint32_t* cell, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* One multigrid V-cycle of (sum of the 6 neighbours - 6 chi) = b with mirrored ghosts (homogeneous Neumann),
+ * b = (B - mean B) * h * 2^-33 read from B: red-black Gauss-Seidel (2 + 2 sweeps), fused residual + 8-cell restriction,
+ * trilinear prolongation, 4^3 coarsest level.  chi: R^3 float32; first != 0 zeroes chi and writes norms[1] = |b|^2; every
+ * call writes norms[0] = |r|^2 after the cycle (fixed-order float64 sums).  workspace:
+ * g2pc_mesh_solve_workspace_bytes(depth), 256-byte aligned (the coarse levels). */
+int64_t g2pc_mesh_solve_workspace_bytes(int32_t depth);
+int g2pc_mesh_vcycle(const int64_t* B, const double* frame, int32_t depth, float* chi, int32_t first, double* norms,
+                     void* workspace, int64_t workspace_bytes, void* stream);
+
+/* Subtracts the mean of chi from chi, then iso (3 float64): iso[0] = that mean, iso[1] = mean over the splatted points
+ * of the trilinear chi at the point (the splat's weights), iso[2] = their count.  Fixed-order float64 sums.
+ * workspace: g2pc_mesh_iso_workspace_bytes(), 8-byte aligned. */
+int64_t g2pc_mesh_iso_workspace_bytes(void);
+int g2pc_mesh_iso(const float* xyz, const uint32_t* cell, int64_t n, const double* frame, int32_t depth, float* chi,
+                  double* iso, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* Marching tetrahedra over the (R-1)^3 cubes of the node lattice, 6 Kuhn tetrahedra per cube; a node is inside iff
+ * chi < iso[1].  extract_count writes counts (2 int64) = vertices m, triangles t; extract_emit (same workspace, after
+ * extract_count) writes vkey (m int64, node*8 + d for the crossed edge (node, node + d), d = 1..7 bit 0 = x, ascending),
+ * vt (m float64, t = (iso - chi_a) / (chi_b - chi_a)), vpos (m,3 float64), faces (t,3 int32, ascending (cube, tetrahedron,
+ * triangle), counter-clockwise seen from chi > iso).  node_scratch: 5 bytes per node (B's memory may be reused).
+ * workspace: g2pc_mesh_extract_workspace_bytes(depth), 256-byte aligned. */
+int64_t g2pc_mesh_extract_workspace_bytes(int32_t depth);
+int g2pc_mesh_extract_count(const float* chi, int32_t depth, const double* iso, int64_t* counts, void* workspace,
+                            int64_t workspace_bytes, void* stream);
+int g2pc_mesh_extract_emit(const float* chi, int32_t depth, const double* frame, const double* iso, void* node_scratch,
+                           int64_t node_scratch_bytes, const void* workspace, int64_t workspace_bytes, int64_t* vkey,
+                           double* vt, double* vpos, int32_t* faces, void* stream);
+
+/* Per vertex: density = (1-t) W_a + t W_b and colour = floor(((1-t) C_a + t C_b) / density + 0.5) clamped to 0..255
+ * (0 where density is 0), W / C = sums of w / w * colour over the points of the 8 dual cells around the node (cells in
+ * ascending index, points in ascending input index, sequential float64).  colours (n,3 int32) and vcolours (m,3 uint8)
+ * may both be NULL.  cell_scratch: 4 bytes per dual cell.  workspace: g2pc_mesh_gather_workspace_bytes(n). */
+int64_t g2pc_mesh_gather_workspace_bytes(int64_t n);
+int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const uint32_t* cell, int64_t n, const double* frame,
+                     int32_t depth, const int64_t* vkey, const double* vt, int64_t m, void* cell_scratch,
+                     int64_t cell_scratch_bytes, double* density, uint8_t* vcolours, void* workspace,
+                     int64_t workspace_bytes, void* stream);
+
+/* threshold = numpy's linear 10 % quantile of the densities; keep (m uint8) = !(density < threshold); triangles with a
+ * removed vertex are dropped and the kept vertices re-indexed in order.  Outputs (capacity m / t) are compacted: counts
+ * (2 int64) = kept vertices, kept triangles.  workspace: g2pc_mesh_trim_workspace_bytes(m, t), 256-byte aligned. */
+int64_t g2pc_mesh_trim_workspace_bytes(int64_t m, int64_t t);
+int g2pc_mesh_trim(const double* density, const double* vpos, const uint8_t* vcolours, int64_t m, const int32_t* faces,
+                   int64_t t, uint8_t* keep, double* threshold, int64_t* counts, double* density_out, double* vpos_out,
+                   uint8_t* vcolours_out, int32_t* faces_out, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* `iterations` Jacobi steps v += (sum w_j v_j / sum w_j - v) / 2, w_j = 1 / (|v - v_j| + 1e-12) over the distinct one-ring
+ * neighbours in ascending index (float64; a vertex without neighbours stays).  vpos (m,3 float64) in place.
+ * workspace: g2pc_mesh_smooth_workspace_bytes(m, t), 256-byte aligned. */
+int64_t g2pc_mesh_smooth_workspace_bytes(int64_t m, int64_t t);
+int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, int64_t t, int32_t iterations, void* workspace,
+                     int64_t workspace_bytes, void* stream);
+
+/* vertices (m,3 float32) = vpos rounded; normals (m,3 float32) = normalised sum of cross(p1 - p0, p2 - p0) over the
+ * incident triangles in ascending order (float64; zero stays zero).  workspace: g2pc_mesh_normals_workspace_bytes(m, t). */
+int64_t g2pc_mesh_normals_workspace_bytes(int64_t m, int64_t t);
+int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* faces, int64_t t, float* vertices, float* normals,
+                      void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- S3-S6: colour stage, renderer_type=python semantics (gauss_render.py:101-465) ------------------------------ */
 /* Replaces GaussPythonRenderer.__call__/render (gauss_render.py:266-465) and — as the native op boundary — the role
  * of _C.rasterize_gaussians (rasterize_points.cu:36-145) in the per-camera loop of gauss_to_pc.py:437-454.

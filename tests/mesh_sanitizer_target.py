@@ -1,0 +1,48 @@
+"""Tiny Poisson mesh, meant to be executed under compute-sanitizer (tests/test_mesh_gpu.py): memcheck and racecheck
+over the splat, the multigrid cycles, the iso-value, the extraction, the gathers, the trim, smoothing and normals.
+
+Without the sanitizer (the test runs it directly when the tool does not support the GPU):
+  G2PC_TARGET_POISON=<byte>   every block PyTorch's caching allocator hands out afterwards starts filled with <byte>
+  G2PC_TARGET_OUT=<file.npz>  every output of the run is saved there, for bit-for-bit comparison between runs"""
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "3dgs-to-pc_b200"))
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from g2pc import mesh  # noqa: E402
+
+dev = "cuda:0"
+
+
+def poison_allocator(byte):
+    """Fill and release blocks of both pools of the caching allocator (it keeps them cached), so a kernel that reads
+    memory nobody wrote sees `byte`."""
+    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(64)]
+    large = [torch.full((64 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(4)]
+    torch.cuda.synchronize()
+    del small, large
+    for nbytes in (4096, 8 << 20):
+        probe = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
+        del probe
+
+
+if os.environ.get("G2PC_TARGET_POISON") is not None:
+    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
+rng = np.random.default_rng(3)
+d = rng.normal(size=(3000, 3))
+d /= np.linalg.norm(d, axis=1, keepdims=True)
+p = np.concatenate([0.8 * d, [[0.0, 0.0, 0.0]]]).astype(np.float32)
+nrm = np.concatenate([d, [[0.0, 0.0, 0.0]]]).astype(np.float32)
+cols = rng.uniform(0, 255, p.shape).astype(np.float32)
+m, dbg = mesh.poisson_mesh(torch.from_numpy(p).to(dev), torch.from_numpy(nrm).to(dev), torch.from_numpy(cols).to(dev),
+                           depth=4, laplacian_iters=2, return_debug=True)
+torch.cuda.synchronize()
+if os.environ.get("G2PC_TARGET_OUT"):
+    outputs = dict(m._asdict(), **{k: dbg[k] for k in ("chi", "iso", "B", "keep", "threshold")})
+    np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
+print("MESH_TARGET_OK", m.vertices.shape[0], m.faces.shape[0])
