@@ -16,6 +16,33 @@ void g2pc_set_error(const char* fmt, ...);
         }                                                          \
     } while (0)
 
+// caller-provided workspace: at least `need` bytes, base aligned to `align` (a power of two)
+#define G2PC_CHECK_WORKSPACE(ptr, bytes, need, align)                                        \
+    do {                                                                                     \
+        if ((int64_t)(bytes) < (int64_t)(need)) {                                            \
+            g2pc_set_error("%s: workspace too small", __func__);                             \
+            return G2PC_ERR_WORKSPACE;                                                       \
+        }                                                                                    \
+        if (((uintptr_t)(ptr) & ((uintptr_t)(align) - 1)) != 0) {                            \
+            g2pc_set_error("%s: workspace must be %d-byte aligned", __func__, (int)(align)); \
+            return G2PC_ERR_WORKSPACE;                                                       \
+        }                                                                                    \
+    } while (0)
+
+// Typed slices of a workspace, each padded to a multiple of 256 bytes, so each starts 256-byte aligned relative to the
+// base.  A null base only adds up the size, so one layout function serves both the size query and the entry point.
+struct WsCarve {
+    char* base;
+    size_t used = 0;
+    static size_t pad(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+    template <class T>
+    T* take(size_t count) {
+        T* p = base ? (T*)(base + used) : nullptr;
+        used += pad(count * sizeof(T));
+        return p;
+    }
+};
+
 #define G2PC_CHECK_LAUNCH()                                                        \
     do {                                                                           \
         cudaError_t e__ = cudaGetLastError();                                      \

@@ -13,7 +13,7 @@
 // the right-hand side b = (B - mean B) * h * 2^-33 formed on the fly from B (no float copy of b is stored).
 // All float64 expressions that a test compares bit for bit are written with __d*_rn intrinsics: no FMA contraction.
 #include <cub/cub.cuh>
-#include "common.cuh"
+#include "cloud_common.cuh"
 
 namespace {
 
@@ -21,17 +21,12 @@ constexpr int MB = 256;                         // threads per CTA of the per-po
 constexpr int RED_BLOCKS = 1024;                // fixed partition of every float64 reduction: bit-identical re-runs
 constexpr int NPT = 4;                          // lattice nodes per thread in the extraction kernels
 constexpr int NODES_PER_CTA = MB * NPT;
-constexpr int BOX_PER_CTA = MB * 8;
 constexpr int COARSE_SWEEPS = 100;              // red-black sweeps of the 4^3 coarsest level
 constexpr uint32_t CELL_NONE = 0x7FFFFFFFu;     // dual cell of a point that was not splatted (sorts last)
 constexpr double TWO32 = 4294967296.0;
 
 // frame words (float64, device): written by g2pc_mesh_splat
 enum { FR_ORIGIN = 0, FR_H = 3, FR_L = 4, FR_MEANB = 5, FR_EXTENT = 6, FR_R = 7 };
-
-__host__ __device__ __forceinline__ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-__device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
 
 struct PointCell {
     int i0[3];
@@ -70,66 +65,20 @@ __device__ __forceinline__ double node_coord(const double* __restrict__ fr, int 
 }
 
 // ---- fixed-order float64 reductions -----------------------------------------------------------------------------
-__device__ __forceinline__ double block_sum(double v, double* s_w) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t = __dadd_rn(t, s_w[w]);
-    return t;  // valid in thread 0
-}
-
-// one CTA of 1024 threads: out[slot] = sum of RED_BLOCKS partials (x scale), in a fixed order
+// one CTA of 1024 threads: *out = sum of RED_BLOCKS partials (x scale), in a fixed order.  Each thread adds its one
+// partial to +0.0, which changes nothing: a partial comes from block_sum_f64, which starts at +0.0, so it is never -0.0.
 __global__ void __launch_bounds__(1024) finish_kernel(const double* __restrict__ partial, double scale,
                                                       double* __restrict__ out) {
     __shared__ double s[1024];
-    s[threadIdx.x] = threadIdx.x < RED_BLOCKS ? partial[threadIdx.x] : 0.0;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (threadIdx.x < o) s[threadIdx.x] = __dadd_rn(s[threadIdx.x], s[threadIdx.x + o]);
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *out = __dmul_rn(s[0], scale);
+    const double t = sum_partials_f64(partial, RED_BLOCKS, s);
+    if (threadIdx.x == 0) *out = __dmul_rn(t, scale);
 }
 
 // ---- splat ------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(MB) bbox_kernel(const float* __restrict__ xyz, int64_t n, float* __restrict__ part) {
-    __shared__ float s[6][MB / 32];
-    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
-    const int64_t base = (int64_t)blockIdx.x * BOX_PER_CTA;
-    for (int r = 0; r < BOX_PER_CTA / MB; ++r) {
-        const int64_t i = base + r * MB + threadIdx.x;
-        if (i >= n) break;
-        const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-        if (!finite3(x, y, z)) continue;
-        mn[0] = fminf(mn[0], x); mn[1] = fminf(mn[1], y); mn[2] = fminf(mn[2], z);
-        mx[0] = fmaxf(mx[0], x); mx[1] = fmaxf(mx[1], y); mx[2] = fmaxf(mx[2], z);
-    }
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-    }
-    if ((threadIdx.x & 31) == 0)
-        for (int a = 0; a < 3; ++a) { s[a][threadIdx.x >> 5] = mn[a]; s[3 + a][threadIdx.x >> 5] = mx[a]; }
-    __syncthreads();
-    if (threadIdx.x < 6) {
-        float v = s[threadIdx.x][0];
-        for (int w = 1; w < MB / 32; ++w) v = threadIdx.x < 3 ? fminf(v, s[threadIdx.x][w]) : fmaxf(v, s[threadIdx.x][w]);
-        part[6 * blockIdx.x + threadIdx.x] = v;
-    }
-}
-
 // one thread: L = 1.1 * largest extent, origin = centre - L / 2, h = L / R (h = 0 when no finite point / zero extent)
 __global__ void frame_kernel(const float* __restrict__ part, int nb, int R, double* __restrict__ fr) {
-    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
-    for (int b = 0; b < nb; ++b)
-        for (int a = 0; a < 3; ++a) { mn[a] = fminf(mn[a], part[6 * b + a]); mx[a] = fmaxf(mx[a], part[6 * b + 3 + a]); }
+    float mn[3], mx[3];
+    fold_bbox(part, nb, mn, mx);
     double ext = 0.0;
     const bool any = mn[0] <= mx[0];
     if (any)
@@ -323,7 +272,7 @@ __global__ void __launch_bounds__(MB) grid_partial_kernel(const float* __restric
             v = __dadd_rn(v, (double)chi[t]);
         }
     }
-    const double tot = block_sum(v, s_w);
+    const double tot = block_sum_f64<MB>(v, s_w);
     if (threadIdx.x == 0) partial[blockIdx.x] = tot;
 }
 
@@ -349,9 +298,9 @@ __global__ void __launch_bounds__(MB) iso_partial_kernel(const float* __restrict
         v = __dadd_rn(v, x);
         cnt += 1.0;
     }
-    const double tv = block_sum(v, s_w);
+    const double tv = block_sum_f64<MB>(v, s_w);
     __syncthreads();
-    const double tc = block_sum(cnt, s_w);
+    const double tc = block_sum_f64<MB>(cnt, s_w);
     if (threadIdx.x == 0) { partial[blockIdx.x] = tv; partial[RED_BLOCKS + blockIdx.x] = tc; }
 }
 
@@ -479,9 +428,9 @@ __global__ void __launch_bounds__(MB) mt_count_kernel(const float* __restrict__ 
         nv += __popc(cross_mask(c));
         if (c.valid == 0xFFu) nt += cube_triangle_count(c.inside);
     }
-    const double sv = block_sum((double)nv, s_w);
+    const double sv = block_sum_f64<MB>((double)nv, s_w);
     __syncthreads();
-    const double st = block_sum((double)nt, s_w);
+    const double st = block_sum_f64<MB>((double)nt, s_w);
     if (threadIdx.x == 0) { vblk[blockIdx.x] = (long long)sv; tblk[blockIdx.x] = (long long)st; }
 }
 
@@ -810,136 +759,149 @@ int64_t cells_of(int depth) { return (int64_t)1 << (3 * depth); }
 
 bool depth_ok(int depth) { return depth >= 2 && depth <= G2PC_MESH_DEPTH_MAX; }
 
-// ---- workspace layouts ----------------------------------------------------------------------------------------------
-struct SplatLayout {
-    size_t part, total, bytes;
-    int nb;
+// ---- workspace layouts: one function per entry point carves the slices; a null base only sizes them ---------------
+struct SplatWs {
+    float* part;
+    unsigned long long* total;
+    size_t bytes;
 };
-SplatLayout splat_layout(int64_t n) {
-    SplatLayout l;
-    l.nb = (int)((n + BOX_PER_CTA - 1) / BOX_PER_CTA);
-    size_t o = 0;
-    l.part = o; o += align256((size_t)(l.nb > 0 ? l.nb : 1) * 6 * sizeof(float));
-    l.total = o; o += align256(8);
-    l.bytes = o;
+SplatWs splat_ws(void* base, int64_t n) {
+    const int nb = bbox_blocks(n);
+    WsCarve w{(char*)base};
+    SplatWs l;
+    l.part = w.take<float>((size_t)(nb > 0 ? nb : 1) * 6);
+    l.total = w.take<unsigned long long>(1);
+    l.bytes = w.used;
     return l;
 }
 
-struct SolveLayout {
-    size_t chi[G2PC_MESH_DEPTH_MAX], rhs[G2PC_MESH_DEPTH_MAX], partial, bytes;
+// the coarse levels 1 .. depth - 2 of the multigrid
+struct SolveWs {
+    float *chi[G2PC_MESH_DEPTH_MAX], *rhs[G2PC_MESH_DEPTH_MAX];
+    double* partial;
+    size_t bytes;
 };
-SolveLayout solve_layout(int depth) {
-    SolveLayout l;
-    size_t o = 0;
+SolveWs solve_ws(void* base, int depth) {
+    WsCarve w{(char*)base};
+    SolveWs l;
     for (int lv = 1; lv <= depth - 2; ++lv) {
-        const size_t c = (size_t)cells_of(depth - lv) * sizeof(float);
-        l.chi[lv] = o; o += align256(c);
-        l.rhs[lv] = o; o += align256(c);
+        l.chi[lv] = w.take<float>(cells_of(depth - lv));
+        l.rhs[lv] = w.take<float>(cells_of(depth - lv));
     }
-    l.partial = o; o += align256(2 * RED_BLOCKS * sizeof(double));
-    l.bytes = o;
+    l.partial = w.take<double>(2 * RED_BLOCKS);
+    l.bytes = w.used;
     return l;
 }
 
-struct ExtractLayout {
-    size_t vblk, tblk, voff, toff, tmp, tmp_bytes, bytes;
+struct ExtractWs {
+    long long *vblk, *tblk, *voff, *toff;
+    void* tmp;
+    size_t tmp_bytes, bytes;
     int64_t nb;
 };
-ExtractLayout extract_layout(int depth) {
-    ExtractLayout l;
+ExtractWs extract_ws(void* base, int depth) {
+    ExtractWs l;
     l.nb = (cells_of(depth) + NODES_PER_CTA - 1) / NODES_PER_CTA;
-    const size_t a = align256((size_t)(l.nb + 1) * 8);
     size_t scan_b = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const long long*)nullptr, (long long*)nullptr, (int)(l.nb + 1));
-    size_t o = 0;
-    l.vblk = o; o += a;
-    l.tblk = o; o += a;
-    l.voff = o; o += a;
-    l.toff = o; o += a;
-    l.tmp = o; l.tmp_bytes = align256(scan_b); o += l.tmp_bytes;
-    l.bytes = o;
+    WsCarve w{(char*)base};
+    l.vblk = w.take<long long>(l.nb + 1);
+    l.tblk = w.take<long long>(l.nb + 1);
+    l.voff = w.take<long long>(l.nb + 1);
+    l.toff = w.take<long long>(l.nb + 1);
+    l.tmp_bytes = WsCarve::pad(scan_b);
+    l.tmp = w.take<char>(l.tmp_bytes);
+    l.bytes = w.used;
     return l;
 }
 
-struct GatherLayout {
-    size_t keys_a, keys_b, idx_a, idx_b, tmp, tmp_bytes, bytes;
+struct GatherWs {
+    uint32_t *keys_a, *keys_b, *idx_a, *idx_b;
+    void* tmp;
+    size_t tmp_bytes, bytes;
 };
-GatherLayout gather_layout(int64_t n) {
-    GatherLayout l;
+GatherWs gather_ws(void* base, int64_t n) {
     size_t sort_b = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const uint32_t*)nullptr, (uint32_t*)nullptr,
                                     (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, 0, 31);
-    const size_t a = align256((size_t)n * 4);
-    size_t o = 0;
-    l.keys_a = o; o += a;
-    l.keys_b = o; o += a;
-    l.idx_a = o; o += a;
-    l.idx_b = o; o += a;
-    l.tmp = o; l.tmp_bytes = align256(sort_b); o += l.tmp_bytes;
-    l.bytes = o;
+    WsCarve w{(char*)base};
+    GatherWs l;
+    l.keys_a = w.take<uint32_t>(n);
+    l.keys_b = w.take<uint32_t>(n);
+    l.idx_a = w.take<uint32_t>(n);
+    l.idx_b = w.take<uint32_t>(n);
+    l.tmp_bytes = WsCarve::pad(sort_b);
+    l.tmp = w.take<char>(l.tmp_bytes);
+    l.bytes = w.used;
     return l;
 }
 
-struct TrimLayout {
-    size_t sorted, thr, vflag, vmap, tflag, tmap, tmp, tmp_bytes, bytes;
+struct TrimWs {
+    double* sorted;
+    int32_t *vflag, *vmap, *tflag, *tmap;
+    void* tmp;
+    size_t tmp_bytes, bytes;
 };
-TrimLayout trim_layout(int64_t m, int64_t t) {
-    TrimLayout l;
+TrimWs trim_ws(void* base, int64_t m, int64_t t) {
     size_t sort_b = 0, scan_v = 0, scan_t = 0;
     cub::DeviceRadixSort::SortKeys(nullptr, sort_b, (const double*)nullptr, (double*)nullptr, (int)m);
     cub::DeviceScan::ExclusiveSum(nullptr, scan_v, (const int32_t*)nullptr, (int32_t*)nullptr, (int)m);
     cub::DeviceScan::ExclusiveSum(nullptr, scan_t, (const int32_t*)nullptr, (int32_t*)nullptr, (int)t);
     size_t tb = sort_b > scan_v ? sort_b : scan_v;
     tb = tb > scan_t ? tb : scan_t;
-    size_t o = 0;
-    l.sorted = o; o += align256((size_t)m * 8);
-    l.thr = o; o += align256(8);
-    l.vflag = o; o += align256((size_t)m * 4);
-    l.vmap = o; o += align256((size_t)m * 4);
-    l.tflag = o; o += align256((size_t)t * 4);
-    l.tmap = o; o += align256((size_t)t * 4);
-    l.tmp = o; l.tmp_bytes = align256(tb); o += l.tmp_bytes;
-    l.bytes = o;
+    WsCarve w{(char*)base};
+    TrimWs l;
+    l.sorted = w.take<double>(m);
+    w.take<double>(1);  // unused slot, kept so that the workspace size stays what callers were told
+    l.vflag = w.take<int32_t>(m);
+    l.vmap = w.take<int32_t>(m);
+    l.tflag = w.take<int32_t>(t);
+    l.tmap = w.take<int32_t>(t);
+    l.tmp_bytes = WsCarve::pad(tb);
+    l.tmp = w.take<char>(l.tmp_bytes);
+    l.bytes = w.used;
     return l;
 }
 
-// one-ring (smooth: e = 6t directed edges) or incidence (normals: e = 3t) lists
-struct ListLayout {
-    size_t keys_a, keys_b, row, pos, tmp, tmp_bytes, bytes;
+// one-ring (smooth: e = 6t directed edges, with the second position buffer) or incidence (normals: e = 3t) lists
+struct ListWs {
+    unsigned long long *keys_a, *keys_b;
+    int32_t* row;
+    double* pos;
+    void* tmp;
+    size_t tmp_bytes, bytes;
 };
-ListLayout list_layout(int64_t m, int64_t e, bool pos) {
-    ListLayout l;
+ListWs list_ws(void* base, int64_t m, int64_t e, bool pos) {
     size_t sort_b = 0;
     cub::DeviceRadixSort::SortKeys(nullptr, sort_b, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                    (int)e);
-    size_t o = 0;
-    l.keys_a = o; o += align256((size_t)e * 8);
-    l.keys_b = o; o += align256((size_t)e * 8);
-    l.row = o; o += align256((size_t)(m + 1) * 4);
-    l.pos = o; o += pos ? align256((size_t)m * 24) : 0;
-    l.tmp = o; l.tmp_bytes = align256(sort_b); o += l.tmp_bytes;
-    l.bytes = o;
+    WsCarve w{(char*)base};
+    ListWs l;
+    l.keys_a = w.take<unsigned long long>(e);
+    l.keys_b = w.take<unsigned long long>(e);
+    l.row = w.take<int32_t>(m + 1);
+    l.pos = w.take<double>(pos ? 3 * m : 0);
+    l.tmp_bytes = WsCarve::pad(sort_b);
+    l.tmp = w.take<char>(l.tmp_bytes);
+    l.bytes = w.used;
     return l;
 }
 
-// sort the keys of an e-entry list and bound its rows; returns the sorted buffer
-int build_lists(char* ws, const ListLayout& l, int64_t m, int64_t e, unsigned long long** sorted, cudaStream_t st) {
-    unsigned long long* ka = (unsigned long long*)(ws + l.keys_a);
-    unsigned long long* kb = (unsigned long long*)(ws + l.keys_b);
+// sort the keys of an e-entry list (from keys_a into keys_b) and bound its rows
+int build_lists(const ListWs& l, int64_t m, int64_t e, cudaStream_t st) {
     int end_bit = 33;  // the high word holds a vertex index < m <= 2^31
     while (end_bit < 64 && ((unsigned long long)m >> (end_bit - 32)) != 0) ++end_bit;
     size_t b = l.tmp_bytes;
-    if (e > 0) G2PC_CUDA(cub::DeviceRadixSort::SortKeys(ws + l.tmp, b, ka, kb, (int)e, 0, end_bit, st));
-    row_kernel<<<grid_of(m + 1), MB, 0, st>>>(kb, e, m, (int32_t*)(ws + l.row));
+    if (e > 0) G2PC_CUDA(cub::DeviceRadixSort::SortKeys(l.tmp, b, l.keys_a, l.keys_b, (int)e, 0, end_bit, st));
+    row_kernel<<<grid_of(m + 1), MB, 0, st>>>(l.keys_b, e, m, l.row);
     G2PC_CHECK_LAUNCH();
-    *sorted = kb;
     return G2PC_OK;
 }
 
 }  // namespace
 
 // ---- C ABI -----------------------------------------------------------------------------------------------------------
-extern "C" int64_t g2pc_mesh_splat_workspace_bytes(int64_t n) { return (int64_t)splat_layout(n).bytes; }
+extern "C" int64_t g2pc_mesh_splat_workspace_bytes(int64_t n) { return (int64_t)splat_ws(nullptr, n).bytes; }
 
 extern "C" int g2pc_mesh_splat(const float* xyz, const void* normals, int normal_dtype, int64_t n, int32_t depth,
                                double* frame, int64_t* B, uint32_t* cell, int32_t* status, void* workspace,
@@ -949,23 +911,20 @@ extern "C" int g2pc_mesh_splat(const float* xyz, const void* normals, int normal
     G2PC_CHECK_ARG(normal_dtype == G2PC_F32 || normal_dtype == G2PC_F64, "normals must be float32 or float64");
     G2PC_CHECK_ARG(frame && B && status && workspace, "null pointer");
     G2PC_CHECK_ARG(n == 0 || (xyz && normals && cell), "null pointer");
-    const SplatLayout l = splat_layout(n);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const SplatWs l = splat_ws(workspace, n);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
     const int R = 1 << depth;
     const int64_t cells = cells_of(depth);
-    float* part = (float*)(ws + l.part);
-    unsigned long long* total = (unsigned long long*)(ws + l.total);
+    const int nb = bbox_blocks(n);
     G2PC_CUDA(cudaMemsetAsync(status, 0, 2 * sizeof(int32_t), st));
     G2PC_CUDA(cudaMemsetAsync(B, 0, (size_t)cells * 8, st));
-    G2PC_CUDA(cudaMemsetAsync(total, 0, 8, st));
+    G2PC_CUDA(cudaMemsetAsync(l.total, 0, 8, st));
     if (n > 0) {
-        bbox_kernel<<<l.nb, MB, 0, st>>>(xyz, n, part);
+        bbox_kernel<<<nb, BBOX_THREADS, 0, st>>>(xyz, n, l.part);
         G2PC_CHECK_LAUNCH();
     }
-    frame_kernel<<<1, 1, 0, st>>>(part, n > 0 ? l.nb : 0, R, frame);
+    frame_kernel<<<1, 1, 0, st>>>(l.part, nb, R, frame);
     G2PC_CHECK_LAUNCH();
     if (n > 0) {
         unsigned long long* Bu = (unsigned long long*)B;
@@ -975,35 +934,33 @@ extern "C" int g2pc_mesh_splat(const float* xyz, const void* normals, int normal
             splat_kernel<double><<<grid_of(n), MB, 0, st>>>(xyz, (const double*)normals, n, R, frame, Bu, cell, status);
         G2PC_CHECK_LAUNCH();
     }
-    sum_b_kernel<<<RED_BLOCKS, MB, 0, st>>>((const long long*)B, cells, total);
+    sum_b_kernel<<<RED_BLOCKS, MB, 0, st>>>((const long long*)B, cells, l.total);
     G2PC_CHECK_LAUNCH();
-    mean_b_kernel<<<1, 1, 0, st>>>(total, cells, frame);
+    mean_b_kernel<<<1, 1, 0, st>>>(l.total, cells, frame);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }
 
 extern "C" int64_t g2pc_mesh_solve_workspace_bytes(int32_t depth) {
-    return depth_ok(depth) ? (int64_t)solve_layout(depth).bytes : 0;
+    return depth_ok(depth) ? (int64_t)solve_ws(nullptr, depth).bytes : 0;
 }
 
 extern "C" int g2pc_mesh_vcycle(const int64_t* B, const double* frame, int32_t depth, float* chi, int32_t first,
                                 double* norms, void* workspace, int64_t workspace_bytes, void* stream) {
     G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
     G2PC_CHECK_ARG(B && frame && chi && norms && workspace, "null pointer");
-    const SolveLayout l = solve_layout(depth);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const SolveWs l = solve_ws(workspace, depth);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
     const int R = 1 << depth, levels = depth - 2;  // level lv has R >> lv cells per axis; the last one has 4
-    double* partial = (double*)(ws + l.partial);
+    double* partial = l.partial;
     float* lchi[G2PC_MESH_DEPTH_MAX];
     Rhs lrhs[G2PC_MESH_DEPTH_MAX];
     lchi[0] = chi;
     lrhs[0] = Rhs{(const long long*)B, nullptr, frame};
     for (int lv = 1; lv <= levels; ++lv) {
-        lchi[lv] = (float*)(ws + l.chi[lv]);
-        lrhs[lv] = Rhs{nullptr, (const float*)(ws + l.rhs[lv]), frame};
+        lchi[lv] = l.chi[lv];
+        lrhs[lv] = Rhs{nullptr, l.rhs[lv], frame};
     }
     const Rhs rhs0 = lrhs[0];
     if (first) {
@@ -1044,7 +1001,7 @@ extern "C" int g2pc_mesh_vcycle(const int64_t* B, const double* frame, int32_t d
     return G2PC_OK;
 }
 
-extern "C" int64_t g2pc_mesh_iso_workspace_bytes(void) { return (int64_t)align256(2 * RED_BLOCKS * sizeof(double)); }
+extern "C" int64_t g2pc_mesh_iso_workspace_bytes(void) { return (int64_t)(2 * RED_BLOCKS * sizeof(double)); }
 
 extern "C" int g2pc_mesh_iso(const float* xyz, const uint32_t* cell, int64_t n, const double* frame, int32_t depth,
                              float* chi, double* iso, void* workspace, int64_t workspace_bytes, void* stream) {
@@ -1052,7 +1009,7 @@ extern "C" int g2pc_mesh_iso(const float* xyz, const uint32_t* cell, int64_t n, 
     G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
     G2PC_CHECK_ARG(frame && chi && iso && workspace, "null pointer");
     G2PC_CHECK_ARG(n == 0 || (xyz && cell), "null pointer");
-    G2PC_CHECK_ARG(workspace_bytes >= g2pc_mesh_iso_workspace_bytes(), "workspace too small");
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, g2pc_mesh_iso_workspace_bytes(), 8);
     cudaStream_t st = (cudaStream_t)stream;
     double* partial = (double*)workspace;
     const int R = 1 << depth;
@@ -1076,30 +1033,25 @@ extern "C" int g2pc_mesh_iso(const float* xyz, const uint32_t* cell, int64_t n, 
 }
 
 extern "C" int64_t g2pc_mesh_extract_workspace_bytes(int32_t depth) {
-    return depth_ok(depth) ? (int64_t)extract_layout(depth).bytes : 0;
+    return depth_ok(depth) ? (int64_t)extract_ws(nullptr, depth).bytes : 0;
 }
 
 extern "C" int g2pc_mesh_extract_count(const float* chi, int32_t depth, const double* iso, int64_t* counts,
                                        void* workspace, int64_t workspace_bytes, void* stream) {
     G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
     G2PC_CHECK_ARG(chi && iso && counts && workspace, "null pointer");
-    const ExtractLayout l = extract_layout(depth);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const ExtractWs l = extract_ws(workspace, depth);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
-    long long* vblk = (long long*)(ws + l.vblk);
-    long long* tblk = (long long*)(ws + l.tblk);
-    G2PC_CUDA(cudaMemsetAsync(vblk + l.nb, 0, 8, st));
-    G2PC_CUDA(cudaMemsetAsync(tblk + l.nb, 0, 8, st));
-    mt_count_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, 1 << depth, iso, vblk, tblk);
+    G2PC_CUDA(cudaMemsetAsync(l.vblk + l.nb, 0, 8, st));
+    G2PC_CUDA(cudaMemsetAsync(l.tblk + l.nb, 0, 8, st));
+    mt_count_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, 1 << depth, iso, l.vblk, l.tblk);
     G2PC_CHECK_LAUNCH();
     size_t b = l.tmp_bytes;
-    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, vblk, (long long*)(ws + l.voff), (int)(l.nb + 1), st));
+    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(l.tmp, b, l.vblk, l.voff, (int)(l.nb + 1), st));
     b = l.tmp_bytes;
-    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, tblk, (long long*)(ws + l.toff), (int)(l.nb + 1), st));
-    totals_kernel<<<1, 1, 0, st>>>((const long long*)(ws + l.voff), (const long long*)(ws + l.toff), l.nb,
-                                   (long long*)counts);
+    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(l.tmp, b, l.tblk, l.toff, (int)(l.nb + 1), st));
+    totals_kernel<<<1, 1, 0, st>>>(l.voff, l.toff, l.nb, (long long*)counts);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }
@@ -1110,24 +1062,22 @@ extern "C" int g2pc_mesh_extract_emit(const float* chi, int32_t depth, const dou
                                       void* stream) {
     G2PC_CHECK_ARG(depth_ok(depth), "depth must be in 2..G2PC_MESH_DEPTH_MAX");
     G2PC_CHECK_ARG(chi && frame && iso && node_scratch && workspace, "null pointer");
-    const ExtractLayout l = extract_layout(depth);
+    const ExtractWs l = extract_ws(const_cast<void*>(workspace), depth);  // read only here
     const int64_t cells = cells_of(depth);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     G2PC_CHECK_ARG(node_scratch_bytes >= 5 * cells, "node scratch too small (5 bytes per node)");
     cudaStream_t st = (cudaStream_t)stream;
-    const char* ws = (const char*)workspace;
     int32_t* base = (int32_t*)node_scratch;
     uint8_t* mask = (uint8_t*)node_scratch + 4 * cells;
     const int R = 1 << depth;
-    mt_vertex_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, R, frame, iso, (const long long*)(ws + l.voff), base, mask,
-                                                    (long long*)vkey, vt, vpos);
+    mt_vertex_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, R, frame, iso, l.voff, base, mask, (long long*)vkey, vt, vpos);
     G2PC_CHECK_LAUNCH();
-    mt_triangle_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, R, iso, (const long long*)(ws + l.toff), base, mask, faces);
+    mt_triangle_kernel<<<(unsigned)l.nb, MB, 0, st>>>(chi, R, iso, l.toff, base, mask, faces);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }
 
-extern "C" int64_t g2pc_mesh_gather_workspace_bytes(int64_t n) { return (int64_t)gather_layout(n).bytes; }
+extern "C" int64_t g2pc_mesh_gather_workspace_bytes(int64_t n) { return (int64_t)gather_ws(nullptr, n).bytes; }
 
 extern "C" int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const uint32_t* cell, int64_t n,
                                 const double* frame, int32_t depth, const int64_t* vkey, const double* vt, int64_t m,
@@ -1139,17 +1089,12 @@ extern "C" int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const 
     const int R = 1 << depth;
     const int64_t dual = (int64_t)(R - 1) * (R - 1) * (R - 1);
     G2PC_CHECK_ARG(cell_scratch_bytes >= 4 * dual, "cell scratch too small (4 bytes per dual cell)");
-    const GatherLayout l = gather_layout(n);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const GatherWs l = gather_ws(workspace, n);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     if (m == 0) return G2PC_OK;
     G2PC_CHECK_ARG(vkey && vt && density && (n == 0 || (xyz && cell)), "null pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
-    uint32_t* ka = (uint32_t*)(ws + l.keys_a);
-    uint32_t* kb = (uint32_t*)(ws + l.keys_b);
-    uint32_t* ia = (uint32_t*)(ws + l.idx_a);
-    uint32_t* ib = (uint32_t*)(ws + l.idx_b);
+    uint32_t *ka = l.keys_a, *kb = l.keys_b, *ia = l.idx_a, *ib = l.idx_b;
     int32_t* start = (int32_t*)cell_scratch;
     G2PC_CUDA(cudaMemsetAsync(start, 0xFF, (size_t)dual * 4, st));
     if (n > 0) {
@@ -1157,7 +1102,7 @@ extern "C" int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const 
         iota_kernel<<<grid_of(n), MB, 0, st>>>(ia, n);
         G2PC_CHECK_LAUNCH();
         size_t b = l.tmp_bytes;  // stable: a cell's points stay in input order
-        G2PC_CUDA(cub::DeviceRadixSort::SortPairs(ws + l.tmp, b, ka, kb, ia, ib, (int)n, 0, 31, st));
+        G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, ka, kb, ia, ib, (int)n, 0, 31, st));
         cell_start_kernel<<<grid_of(n), MB, 0, st>>>(kb, n, start);
         G2PC_CHECK_LAUNCH();
     }
@@ -1167,7 +1112,7 @@ extern "C" int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const 
     return G2PC_OK;
 }
 
-extern "C" int64_t g2pc_mesh_trim_workspace_bytes(int64_t m, int64_t t) { return (int64_t)trim_layout(m, t).bytes; }
+extern "C" int64_t g2pc_mesh_trim_workspace_bytes(int64_t m, int64_t t) { return (int64_t)trim_ws(nullptr, m, t).bytes; }
 
 extern "C" int g2pc_mesh_trim(const double* density, const double* vpos, const uint8_t* vcolours, int64_t m,
                               const int32_t* faces, int64_t t, uint8_t* keep, double* threshold, int64_t* counts,
@@ -1178,29 +1123,24 @@ extern "C" int g2pc_mesh_trim(const double* density, const double* vpos, const u
                    "null pointer");
     G2PC_CHECK_ARG(!vcolours == !vcolours_out, "vertex colours need an output");
     G2PC_CHECK_ARG(t == 0 || (faces && faces_out), "null pointer");
-    const TrimLayout l = trim_layout(m, t);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const TrimWs l = trim_ws(workspace, m, t);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
-    double* sorted = (double*)(ws + l.sorted);
-    int32_t* vflag = (int32_t*)(ws + l.vflag);
-    int32_t* vmap = (int32_t*)(ws + l.vmap);
-    int32_t* tflag = (int32_t*)(ws + l.tflag);
-    int32_t* tmap = (int32_t*)(ws + l.tmap);
+    double* sorted = l.sorted;
+    int32_t *vflag = l.vflag, *vmap = l.vmap, *tflag = l.tflag, *tmap = l.tmap;
     size_t b = l.tmp_bytes;
-    G2PC_CUDA(cub::DeviceRadixSort::SortKeys(ws + l.tmp, b, density, sorted, (int)m, 0, 64, st));
+    G2PC_CUDA(cub::DeviceRadixSort::SortKeys(l.tmp, b, density, sorted, (int)m, 0, 64, st));
     quantile_kernel<<<1, 1, 0, st>>>(sorted, m, threshold);
     G2PC_CHECK_LAUNCH();
     keep_kernel<<<grid_of(m), MB, 0, st>>>(density, m, threshold, keep, vflag);
     G2PC_CHECK_LAUNCH();
     b = l.tmp_bytes;
-    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, vflag, vmap, (int)m, st));
+    G2PC_CUDA(cub::DeviceScan::ExclusiveSum(l.tmp, b, vflag, vmap, (int)m, st));
     if (t > 0) {
         tri_flag_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, keep, tflag);
         G2PC_CHECK_LAUNCH();
         b = l.tmp_bytes;
-        G2PC_CUDA(cub::DeviceScan::ExclusiveSum(ws + l.tmp, b, tflag, tmap, (int)t, st));
+        G2PC_CUDA(cub::DeviceScan::ExclusiveSum(l.tmp, b, tflag, tmap, (int)t, st));
         compact_faces_kernel<<<grid_of(t), MB, 0, st>>>(faces, tflag, tmap, t, vmap, faces_out);
         G2PC_CHECK_LAUNCH();
     }
@@ -1213,7 +1153,7 @@ extern "C" int g2pc_mesh_trim(const double* density, const double* vpos, const u
 }
 
 extern "C" int64_t g2pc_mesh_smooth_workspace_bytes(int64_t m, int64_t t) {
-    return (int64_t)list_layout(m, 6 * t, true).bytes;
+    return (int64_t)list_ws(nullptr, m, 6 * t, true).bytes;
 }
 
 extern "C" int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, int64_t t, int32_t iterations,
@@ -1222,23 +1162,18 @@ extern "C" int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, i
     G2PC_CHECK_ARG(iterations >= 0, "iterations < 0");
     if (m == 0 || iterations == 0) return G2PC_OK;
     G2PC_CHECK_ARG(vpos && workspace && (t == 0 || faces), "null pointer");
-    const ListLayout l = list_layout(m, 6 * t, true);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const ListWs l = list_ws(workspace, m, 6 * t, true);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
     if (t > 0) {
-        ring_keys_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, (unsigned long long*)(ws + l.keys_a));
+        ring_keys_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, l.keys_a);
         G2PC_CHECK_LAUNCH();
     }
-    unsigned long long* keys;
-    if (build_lists(ws, l, m, 6 * t, &keys, st)) return G2PC_ERR_CUDA;
-    const int32_t* row = (const int32_t*)(ws + l.row);
-    double* other = (double*)(ws + l.pos);
+    if (build_lists(l, m, 6 * t, st)) return G2PC_ERR_CUDA;
     double* src = vpos;
-    double* dst = other;
+    double* dst = l.pos;
     for (int it = 0; it < iterations; ++it) {
-        smooth_kernel<<<grid_of(m), MB, 0, st>>>(src, m, keys, row, dst);
+        smooth_kernel<<<grid_of(m), MB, 0, st>>>(src, m, l.keys_b, l.row, dst);
         G2PC_CHECK_LAUNCH();
         double* x = src; src = dst; dst = x;
     }
@@ -1247,7 +1182,7 @@ extern "C" int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, i
 }
 
 extern "C" int64_t g2pc_mesh_normals_workspace_bytes(int64_t m, int64_t t) {
-    return (int64_t)list_layout(m, 3 * t, false).bytes;
+    return (int64_t)list_ws(nullptr, m, 3 * t, false).bytes;
 }
 
 extern "C" int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* faces, int64_t t, float* vertices,
@@ -1255,18 +1190,15 @@ extern "C" int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* f
     G2PC_CHECK_ARG(m >= 0 && m < 0x7FFFFFFFll && t >= 0 && 3 * t < 0x7FFFFFFFll, "bad sizes");
     if (m == 0) return G2PC_OK;
     G2PC_CHECK_ARG(vpos && vertices && normals && workspace && (t == 0 || faces), "null pointer");
-    const ListLayout l = list_layout(m, 3 * t, false);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.bytes, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    const ListWs l = list_ws(workspace, m, 3 * t, false);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
     cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
     if (t > 0) {
-        incidence_keys_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, (unsigned long long*)(ws + l.keys_a));
+        incidence_keys_kernel<<<grid_of(t), MB, 0, st>>>(faces, t, l.keys_a);
         G2PC_CHECK_LAUNCH();
     }
-    unsigned long long* keys;
-    if (build_lists(ws, l, m, 3 * t, &keys, st)) return G2PC_ERR_CUDA;
-    normals_kernel<<<grid_of(m), MB, 0, st>>>(vpos, m, faces, keys, (const int32_t*)(ws + l.row), vertices, normals);
+    if (build_lists(l, m, 3 * t, st)) return G2PC_ERR_CUDA;
+    normals_kernel<<<grid_of(m), MB, 0, st>>>(vpos, m, faces, l.keys_b, l.row, vertices, normals);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }

@@ -10,7 +10,7 @@
 // index list; g2pc_gather_rows compacts any number of row-major arrays through that list (the host reads the count once
 // to size the outputs).  The magnitude chain is one kernel + a fixed-order reduction (deterministic sum), the point
 // budget three small kernels — no `.item()` on the way (the reference syncs at :87 and inside every boolean index).
-#include "common.cuh"
+#include "cloud_common.cuh"
 
 namespace {
 
@@ -142,30 +142,16 @@ __global__ void __launch_bounds__(256) magnitudes_kernel(const float* __restrict
         m = (double)(area * contrib[base + threadIdx.x]);
         mag[base + threadIdx.x] = m;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
-    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = m;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0.0;
-        for (int w = 0; w < 8; ++w) t += s_w[w];
-        partial[blockIdx.x] = t;
-    }
+    const double t = block_sum_f64<256>(m, s_w);
+    if (threadIdx.x == 0) partial[blockIdx.x] = t;
 }
 
 // fixed-order sum of the partials (one CTA): sum[0]
 __global__ void __launch_bounds__(1024) sum_partials_kernel(const double* __restrict__ partial, int32_t nb,
                                                             double* __restrict__ sum) {
     __shared__ double s[1024];
-    double t = 0.0;
-    for (int i = threadIdx.x; i < nb; i += 1024) t += partial[i];
-    s[threadIdx.x] = t;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) sum[0] = s[0];
+    const double t = sum_partials_f64(partial, nb, s);
+    if (threadIdx.x == 0) sum[0] = t;
 }
 
 // ppg = rint(mag * (P / sum)) (torch.round = round half to even); per-CTA (sum of ppg, zero count)
@@ -236,6 +222,27 @@ __global__ void __launch_bounds__(256) ppg_fix_kernel(int32_t* __restrict__ ppg,
     if (zero && before + __popc(m & ((1u << lane) - 1u)) < take[0]) ppg[i] = 1;
 }
 
+// workspace of g2pc_points_per_gaussian; a null base only sizes it
+struct PpgWs {
+    double* partial;  // per-CTA magnitude sums
+    long long* blk;   // per-CTA (sum of ppg, zero count), then the zero counts' exclusive scan
+    double* sum;
+    long long* take;
+    size_t bytes;
+};
+
+PpgWs ppg_ws(void* base, int64_t n) {
+    const size_t nb = (size_t)((n + 255) / 256);
+    WsCarve w{(char*)base};
+    PpgWs l;
+    l.partial = w.take<double>(nb);
+    l.blk = w.take<long long>(2 * nb);
+    l.sum = w.take<double>(1);
+    l.take = w.take<long long>(1);
+    l.bytes = w.used;
+    return l;
+}
+
 }  // namespace
 
 extern "C" int64_t g2pc_cull_workspace_bytes(int64_t n) {
@@ -250,7 +257,7 @@ extern "C" int g2pc_cull_select(const float* max_contrib, float vis_threshold, c
     G2PC_CHECK_ARG(n >= 0, "n < 0");
     G2PC_CHECK_ARG(index || n == 0, "null index");
     G2PC_CHECK_ARG(count && workspace, "null pointer");
-    G2PC_CHECK_ARG(workspace_bytes >= g2pc_cull_workspace_bytes(n), "workspace too small");
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, g2pc_cull_workspace_bytes(n), 4);
     G2PC_CHECK_ARG(n < 0x7FFFFFFFll, "n must fit int32 indices");
     G2PC_CHECK_ARG(!(bbox_min3_host || bbox_max3_host) || xyz, "bounding box needs xyz");
     G2PC_CHECK_ARG((surface_dist == nullptr) == (surface_threshold_dev == nullptr), "surface distance needs its threshold");
@@ -289,10 +296,7 @@ extern "C" int g2pc_gather_rows(const int32_t* index, int64_t m, int32_t num_arr
     return G2PC_OK;
 }
 
-extern "C" int64_t g2pc_ppg_workspace_bytes(int64_t n) {
-    const int64_t nb = (n + 255) / 256;
-    return (int64_t)(nb * sizeof(double) + 2 * nb * sizeof(long long) + 4 * sizeof(double));
-}
+extern "C" int64_t g2pc_ppg_workspace_bytes(int64_t n) { return (int64_t)ppg_ws(nullptr, n).bytes; }
 
 /* magnitudes (n float64) and points per Gaussian (n int32) from covariances (n,3,3) f32 and contributions (n) f32. */
 extern "C" int g2pc_points_per_gaussian(const float* cov, const float* contrib, int64_t n, double num_points,
@@ -301,23 +305,19 @@ extern "C" int g2pc_points_per_gaussian(const float* cov, const float* contrib, 
     G2PC_CHECK_ARG(n >= 0, "n < 0");
     if (n == 0) return G2PC_OK;
     G2PC_CHECK_ARG(cov && contrib && magnitudes && ppg && workspace, "null pointer");
-    G2PC_CHECK_ARG(workspace_bytes >= g2pc_ppg_workspace_bytes(n), "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 7) == 0, "workspace must be 8-byte aligned");
+    const PpgWs l = ppg_ws(workspace, n);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 8);
     cudaStream_t st = (cudaStream_t)stream;
     const int nb = (int)((n + 255) / 256);
-    double* partial = (double*)workspace;
-    long long* blk = (long long*)(partial + nb);
-    double* sum = (double*)(blk + 2 * (int64_t)nb);
-    long long* take = (long long*)(sum + 1);
-    magnitudes_kernel<<<nb, 256, 0, st>>>(cov, contrib, n, magnitudes, partial);
+    magnitudes_kernel<<<nb, 256, 0, st>>>(cov, contrib, n, magnitudes, l.partial);
     G2PC_CHECK_LAUNCH();
-    sum_partials_kernel<<<1, 1024, 0, st>>>(partial, nb, sum);
+    sum_partials_kernel<<<1, 1024, 0, st>>>(l.partial, nb, l.sum);
     G2PC_CHECK_LAUNCH();
-    ppg_round_kernel<<<nb, 256, 0, st>>>(magnitudes, sum, num_points, n, ppg, blk);
+    ppg_round_kernel<<<nb, 256, 0, st>>>(magnitudes, l.sum, num_points, n, ppg, l.blk);
     G2PC_CHECK_LAUNCH();
-    ppg_plan_kernel<<<1, 1024, 0, st>>>(blk, nb, num_points, take);
+    ppg_plan_kernel<<<1, 1024, 0, st>>>(l.blk, nb, num_points, l.take);
     G2PC_CHECK_LAUNCH();
-    ppg_fix_kernel<<<nb, 256, 0, st>>>(ppg, blk, take, n);
+    ppg_fix_kernel<<<nb, 256, 0, st>>>(ppg, l.blk, l.take, n);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }

@@ -21,7 +21,7 @@
 // Box distances are lowered by a margin of E * 2^-48, which covers the rounding of the quantisation and of the distance
 // arithmetic, so a cell is skipped only when no point in it can enter the list: the result is exact.
 #include <cub/cub.cuh>
-#include "common.cuh"
+#include "cloud_common.cuh"
 
 namespace {
 
@@ -32,8 +32,7 @@ constexpr int WIN = 2 * K_MAX;     // a run of >= k exact copies through the que
 constexpr int LEAF_T = 32;         // a cell with at most this many points is scanned, a larger one is entered
 constexpr int QBITS = 42;          // quantisation bits per axis (deepest octree level)
 constexpr int QB = 128;            // query threads per CTA
-constexpr int BB = 256;            // bounding-box / key / gather threads per CTA
-constexpr int BOX_PER_CTA = BB * 8;
+constexpr int BB = 256;            // key / gather threads per CTA
 constexpr uint64_t MASK21 = (1ull << 21) - 1;
 constexpr uint64_t KEY_NONFINITE = (1ull << 63) - 1;  // non-finite points sort last and are nobody's neighbour
 
@@ -43,10 +42,6 @@ struct Frame {
     double edge;    // E: power of two >= the largest bounding-box extent
     double margin;  // E * 2^-48
 };
-
-__host__ __device__ __forceinline__ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-__device__ __forceinline__ bool finite3(float x, float y, float z) { return isfinite(x) && isfinite(y) && isfinite(z); }
 
 // 21-bit integer -> every third bit of 63
 __device__ __forceinline__ uint64_t spread3(uint64_t v) {
@@ -68,43 +63,10 @@ __device__ __forceinline__ u128 key126(uint64_t x, uint64_t y, uint64_t z) {
     return (u128)morton63(x >> 21, y >> 21, z >> 21) << 63 | morton63(x & MASK21, y & MASK21, z & MASK21);
 }
 
-// per-CTA min / max of the finite coordinates: part[6 * b ..] = (min x, min y, min z, max x, max y, max z)
-__global__ void __launch_bounds__(BB) bbox_kernel(const float* __restrict__ xyz, int64_t n, float* __restrict__ part) {
-    __shared__ float s[6][BB / 32];
-    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
-    const int64_t base = (int64_t)blockIdx.x * BOX_PER_CTA;
-    for (int r = 0; r < BOX_PER_CTA / BB; ++r) {
-        const int64_t i = base + r * BB + threadIdx.x;
-        if (i >= n) break;
-        const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-        if (!finite3(x, y, z)) continue;
-        mn[0] = fminf(mn[0], x); mn[1] = fminf(mn[1], y); mn[2] = fminf(mn[2], z);
-        mx[0] = fmaxf(mx[0], x); mx[1] = fmaxf(mx[1], y); mx[2] = fmaxf(mx[2], z);
-    }
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-    }
-    if ((threadIdx.x & 31) == 0) {
-        for (int a = 0; a < 3; ++a) { s[a][threadIdx.x >> 5] = mn[a]; s[3 + a][threadIdx.x >> 5] = mx[a]; }
-    }
-    __syncthreads();
-    if (threadIdx.x < 6) {
-        float v = s[threadIdx.x][0];
-        for (int w = 1; w < BB / 32; ++w) v = threadIdx.x < 3 ? fminf(v, s[threadIdx.x][w]) : fmaxf(v, s[threadIdx.x][w]);
-        part[6 * blockIdx.x + threadIdx.x] = v;
-    }
-}
-
 // one thread: fold the per-CTA boxes into the quantisation frame
 __global__ void frame_kernel(const float* __restrict__ part, int nb, Frame* __restrict__ fr) {
-    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
-    for (int b = 0; b < nb; ++b)
-        for (int a = 0; a < 3; ++a) { mn[a] = fminf(mn[a], part[6 * b + a]); mx[a] = fmaxf(mx[a], part[6 * b + 3 + a]); }
+    float mn[3], mx[3];
+    fold_bbox(part, nb, mn, mx);
     Frame f;
     double ext = 0.0;
     if (mn[0] <= mx[0]) {
@@ -282,15 +244,8 @@ __global__ void __launch_bounds__(SB) sor_partial_kernel(const double* __restric
         const double x = avg[i];
         if (x > 0.0) v = __dadd_rn(v, PASS == 0 ? x : __dmul_rn(x - mean, x - mean));
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double tot = 0.0;
-        for (int w = 0; w < SB / 32; ++w) tot = __dadd_rn(tot, s_w[w]);
-        partial[blockIdx.x] = tot;
-    }
+    const double tot = block_sum_f64<SB>(v, s_w);
+    if (threadIdx.x == 0) partial[blockIdx.x] = tot;
 }
 
 // one CTA: fixed-order sum of the partials; pass 0 -> stats[0] = mean, pass 1 -> stats[1] = std, stats[2] = threshold.
@@ -299,19 +254,12 @@ template <int PASS>
 __global__ void __launch_bounds__(1024) sor_finish_kernel(const double* __restrict__ partial, int nb, int64_t n,
                                                           double std_ratio, double* __restrict__ stats) {
     __shared__ double s[1024];
-    double t = 0.0;
-    for (int i = threadIdx.x; i < nb; i += 1024) t = __dadd_rn(t, partial[i]);
-    s[threadIdx.x] = t;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (threadIdx.x < o) s[threadIdx.x] = __dadd_rn(s[threadIdx.x], s[threadIdx.x + o]);
-        __syncthreads();
-    }
+    const double t = sum_partials_f64(partial, nb, s);
     if (threadIdx.x == 0) {
         if (PASS == 0) {
-            stats[0] = s[0] / (double)n;
+            stats[0] = t / (double)n;
         } else {
-            const double sd = sqrt(s[0] / (double)(n - 1));  // n == 1: 0 / 0 = NaN, nothing is kept
+            const double sd = sqrt(t / (double)(n - 1));  // n == 1: 0 / 0 = NaN, nothing is kept
             stats[1] = sd;
             stats[2] = __dadd_rn(stats[0], __dmul_rn(std_ratio, sd));
         }
@@ -326,35 +274,42 @@ __global__ void __launch_bounds__(SB) sor_keep_kernel(const double* __restrict__
     keep[i] = (x > 0.0 && x < stats[2]) ? 1 : 0;
 }
 
-// workspace layout of g2pc_knn_mean_dist
-struct KnnLayout {
-    size_t frame, part, hi, lo, keys, idx_a, idx_b, pts, tmp, tmp_bytes, total;
+// workspace of g2pc_knn_mean_dist; a null base only sizes it
+struct KnnWs {
+    Frame* fr;
+    float* part;
+    uint64_t *hi, *lo;
+    uint64_t *lo_by_lo, *hi_by_lo;  // sort 1 output keys and hi gathered in that order; later the (lo, hi) key pairs
+    uint32_t *idx_a, *idx_b;
+    float4* pts;
+    void* tmp;
+    size_t tmp_bytes, bytes;
 };
 
-KnnLayout knn_layout(int64_t n) {
-    KnnLayout l;
+KnnWs knn_ws(void* base, int64_t n) {
     size_t sort_b = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const uint64_t*)nullptr, (uint64_t*)nullptr,
                                     (const uint32_t*)nullptr, (uint32_t*)nullptr, n, 0, 63);
-    const size_t nb = (size_t)((n + BOX_PER_CTA - 1) / BOX_PER_CTA);
-    const size_t un = (size_t)n;
-    size_t o = 0;
-    l.frame = o; o += align256(sizeof(Frame));
-    l.part = o; o += align256(nb * 6 * sizeof(float));
-    l.hi = o; o += align256(un * 8);
-    l.lo = o; o += align256(un * 8);
-    l.keys = o; o += 2 * align256(un * 8);  // first the two 8n-byte sort buffers, then the (lo, hi) key pairs
-    l.idx_a = o; o += align256(un * 4);
-    l.idx_b = o; o += align256(un * 4);
-    l.pts = o; o += align256(un * 16);
-    l.tmp = o; l.tmp_bytes = align256(sort_b); o += l.tmp_bytes;
-    l.total = o;
+    WsCarve w{(char*)base};
+    KnnWs l;
+    l.fr = w.take<Frame>(1);
+    l.part = w.take<float>((size_t)bbox_blocks(n) * 6);
+    l.hi = w.take<uint64_t>(n);
+    l.lo = w.take<uint64_t>(n);
+    l.lo_by_lo = w.take<uint64_t>(n);  // adjacent to hi_by_lo: together at least 16n bytes for the key pairs
+    l.hi_by_lo = w.take<uint64_t>(n);
+    l.idx_a = w.take<uint32_t>(n);
+    l.idx_b = w.take<uint32_t>(n);
+    l.pts = w.take<float4>(n);
+    l.tmp_bytes = WsCarve::pad(sort_b);
+    l.tmp = w.take<char>(l.tmp_bytes);
+    l.bytes = w.used;
     return l;
 }
 
 }  // namespace
 
-extern "C" int64_t g2pc_knn_workspace_bytes(int64_t n) { return n <= 0 ? 0 : (int64_t)knn_layout(n).total; }
+extern "C" int64_t g2pc_knn_workspace_bytes(int64_t n) { return n <= 0 ? 0 : (int64_t)knn_ws(nullptr, n).bytes; }
 
 extern "C" int g2pc_knn_mean_dist(const float* xyz, int64_t n, int32_t k, double* avg, int32_t* status, void* workspace,
                                   int64_t workspace_bytes, void* stream) {
@@ -366,40 +321,28 @@ extern "C" int g2pc_knn_mean_dist(const float* xyz, int64_t n, int32_t k, double
     G2PC_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
     if (n == 0) return G2PC_OK;
     G2PC_CHECK_ARG(xyz && avg && workspace, "null pointer");
-    const KnnLayout l = knn_layout(n);
-    G2PC_CHECK_ARG(workspace_bytes >= (int64_t)l.total, "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
-    char* ws = (char*)workspace;
-    Frame* fr = (Frame*)(ws + l.frame);
-    float* part = (float*)(ws + l.part);
-    uint64_t* hi = (uint64_t*)(ws + l.hi);
-    uint64_t* lo = (uint64_t*)(ws + l.lo);
-    uint64_t* lo_by_lo = (uint64_t*)(ws + l.keys);               // sort 1 output keys
-    uint64_t* hi_by_lo = (uint64_t*)(ws + l.keys + align256((size_t)n * 8));  // hi gathered in that order
-    uint64_t* hi_sorted = hi;                                      // sort 2 output keys (hi is dead by then)
-    ulonglong2* keys = (ulonglong2*)(ws + l.keys);
-    uint32_t* idx_a = (uint32_t*)(ws + l.idx_a);
-    uint32_t* idx_b = (uint32_t*)(ws + l.idx_b);
-    float4* pts = (float4*)(ws + l.pts);
-    void* tmp = ws + l.tmp;
-    const int nbox = (int)((n + BOX_PER_CTA - 1) / BOX_PER_CTA);
+    const KnnWs l = knn_ws(workspace, n);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
+    uint64_t* hi_sorted = l.hi;                          // sort 2 output keys (hi is dead by then)
+    ulonglong2* keys = (ulonglong2*)l.lo_by_lo;          // both sort 1 buffers are dead by then
+    const int nbox = bbox_blocks(n);
     const unsigned g = (unsigned)((n + BB - 1) / BB);
 
-    bbox_kernel<<<nbox, BB, 0, st>>>(xyz, n, part);
+    bbox_kernel<<<nbox, BBOX_THREADS, 0, st>>>(xyz, n, l.part);
     G2PC_CHECK_LAUNCH();
-    frame_kernel<<<1, 1, 0, st>>>(part, nbox, fr);
+    frame_kernel<<<1, 1, 0, st>>>(l.part, nbox, l.fr);
     G2PC_CHECK_LAUNCH();
-    key_kernel<<<g, BB, 0, st>>>(xyz, n, fr, hi, lo, idx_a, status);
+    key_kernel<<<g, BB, 0, st>>>(xyz, n, l.fr, l.hi, l.lo, l.idx_a, status);
     G2PC_CHECK_LAUNCH();
     size_t b = l.tmp_bytes;
-    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, lo, lo_by_lo, idx_a, idx_b, n, 0, 63, st));
-    gather_u64_kernel<<<g, BB, 0, st>>>(hi, idx_b, n, hi_by_lo);
+    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, l.lo, l.lo_by_lo, l.idx_a, l.idx_b, n, 0, 63, st));
+    gather_u64_kernel<<<g, BB, 0, st>>>(l.hi, l.idx_b, n, l.hi_by_lo);
     G2PC_CHECK_LAUNCH();
     b = l.tmp_bytes;  // stable: points with equal hi keep their lo order
-    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, hi_by_lo, hi_sorted, idx_b, idx_a, n, 0, 63, st));
-    gather_sorted_kernel<<<g, BB, 0, st>>>(hi_sorted, lo, idx_a, xyz, n, keys, pts);
+    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, l.hi_by_lo, hi_sorted, l.idx_b, l.idx_a, n, 0, 63, st));
+    gather_sorted_kernel<<<g, BB, 0, st>>>(hi_sorted, l.lo, l.idx_a, xyz, n, keys, l.pts);
     G2PC_CHECK_LAUNCH();
-    knn_kernel<<<(unsigned)((n + QB - 1) / QB), QB, 0, st>>>(keys, pts, idx_a, fr, (int)n, k, avg);
+    knn_kernel<<<(unsigned)((n + QB - 1) / QB), QB, 0, st>>>(keys, l.pts, l.idx_a, l.fr, (int)n, k, avg);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }
@@ -414,8 +357,7 @@ extern "C" int g2pc_sor_mask(const double* avg, int64_t n, double std_ratio, uin
     G2PC_CHECK_ARG(std_ratio > 0.0, "std_ratio must be > 0");
     if (n == 0) return G2PC_OK;
     G2PC_CHECK_ARG(avg && keep && stats && workspace, "null pointer");
-    G2PC_CHECK_ARG(workspace_bytes >= g2pc_sor_workspace_bytes(n), "workspace too small");
-    G2PC_CHECK_ARG(((uintptr_t)workspace & 7) == 0, "workspace must be 8-byte aligned");
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, g2pc_sor_workspace_bytes(n), 8);
     cudaStream_t st = (cudaStream_t)stream;
     const int nb = (int)((n + SOR_PER_CTA - 1) / SOR_PER_CTA);
     double* partial = (double*)workspace;

@@ -156,13 +156,9 @@ _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sor
                 "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_sor_mask": 5, "g2pc_mesh_splat": 5,
                 "g2pc_mesh_iso": 7, "g2pc_mesh_extract_count": 2, "g2pc_mesh_extract_emit": 2, "g2pc_mesh_gather": 3,
                 "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3}
+# host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",
-                "g2pc_multisplit_rows", "g2pc_blend_set_compact", "g2pc_cull_workspace_bytes", "g2pc_ppg_workspace_bytes",
-                "g2pc_depth_sort_workspace_bytes", "g2pc_knn_workspace_bytes", "g2pc_sor_workspace_bytes",
-                "g2pc_mesh_splat_workspace_bytes", "g2pc_mesh_solve_workspace_bytes", "g2pc_mesh_iso_workspace_bytes",
-                "g2pc_mesh_extract_workspace_bytes", "g2pc_mesh_gather_workspace_bytes",
-                "g2pc_mesh_trim_workspace_bytes", "g2pc_mesh_smooth_workspace_bytes",
-                "g2pc_mesh_normals_workspace_bytes"}
+                "g2pc_multisplit_rows", "g2pc_blend_set_compact"}
 
 
 def call(name, *args):
@@ -170,7 +166,7 @@ def call(name, *args):
     dict — bracket it with CUDA events on the current stream."""
     global LAUNCHES
     fn = getattr(load(), name)
-    if TIMING is not None and name not in _NOT_KERNELS:
+    if TIMING is not None and name not in _NOT_KERNELS and not name.endswith("_workspace_bytes"):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         status = fn(*args)
@@ -193,6 +189,12 @@ def ptr(t):
     if t is None:
         return None
     return t.data_ptr()
+
+
+def workspace(nbytes, device):
+    """Scratch for an entry point's workspace argument: a uint8 tensor of at least nbytes, and of at least 256 bytes, so
+    that it is never empty (an empty tensor's NULL pointer is refused).  Pass its numel() as the size."""
+    return torch.empty((max(int(nbytes), 256),), dtype=torch.uint8, device=device)
 
 
 def stream_ptr(device=None):

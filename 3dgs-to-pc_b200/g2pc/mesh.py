@@ -25,10 +25,6 @@ NB_NEIGHBORS = 20
 Mesh = collections.namedtuple("Mesh", ["vertices", "faces", "colours", "normals", "densities"])
 
 
-def _ws(nbytes, dev):
-    return torch.empty((max(int(nbytes), 256),), dtype=torch.uint8, device=dev)
-
-
 @contextlib.contextmanager
 def _phase(timings, name):
     """Brackets a phase with CUDA events on the current stream when `timings` is a dict."""
@@ -50,7 +46,7 @@ def splat(points, normals, depth):
     B = torch.empty((R ** 3,), dtype=torch.int64, device=dev)
     cell = torch.empty((n,), dtype=torch.int32, device=dev)
     status = torch.empty((2,), dtype=torch.int32, device=dev)
-    ws = _ws(capi.load().g2pc_mesh_splat_workspace_bytes(n), dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_splat_workspace_bytes(n), dev)
     capi.call("g2pc_mesh_splat", capi.ptr(points), capi.ptr(normals), capi.dtype_code(normals), n, depth,
               capi.ptr(frame), capi.ptr(B), capi.ptr(cell), capi.ptr(status), capi.ptr(ws), ws.numel(),
               capi.stream_ptr(dev))
@@ -62,7 +58,7 @@ def solve(B, frame, depth, max_cycles=MAX_CYCLES, tol=TOLERANCE):
     dev = B.device
     chi = torch.empty((1 << (3 * depth),), dtype=torch.float32, device=dev)
     norms = torch.zeros((2,), dtype=torch.float64, device=dev)
-    ws = _ws(capi.load().g2pc_mesh_solve_workspace_bytes(depth), dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_solve_workspace_bytes(depth), dev)
     st = capi.stream_ptr(dev)
     ratio, cycles = 0.0, 0
     for c in range(max_cycles):
@@ -82,7 +78,7 @@ def iso_value(points, cell, frame, depth, chi):
     """Subtracts the mean of chi in place; returns iso (3,) float64 on the device: (that mean, iso, used points)."""
     dev = points.device
     iso = torch.empty((3,), dtype=torch.float64, device=dev)
-    ws = _ws(capi.load().g2pc_mesh_iso_workspace_bytes(), dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_iso_workspace_bytes(), dev)
     capi.call("g2pc_mesh_iso", capi.ptr(points), capi.ptr(cell), points.shape[0], capi.ptr(frame), depth, capi.ptr(chi),
               capi.ptr(iso), capi.ptr(ws), ws.numel(), capi.stream_ptr(dev))
     return iso
@@ -92,7 +88,7 @@ def extract(chi, depth, frame, iso, node_scratch):
     """Marching tetrahedra: vkey (m,) int64, vt (m,) float64, vpos (m,3) float64, faces (t,3) int32.  node_scratch: a
     CUDA tensor of at least 5 bytes per node (its contents are overwritten)."""
     dev = chi.device
-    ws = _ws(capi.load().g2pc_mesh_extract_workspace_bytes(depth), dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_extract_workspace_bytes(depth), dev)
     counts = torch.empty((2,), dtype=torch.int64, device=dev)
     st = capi.stream_ptr(dev)
     capi.call("g2pc_mesh_extract_count", capi.ptr(chi), depth, capi.ptr(iso), capi.ptr(counts), capi.ptr(ws),
@@ -116,7 +112,7 @@ def gather(points, colours, cell, frame, depth, vkey, vt, cell_scratch):
     dev, n, m = points.device, points.shape[0], vkey.shape[0]
     dens = torch.empty((m,), dtype=torch.float64, device=dev)
     vcol = torch.empty((m, 3), dtype=torch.uint8, device=dev) if colours is not None else None
-    ws = _ws(capi.load().g2pc_mesh_gather_workspace_bytes(n), dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_gather_workspace_bytes(n), dev)
     capi.call("g2pc_mesh_gather", capi.ptr(points), capi.ptr(colours), capi.ptr(cell), n, capi.ptr(frame), depth,
               capi.ptr(vkey), capi.ptr(vt), m, capi.ptr(cell_scratch),
               cell_scratch.numel() * cell_scratch.element_size(), capi.ptr(dens), capi.ptr(vcol), capi.ptr(ws),
@@ -133,7 +129,7 @@ def trim(dens, vpos, vcol, faces):
     counts = torch.empty((2,), dtype=torch.int64, device=dev)
     outs = [torch.empty_like(dens), torch.empty_like(vpos), torch.empty_like(vcol) if vcol is not None else None,
             torch.empty_like(faces)]
-    ws = _ws(capi.load().g2pc_mesh_trim_workspace_bytes(m, t), dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_trim_workspace_bytes(m, t), dev)
     capi.call("g2pc_mesh_trim", capi.ptr(dens), capi.ptr(vpos), capi.ptr(vcol), m, capi.ptr(faces), t, capi.ptr(keep),
               capi.ptr(thr), capi.ptr(counts), *[capi.ptr(o) for o in outs], capi.ptr(ws), ws.numel(),
               capi.stream_ptr(dev))
@@ -147,7 +143,7 @@ def smooth(vpos, faces, iterations):
     m, t = vpos.shape[0], faces.shape[0]
     if m == 0 or iterations == 0:
         return vpos
-    ws = _ws(capi.load().g2pc_mesh_smooth_workspace_bytes(m, t), vpos.device)
+    ws = capi.workspace(capi.load().g2pc_mesh_smooth_workspace_bytes(m, t), vpos.device)
     capi.call("g2pc_mesh_smooth", capi.ptr(vpos), m, capi.ptr(faces), t, int(iterations), capi.ptr(ws), ws.numel(),
               capi.stream_ptr(vpos.device))
     return vpos
@@ -159,7 +155,7 @@ def vertex_normals(vpos, faces):
     v = torch.empty((m, 3), dtype=torch.float32, device=dev)
     nrm = torch.empty((m, 3), dtype=torch.float32, device=dev)
     if m:
-        ws = _ws(capi.load().g2pc_mesh_normals_workspace_bytes(m, t), dev)
+        ws = capi.workspace(capi.load().g2pc_mesh_normals_workspace_bytes(m, t), dev)
         capi.call("g2pc_mesh_normals", capi.ptr(vpos), m, capi.ptr(faces), t, capi.ptr(v), capi.ptr(nrm), capi.ptr(ws),
                   ws.numel(), capi.stream_ptr(dev))
     return v, nrm

@@ -20,7 +20,7 @@ def mean_distances(xyz, k):
     n = xyz.shape[0]
     avg = torch.empty((n,), dtype=torch.float64, device=xyz.device)
     status = torch.empty((1,), dtype=torch.int32, device=xyz.device)
-    ws = torch.empty((max(int(capi.load().g2pc_knn_workspace_bytes(n)), 256),), dtype=torch.uint8, device=xyz.device)
+    ws = capi.workspace(capi.load().g2pc_knn_workspace_bytes(n), xyz.device)
     capi.call("g2pc_knn_mean_dist", capi.ptr(xyz), n, int(k), capi.ptr(avg), capi.ptr(status), capi.ptr(ws),
               ws.numel(), capi.stream_ptr(xyz.device))
     return avg, status
@@ -31,10 +31,9 @@ def sor_mask(avg, std_ratio):
     n = avg.shape[0]
     keep = torch.empty((n,), dtype=torch.uint8, device=avg.device)
     stats = torch.full((3,), float("nan"), dtype=torch.float64, device=avg.device)
-    ws = torch.empty((max(int(capi.load().g2pc_sor_workspace_bytes(n)), 8) // 8,), dtype=torch.float64,
-                     device=avg.device)
+    ws = capi.workspace(capi.load().g2pc_sor_workspace_bytes(n), avg.device)
     capi.call("g2pc_sor_mask", capi.ptr(avg), n, float(std_ratio), capi.ptr(keep), capi.ptr(stats), capi.ptr(ws),
-              ws.numel() * 8, capi.stream_ptr(avg.device))
+              ws.numel(), capi.stream_ptr(avg.device))
     return keep, stats
 
 
@@ -64,7 +63,7 @@ def remove_statistical_outliers(points, colours, normals, nb_neighbors=20, std_r
 
     index = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
     count = torch.zeros((1,), dtype=torch.int64, device=dev)
-    ws = torch.empty((max(int(capi.load().g2pc_cull_workspace_bytes(n)), 8),), dtype=torch.uint8, device=dev)
+    ws = capi.workspace(capi.load().g2pc_cull_workspace_bytes(n), dev)
     st = capi.stream_ptr(dev)
     capi.call("g2pc_cull_select", None, 0.0, None, 0.0, None, None, None, None, None, capi.ptr(keep), 0, n, n,
               capi.ptr(index), capi.ptr(count), capi.ptr(ws), ws.numel(), st)

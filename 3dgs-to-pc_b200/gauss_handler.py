@@ -155,7 +155,7 @@ class Gaussians():
         lo, hi = (0, n) if index_range is None else index_range
         index = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
         count = torch.zeros((1,), dtype=torch.int64, device=dev)
-        ws = torch.empty((max(int(capi.load().g2pc_cull_workspace_bytes(n)), 8),), dtype=torch.uint8, device=dev)
+        ws = capi.workspace(capi.load().g2pc_cull_workspace_bytes(n), dev)
         capi.call("g2pc_cull_select", capi.ptr(mc), float(visibility_threshold), capi.ptr(op), float(min_opacity),
                   capi.ptr(xyz), bmin, bmax, capi.ptr(sd), capi.ptr(thr), capi.ptr(extra_u8), int(lo), int(hi), n,
                   capi.ptr(index), capi.ptr(count), capi.ptr(ws), ws.numel(), st)
@@ -186,9 +186,9 @@ class Gaussians():
         cov = self.covariances.to(torch.float32).contiguous()
         mag = torch.empty((max(n, 1),), dtype=torch.float64, device=dev)
         ppg = torch.zeros((max(n, 1),), dtype=torch.int32, device=dev)
-        ws = torch.empty((max(int(capi.load().g2pc_ppg_workspace_bytes(n)) // 8 + 1, 1),), dtype=torch.float64, device=dev)
+        ws = capi.workspace(capi.load().g2pc_ppg_workspace_bytes(n), dev)
         capi.call("g2pc_points_per_gaussian", capi.ptr(cov), capi.ptr(contrib), n, float(num_points), capi.ptr(mag),
-                  capi.ptr(ppg), capi.ptr(ws), ws.numel() * 8, capi.stream_ptr(dev))
+                  capi.ptr(ppg), capi.ptr(ws), ws.numel(), capi.stream_ptr(dev))
         return ppg[:n], mag[:n]
 
     def set_default_filter(self):

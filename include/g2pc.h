@@ -28,7 +28,7 @@ extern "C" {
 #define G2PC_OK 0
 #define G2PC_ERR_INVALID 1   /* bad argument */
 #define G2PC_ERR_CUDA 2      /* a CUDA runtime call / launch failed */
-#define G2PC_ERR_WORKSPACE 3 /* caller-provided scratch too small */
+#define G2PC_ERR_WORKSPACE 3 /* caller-provided workspace too small or misaligned */
 
 #define G2PC_F32 0
 #define G2PC_F64 1
@@ -135,7 +135,7 @@ int g2pc_dump_eps(const int64_t* gids, int64_t n_gids, int32_t k, int32_t attemp
  * && max_contrib[i] > vis_threshold && opacity[i] > min_opacity && bbox_min < xyz[i] < bbox_max (open box)
  * && surface_dist[i] < *surface_threshold_dev && extra_mask[i]; every criterion whose array is NULL is skipped
  * (bbox_*_host: 3 host floats or NULL).  index: ascending row numbers of the kept Gaussians (capacity n int32);
- * count: one int64 in device memory.  workspace: g2pc_cull_workspace_bytes(n). */
+ * count: one int64 in device memory.  workspace: g2pc_cull_workspace_bytes(n), 4-byte aligned. */
 int64_t g2pc_cull_workspace_bytes(int64_t n);
 int g2pc_cull_select(const float* max_contrib, float vis_threshold, const float* opacity, float min_opacity,
                      const float* xyz, const float* bbox_min3_host, const float* bbox_max3_host,
@@ -150,7 +150,8 @@ int g2pc_gather_rows(const int32_t* index, int64_t m, int32_t num_arrays, const 
 /* Magnitudes and point budget without a host round trip: magnitudes[i] (float64) = sqrt(ellipsoid area of Sigma_i,
  * p = 1.6075) * contrib[i] (gauss_handler.py:252-279, float32 chain, closed-form eigenvalues), ppg[i] (int32) =
  * round-half-even(magnitude * num_points / sum) with the first min(deficit, #zeros) zero entries raised to 1
- * (gauss_to_pc.py:73-90; the sum is reduced in a fixed order: bit-identical re-runs). */
+ * (gauss_to_pc.py:73-90; the sum is reduced in a fixed order: bit-identical re-runs).  workspace:
+ * g2pc_ppg_workspace_bytes(n), 8-byte aligned. */
 int64_t g2pc_ppg_workspace_bytes(int64_t n);
 int g2pc_points_per_gaussian(const float* cov, const float* contrib, int64_t n, double num_points, double* magnitudes,
                              int32_t* ppg, void* workspace, int64_t workspace_bytes, void* stream);
@@ -228,7 +229,8 @@ int g2pc_mesh_extract_emit(const float* chi, int32_t depth, const double* frame,
 /* Per vertex: density = (1-t) W_a + t W_b and colour = floor(((1-t) C_a + t C_b) / density + 0.5) clamped to 0..255
  * (0 where density is 0), W / C = sums of w / w * colour over the points of the 8 dual cells around the node (cells in
  * ascending index, points in ascending input index, sequential float64).  colours (n,3 int32) and vcolours (m,3 uint8)
- * may both be NULL.  cell_scratch: 4 bytes per dual cell.  workspace: g2pc_mesh_gather_workspace_bytes(n). */
+ * may both be NULL.  cell_scratch: 4 bytes per dual cell.  workspace: g2pc_mesh_gather_workspace_bytes(n), 256-byte
+ * aligned. */
 int64_t g2pc_mesh_gather_workspace_bytes(int64_t n);
 int g2pc_mesh_gather(const float* xyz, const int32_t* colours, const uint32_t* cell, int64_t n, const double* frame,
                      int32_t depth, const int64_t* vkey, const double* vt, int64_t m, void* cell_scratch,
@@ -251,7 +253,8 @@ int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, int64_t t, i
                      int64_t workspace_bytes, void* stream);
 
 /* vertices (m,3 float32) = vpos rounded; normals (m,3 float32) = normalised sum of cross(p1 - p0, p2 - p0) over the
- * incident triangles in ascending order (float64; zero stays zero).  workspace: g2pc_mesh_normals_workspace_bytes(m, t). */
+ * incident triangles in ascending order (float64; zero stays zero).  workspace: g2pc_mesh_normals_workspace_bytes(m, t),
+ * 256-byte aligned. */
 int64_t g2pc_mesh_normals_workspace_bytes(int64_t m, int64_t t);
 int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* faces, int64_t t, float* vertices, float* normals,
                       void* workspace, int64_t workspace_bytes, void* stream);

@@ -14,23 +14,9 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from g2pc import mesh  # noqa: E402
+from sanitizer_harness import poison_allocator  # noqa: E402
 
 dev = "cuda:0"
-
-
-def poison_allocator(byte):
-    """Fill and release blocks of both pools of the caching allocator (it keeps them cached), so a kernel that reads
-    memory nobody wrote sees `byte`."""
-    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(64)]
-    large = [torch.full((64 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(4)]
-    torch.cuda.synchronize()
-    del small, large
-    for nbytes in (4096, 8 << 20):
-        probe = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
-        del probe
-
-
 if os.environ.get("G2PC_TARGET_POISON") is not None:
     poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
 rng = np.random.default_rng(3)

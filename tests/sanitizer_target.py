@@ -19,25 +19,11 @@ import gauss_handler as gh  # noqa: E402
 import gauss_render as gr  # noqa: E402
 import gauss_to_pc as g2p  # noqa: E402
 from g2pc import synth  # noqa: E402
+from sanitizer_harness import poison_allocator  # noqa: E402
 
 dev = "cuda:0"
-
-
-def poison_allocator(byte):
-    """Fill and release blocks of both pools of the caching allocator (it keeps them cached), so a kernel that reads
-    memory nobody wrote sees `byte`.  Small pool: blocks of <= 1 MB carved from 2 MB segments; large pool: split blocks."""
-    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(64)]
-    large = [torch.full((256 << 20,), byte, dtype=torch.uint8, device=dev) for _ in range(4)]
-    torch.cuda.synchronize()
-    del small, large
-    for nbytes in (4096, 8 << 20):  # later blocks of both pools really start out filled
-        probe = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
-        del probe
-
-
 if os.environ.get("G2PC_TARGET_POISON") is not None:
-    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
+    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0), large_bytes=256 << 20)
 outputs = {}
 sc = synth.make_scene(1500, seed=31, sh_degree=3)
 d = {k: v.to(dev) for k, v in sc.items()}

@@ -6,9 +6,6 @@ oracle, so they must be bit-identical.  The cloud statistics are reduced in a fi
 sequentially in the oracle, so they agree to 1e-12 relative; a point whose avg lies within 1e-12 * threshold of the
 threshold may then be kept by one and not the other (counted and printed; none are expected)."""
 import os
-import shutil
-import subprocess
-import sys
 import time
 import zlib
 
@@ -17,6 +14,7 @@ import pytest
 import torch
 
 import f64ref_outliers
+from sanitizer_harness import check_target, poison_allocator
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -164,23 +162,6 @@ def test_output_rows(lib):
     assert pe.shape == (0, 3) and ce.shape == (0, 3) and ce.dtype == torch.int32 and ne is None
 
 
-def poison_allocator(byte):
-    """Fill and release blocks of both pools of PyTorch's caching allocator (it keeps them cached), so any memory a
-    kernel reads without writing it first holds `byte`.  Blocks the allocator serves from elsewhere (a free tail of a
-    segment that still holds a live tensor, or a fresh cudaMalloc) are not poisoned: this run checks that a clean on
-    reused memory repeats bit for bit; the small sanitizer target, poisoned before its first allocation, checks reads
-    of unwritten memory."""
-    torch.cuda.empty_cache()
-    small = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=DEV) for _ in range(64)]
-    large = [torch.full((1 << 30,), byte, dtype=torch.uint8, device=DEV) for _ in range(4)]
-    torch.cuda.synchronize()
-    del small, large
-    for nbytes in (4096, 8 << 20):
-        probe = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
-        assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
-        del probe
-
-
 def _clean_to_host(xyz, cols, nrm):
     from g2pc import outliers
     out = outliers.remove_statistical_outliers(xyz, cols, nrm, 20, 10.0, return_debug=True)
@@ -197,7 +178,7 @@ def test_scale_c3_cloud(lib):
     assert n > 9_000_000
     runs = [_clean_to_host(pc.points, pc.colours, pc.normals) for _ in range(2)]
     del pc
-    poison_allocator(0x5A)
+    poison_allocator(0x5A, large_bytes=1 << 30)
     runs.append(_clean_to_host(*[t.to(DEV) for t in host]))
     for r in runs[1:]:
         for a, b in zip(runs[0], r):
@@ -301,47 +282,6 @@ def test_errors(lib):
         capi.call("g2pc_knn_mean_dist", capi.ptr(p), 100, K_MAX + 1, None, None, None, 0, capi.stream_ptr(DEV))
 
 
-def _sanitizer():
-    return shutil.which("compute-sanitizer") or (
-        "/usr/local/cuda/bin/compute-sanitizer" if os.path.exists("/usr/local/cuda/bin/compute-sanitizer") else None)
-
-
-def _run_target(env_extra, out):
-    env = dict(os.environ, G2PC_TARGET_OUT=str(out), **env_extra)
-    r = subprocess.run([sys.executable, TARGET], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env,
-                       timeout=600)
-    assert r.returncode == 0 and "CLEAN_TARGET_OK" in r.stdout, r.stdout[-3000:]
-    with np.load(out) as z:
-        return {k: z[k] for k in z.files}
-
-
-def _check_from_outputs(tmp_path):
-    runs = [_run_target({"G2PC_TARGET_POISON": b, "CUDA_LAUNCH_BLOCKING": "1"}, tmp_path / f"fill_{b}.npz")
-            for b in ("0x00", "0xff", "0x5a")]
-    for other in runs[1:]:
-        assert sorted(other) == sorted(runs[0])
-        for k in runs[0]:
-            assert _same(other[k], runs[0][k]), k
-
-
 @pytest.mark.parametrize("tool", ["memcheck", "racecheck"])
 def test_clean_under_compute_sanitizer(lib, tool, tmp_path):
-    exe = _sanitizer()
-    if exe is None:
-        _check_from_outputs(tmp_path)
-        return
-    cmd = [exe, "--tool", tool, "--kernel-name", "kns=_GLOBAL__N_"] + \
-          (["--report-api-errors", "no"] if tool == "memcheck" else []) + ["--print-limit", "5", sys.executable, TARGET]
-    try:
-        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
-    except subprocess.TimeoutExpired:
-        pytest.skip("compute-sanitizer run exceeded 10 minutes on this box")
-    if "Error: Device not supported" in r.stdout:
-        _check_from_outputs(tmp_path)
-        return
-    tail = r.stdout[-3000:]
-    assert "CLEAN_TARGET_OK" in r.stdout, tail
-    if tool == "racecheck":
-        assert "RACECHECK SUMMARY: 0 hazards displayed (0 errors, 0 warnings)" in r.stdout, tail
-    else:
-        assert "ERROR SUMMARY: 0 errors" in r.stdout, tail
+    check_target(TARGET, "CLEAN_TARGET_OK", tool, tmp_path, timeout=600)

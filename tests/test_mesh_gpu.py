@@ -6,9 +6,6 @@ vertex keys, triangles, positions, densities, colours and the trim mask of the e
 chi and iso.  The float32 multigrid solve is compared with a sparse direct solve within a stated fraction of chi's
 range; the iso-value, the smoothed positions and the normals within stated tolerances."""
 import os
-import shutil
-import subprocess
-import sys
 import time
 
 import numpy as np
@@ -16,6 +13,7 @@ import pytest
 import torch
 
 import f64ref_mesh as fm
+from sanitizer_harness import check_target, poison_allocator
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -228,17 +226,6 @@ def test_end_to_end_shapes(lib):
     assert bool(((ln - 1).abs() < 1e-5).logical_or(ln == 0).all())
 
 
-def poison_allocator(byte):
-    torch.cuda.empty_cache()
-    blocks = [torch.full((1 << 20,), byte, dtype=torch.uint8, device=DEV) for _ in range(64)]
-    blocks += [torch.full((1 << 30,), byte, dtype=torch.uint8, device=DEV) for _ in range(2)]
-    torch.cuda.synchronize()
-    del blocks
-    probe = torch.empty(4096, dtype=torch.uint8, device=DEV)  # the small pool is served from the poisoned blocks
-    assert bool((probe == byte).all())
-    del probe
-
-
 def _run_to_host(p, n, c):
     from g2pc import mesh
     m, dbg = mesh.poisson_mesh(_t(p), _t(n), _t(c), depth=7, laplacian_iters=4, return_debug=True)
@@ -252,7 +239,7 @@ def test_determinism_on_poisoned_memory(lib):
     p, n = _sphere(200_000, rng, noise=1e-3)
     c = rng.uniform(0, 255, p.shape).astype(np.float32)
     runs = [_run_to_host(p, n, c) for _ in range(2)]
-    poison_allocator(0xFF)
+    poison_allocator(0xFF, large_bytes=1 << 30, large_blocks=2)
     runs.append(_run_to_host(p, n, c))
     for r in runs[1:]:
         for a, b in zip(runs[0], r):
@@ -322,47 +309,6 @@ def test_mesh_pc_command(lib, tmp_path):
     assert np.isfinite(v).all() and np.isfinite(nn).all()
 
 
-def _sanitizer():
-    return shutil.which("compute-sanitizer") or (
-        "/usr/local/cuda/bin/compute-sanitizer" if os.path.exists("/usr/local/cuda/bin/compute-sanitizer") else None)
-
-
-def _run_target(env_extra, out):
-    env = dict(os.environ, G2PC_TARGET_OUT=str(out), **env_extra)
-    r = subprocess.run([sys.executable, TARGET], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env,
-                       timeout=600)
-    assert r.returncode == 0 and "MESH_TARGET_OK" in r.stdout, r.stdout[-3000:]
-    with np.load(out) as z:
-        return {k: z[k] for k in z.files}
-
-
-def _check_from_outputs(tmp_path):
-    runs = [_run_target({"G2PC_TARGET_POISON": b, "CUDA_LAUNCH_BLOCKING": "1"}, tmp_path / f"fill_{b}.npz")
-            for b in ("0x00", "0xff", "0x5a")]
-    for other in runs[1:]:
-        assert sorted(other) == sorted(runs[0])
-        for k in runs[0]:
-            assert _same(other[k], runs[0][k]), k
-
-
 @pytest.mark.parametrize("tool", ["memcheck", "racecheck"])
 def test_mesh_under_compute_sanitizer(lib, tool, tmp_path):
-    exe = _sanitizer()
-    if exe is None:
-        _check_from_outputs(tmp_path)
-        return
-    cmd = [exe, "--tool", tool, "--kernel-name", "kns=_GLOBAL__N_"] + \
-          (["--report-api-errors", "no"] if tool == "memcheck" else []) + ["--print-limit", "5", sys.executable, TARGET]
-    try:
-        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
-    except subprocess.TimeoutExpired:
-        pytest.skip("compute-sanitizer run exceeded 10 minutes on this box")
-    if "Error: Device not supported" in r.stdout:
-        _check_from_outputs(tmp_path)
-        return
-    tail = r.stdout[-3000:]
-    assert "MESH_TARGET_OK" in r.stdout, tail
-    if tool == "racecheck":
-        assert "RACECHECK SUMMARY: 0 hazards displayed (0 errors, 0 warnings)" in r.stdout, tail
-    else:
-        assert "ERROR SUMMARY: 0 errors" in r.stdout, tail
+    check_target(TARGET, "MESH_TARGET_OK", tool, tmp_path, timeout=600)

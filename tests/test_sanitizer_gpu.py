@@ -9,69 +9,17 @@ made from its outputs, which are deterministic (integer atomics only, order-inde
              multisplit bit matrix or between the frame streams makes them disagree.
 Every output (per-Gaussian accumulators of both back-ends, cull index, point cloud) must match bit for bit."""
 import os
-import shutil
-import subprocess
-import sys
 
-import numpy as np
 import pytest
 
+from sanitizer_harness import check_target
+
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
-TARGET = os.path.join(HERE, "sanitizer_target.py")
-
-
-def _sanitizer():
-    return shutil.which("compute-sanitizer") or (
-        "/usr/local/cuda/bin/compute-sanitizer" if os.path.exists("/usr/local/cuda/bin/compute-sanitizer") else None)
-
-
-def _run_target(env_extra, out):
-    env = dict(os.environ, G2PC_TARGET_OUT=str(out), **env_extra)
-    r = subprocess.run([sys.executable, TARGET], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env,
-                       timeout=900)
-    assert r.returncode == 0 and "SANITIZER_TARGET_OK" in r.stdout, r.stdout[-3000:]
-    with np.load(out) as z:
-        return {k: z[k] for k in z.files}
-
-
-def _check_from_outputs(tool, tmp_path):
-    if tool == "memcheck":
-        runs = [_run_target({"G2PC_TARGET_POISON": b, "CUDA_LAUNCH_BLOCKING": "1"}, tmp_path / f"fill_{b}.npz")
-                for b in ("0x00", "0xff", "0x5a")]
-    else:
-        runs = [_run_target({"G2PC_TARGET_POISON": "0x00"}, tmp_path / f"repeat_{i}.npz") for i in range(3)]
-    first = runs[0]
-    assert len(first) >= 10 and first["points"].shape[0] > 0
-    for i, other in enumerate(runs[1:], 1):
-        assert sorted(other) == sorted(first)
-        for k in first:
-            assert other[k].dtype == first[k].dtype and other[k].shape == first[k].shape, (tool, i, k)
-            assert other[k].tobytes() == first[k].tobytes(), f"{tool}: run {i} differs from run 0 in {k}"
+TARGET = os.path.join(os.path.dirname(os.path.abspath(__file__)), "sanitizer_target.py")
 
 
 @pytest.mark.parametrize("tool", ["memcheck", "racecheck"])
 def test_hot_path_is_clean_under_compute_sanitizer(lib, tool, tmp_path):
-    exe = _sanitizer()
-    if exe is None:
-        _check_from_outputs(tool, tmp_path)
-        return
-    # only the library's own kernels (all live in anonymous namespaces of libg2pc.so) are instrumented
-    # --report-api-errors no: the CUDA runtime's lazy module loading probes kernels with cuKernelGetFunction and handles
-    # the INVALID_HANDLE return itself; memcheck would otherwise count that host-API return code as an error
-    cmd = [exe, "--tool", tool, "--kernel-name", "kns=_GLOBAL__N_"] + \
-          (["--report-api-errors", "no"] if tool == "memcheck" else []) + ["--print-limit", "5", sys.executable,
-           TARGET]
-    try:
-        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
-    except subprocess.TimeoutExpired:
-        pytest.skip("compute-sanitizer run exceeded 15 minutes on this box")
-    tail = r.stdout[-3000:]
-    if "Error: Device not supported" in r.stdout:
-        _check_from_outputs(tool, tmp_path)
-        return
-    assert "SANITIZER_TARGET_OK" in r.stdout, tail
-    if tool == "racecheck":
-        assert "RACECHECK SUMMARY: 0 hazards displayed (0 errors, 0 warnings)" in r.stdout, tail
-    else:
-        assert "ERROR SUMMARY: 0 errors" in r.stdout, tail
+    first = check_target(TARGET, "SANITIZER_TARGET_OK", tool, tmp_path, timeout=900, repeat_racecheck=True)
+    if first is not None:
+        assert len(first) >= 10 and first["points"].shape[0] > 0
