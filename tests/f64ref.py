@@ -155,17 +155,23 @@ def unpack_rect(bits):
     return b & 0xFF, (b >> 8) & 0xFF, (b >> 16) & 0xFF, (b >> 24) & 0xFF
 
 
-def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True):
+def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True, mask=None):
     """renderCUDA (forward.cu:303-497) in f64, stage-wise: fed the kernel's own projection records `rec` ((n,12): {px,py,
     K kx, 2K ky} {K kz, log2 o, r, g} {b, depth, radius, tile rect}) and its `ok` mask, with the kernel's list order
     (stable by the depth's float bits).  Per tile in rounds of 256 list entries: alpha = min(0.99, o exp(power)),
     skip power > 0 or alpha < 1/255, stop before T (1 - alpha) < 1e-4, deterministic surface distance after each round.
 
+    `mask` ((H*W) or (H,W), 0 = ignore): a masked pixel is never live, takes no part in the surface distances and is not
+    written (image, depth and inverse depth stay 0).  A tile with no live pixel at the start of a round — round 0
+    included — leaves before that round.
+
     A skip / stop decision whose f64 operand lies within a relative band of its threshold may go either way in f32:
-    the pixel is marked `tainted` from that entry on.  Returns image (3,H,W), depth, contrib (n) max over untainted pairs,
-    pixel (n, lowest id among exact equals), second (n, the runner-up at another pixel), any_taint (n: a pair of that Gaussian was tainted or followed a taint),
-    surface (n), surf_taint (n), and the decision counts."""
+    the pixel is marked `tainted` from that entry on.  Returns image (3,H,W), depth, invdepth (sum of c / depth),
+    contrib (n) max over untainted pairs, pixel (n, lowest id among exact equals), second (n, the runner-up at another
+    pixel), any_taint (n: a pair of that Gaussian was tainted or followed a taint), surface (n), surf_taint (n), and the
+    decision counts."""
     n = rec.shape[0]
+    mflat = None if mask is None else np.asarray(mask).reshape(-1) != 0
     px, py = rec[:, 0].astype(np.float64), rec[:, 1].astype(np.float64)
     kx, ky, kz = rec[:, 2] / K_EXP2, rec[:, 3] / (2 * K_EXP2), rec[:, 4] / K_EXP2
     op = np.exp2(rec[:, 5].astype(np.float64))
@@ -177,6 +183,7 @@ def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True):
     gx, gy = (W + 15) // 16, (H + 15) // 16
     img = np.zeros((3, H, W))
     dimg = np.zeros((H, W))
+    iimg = np.zeros((H, W))
     contrib = np.zeros(n)
     pixel = np.full(n, -1, dtype=np.int64)
     second = np.zeros(n)  # runner-up: the largest untainted contribution at any other pixel
@@ -192,13 +199,27 @@ def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True):
             ys, xs = ys.reshape(-1), xs.reshape(-1)
             inside = (xs < W) & (ys < H)
             pid = ys * W + xs
+            live0 = inside.copy()
+            if mflat is not None:
+                live0[inside] = mflat[pid[inside]]
+            # surface distances: unmasked pixels hold their expected depth, threads outside the image hold 0
+            part = live0 | ~inside
             T = np.ones(256)
-            done = ~inside
+            done = ~live0
             tainted = np.zeros(256, dtype=bool)
+            band_done = np.zeros(256, dtype=bool)  # stopped by a decision in the band: may still be live in f32
+            slack = np.zeros(256)  # bound on how far a tainted pixel's expected depth may lie from the f32 one
+            dmax = float(depth[sel].max()) if sel.shape[0] else 0.0
             C = np.zeros((256, 3))
             E = np.zeros(256)
+            IE = np.zeros(256)
             rounds = 0
             for r0 in range(0, sel.shape[0], 256):
+                # whether the tile leaves here is undetermined when a tainted pixel could be live in f32 and no
+                # untainted one is
+                if tainted.any() and not (~done & ~tainted).any() and (band_done.any() or not done.all()):
+                    staint[sel[r0:]] = True
+                    taint[sel[r0:]] = True
                 if bool(done.all()):
                     break  # the tile leaves at the start of a round
                 rounds += 1
@@ -216,15 +237,20 @@ def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True):
                     counts["skip_band"] += int(near_skip.sum())
                     counts["stop_band"] += int(near_stop.sum())
                     tainted |= near_skip | near_stop
+                    # a flipped skip moves E by at most alpha (its own share and the attenuation of the rest) times the
+                    # deepest entry, twice over; a flipped stop by at most T times it, twice over
+                    slack += 2.0 * dmax * (np.where(near_skip, alpha, 0.0) + np.where(near_stop, T, 0.0))
                     stop = keep & (testT < 1e-4)
+                    band_done |= stop & near_stop
                     done |= stop
                     take = keep & ~stop
                     c = np.where(take, alpha * T, 0.0)
                     C += c[:, None] * col[g][None, :]
                     E += depth[g] * c
+                    IE += c / depth[g]
                     T = np.where(take, testT, T)
                     cu = np.where(tainted, 0.0, c)
-                    if tainted[act].any():
+                    if tainted[act | band_done].any():
                         taint[g] = True
                     at_max = np.flatnonzero(cu == cu.max())
                     k1 = int(at_max[np.argmin(pid[at_max])])  # lowest pixel id among the maxima
@@ -236,21 +262,115 @@ def tiles_blend(rec, ok, W, H, bg, band_alpha=2e-5, band_T=1e-4, surface=True):
                     else:
                         loser = v1
                     second[g] = max(second[g], v2, loser)
-                if surface:
+                if surface and part.any():
                     Ep = np.where(inside, E, 0.0)
-                    d = np.abs(depth[rnd][:, None] - Ep[None, :]).min(axis=1)
+                    dist = np.abs(depth[rnd][:, None] - Ep[None, :])
+                    d = dist[:, part].min(axis=1)
                     surf[rnd] = np.minimum(surf[rnd], d)
-                    if tainted.any():
-                        staint[rnd] = True
+                    # tainted: a tainted pixel, moved by its slack (plus a stop one entry early or late), could come
+                    # at least as close as the others
+                    tp = part & tainted
+                    if tp.any():
+                        d_clean = dist[:, part & ~tainted].min(axis=1, initial=np.inf)
+                        d_low = (dist[:, tp] - (slack[tp] + 2e-4 * dmax)[None, :]).min(axis=1)
+                        staint[rnd[d_low <= d_clean]] = True
             counts["rounds_max"] = max(counts["rounds_max"], rounds)
-            w = inside
+            w = live0
             img[:, ys[w], xs[w]] = (C[w] + T[w][:, None] * np.asarray(bg, dtype=np.float64)[None, :]).T
             dimg[ys[w], xs[w]] = E[w]
+            iimg[ys[w], xs[w]] = IE[w]
             if tainted.any():
                 img[:, ys[w & tainted], xs[w & tainted]] = np.nan
                 dimg[ys[w & tainted], xs[w & tainted]] = np.nan
-    return dict(image=img, depth=dimg, contrib=contrib, pixel=pixel, second=second, taint=taint, surface=surf, surf_taint=staint,
-                **counts)
+                iimg[ys[w & tainted], xs[w & tainted]] = np.nan
+    return dict(image=img, depth=dimg, invdepth=iimg, contrib=contrib, pixel=pixel, second=second, taint=taint,
+                surface=surf, surf_taint=staint, **counts)
+
+
+def _sh_basis(deg):
+    """Real spherical harmonics Y_lm (l <= deg, m = -l..l at index l^2 + l + m, Condon-Shortley phase) as polynomials
+    in the unit direction: a list of {(a, b, c): coefficient of x^a y^b z^c}.  From the definitions:
+    Y_l0 = K_l0 P_l(z), Y_lm = sqrt(2) K_lm P_l^|m|(z) {cos m phi (m > 0), sin |m| phi (m < 0)},
+    K_lm = sqrt((2l + 1) / (4 pi) (l - |m|)! / (l + |m|)!), P_l^m(z) = (-1)^m (1 - z^2)^(m/2) d^m P_l / dz^m, and
+    (1 - z^2)^(m/2) (cos m phi + i sin m phi) = (x + i y)^m on the unit sphere."""
+    from numpy.polynomial import legendre as L
+    out = []
+    for l in range(deg + 1):
+        for m in range(-l, l + 1):
+            a = abs(m)
+            K = math.sqrt((2 * l + 1) / (4.0 * math.pi) * math.factorial(l - a) / math.factorial(l + a))
+            dz = L.leg2poly(L.legder(np.eye(l + 1)[l], a))  # d^a P_l / dz^a in the power basis
+            # (x + i y)^a = sum_k C(a, k) x^(a-k) (i y)^k: real part (cos) even k, imaginary part (sin) odd k
+            xy = {}
+            for k in range(a + 1):
+                if (m >= 0 and k % 2 == 0) or (m < 0 and k % 2 == 1):
+                    xy[(a - k, k)] = math.comb(a, k) * (-1.0) ** (k // 2)
+            scale = K * (1.0 if m == 0 else math.sqrt(2.0) * (-1.0) ** a)
+            poly = {}
+            for (px_, py_), cxy in xy.items():
+                for pz, cz in enumerate(dz):
+                    if cz != 0.0:
+                        key = (px_, py_, pz)
+                        poly[key] = poly.get(key, 0.0) + scale * cxy * cz
+            out.append(poly)
+    return out
+
+
+def sh_colour(deg, shs, dirs, layout=0):
+    """Colour of real SH degree `deg` in f64: max(sum_k Y_k(d) s_k + 0.5, 0) per channel.  shs: (n,3,stride) for layout 0
+    (channel-major), (n,stride,3) for layout 1; dirs (n,3) unit directions.  Returns (rgb (n,3), bound (n,3)): bound is
+    0.5 + sum over every monomial term of |coefficient x^a y^b z^c s_k|, the scale of the float32 rounding."""
+    s = np.asarray(shs, dtype=np.float64)
+    if layout == 1:
+        s = s.transpose(0, 2, 1)
+    d = np.asarray(dirs, dtype=np.float64)
+    x, y, z = d[:, 0], d[:, 1], d[:, 2]
+    r = np.zeros((d.shape[0], 3))
+    bound = np.full((d.shape[0], 3), 0.5)
+    for k, poly in enumerate(_sh_basis(deg)):
+        for (a, b, c), coef in poly.items():
+            t = (coef * x ** a * y ** b * z ** c)[:, None] * s[:, :, k]
+            r += t
+            bound += np.abs(t)
+    return np.maximum(r + 0.5, 0.0), bound
+
+
+def accumulate(per_camera, near=1e-6):
+    """Fold per-camera f64 results in camera order, as the per-Gaussian accumulators do: maximum by strict > (the first
+    camera keeps an exact tie), colour = the winning camera's f64 image at its arg-max pixel, total = f64 sum of the
+    per-camera maxima, surface distance = minimum.  per_camera: dicts of tiles_blend (image, contrib, pixel, second,
+    taint, surface, surf_taint).  A Gaussian tainted in any camera stays tainted.  `near_tie` marks a Gaussian whose
+    maxima in two cameras lie within `near` of each other without being equal (which camera wins is undetermined in
+    f32); `pixel_tie` one whose winning camera's arg-max pixel is a near-tie within that camera."""
+    n = per_camera[0]["contrib"].shape[0]
+    mx = np.zeros(n)
+    winner = np.full(n, -1, dtype=np.int64)
+    colour = np.zeros((n, 3))
+    total = np.zeros(n)
+    surf = np.full(n, np.inf)
+    taint = np.zeros(n, dtype=bool)
+    staint = np.zeros(n, dtype=bool)
+    near_tie = np.zeros(n, dtype=bool)
+    pixel_tie = np.zeros(n, dtype=bool)
+    seen = []  # maxima of the earlier cameras
+    for ci, f in enumerate(per_camera):
+        v = f["contrib"]
+        for prev in seen:
+            near_tie |= (v > 0) & (prev > 0) & (v != prev) & (np.abs(v - prev) <= near)
+        seen.append(v)
+        upd = v > mx
+        flat = f["image"].reshape(3, -1)
+        pix = np.where(f["pixel"] >= 0, f["pixel"], 0)
+        mx = np.where(upd, v, mx)
+        winner = np.where(upd, ci, winner)
+        colour = np.where(upd[:, None], flat[:, pix].T, colour)
+        pixel_tie = np.where(upd, (v - f["second"]) < near, pixel_tie)
+        total += v
+        surf = np.minimum(surf, f["surface"])
+        taint |= f["taint"]
+        staint |= f["surf_taint"]
+    return dict(max=mx, winner=winner, colour=colour, total=total, surface=surf, taint=taint, surf_taint=staint,
+                near_tie=near_tie, pixel_tie=pixel_tie)
 
 
 def leaf_blend(r0, c0, w, h, ids, proj, bg=1.0, transmittance=False):

@@ -15,6 +15,7 @@ import torch
 
 import edge_scenes as es
 import f64ref as fr
+import tiles_harness as th
 from util import scene_to
 
 pytestmark = pytest.mark.gpu
@@ -279,27 +280,12 @@ def test_opacity_clamp_and_alpha_skip(lib):
 
 # ---- blends, stage-wise --------------------------------------------------------------------------------------------
 def _cuda_setup(sc, cams, intr, surf=True):
-    from g2pc.rasterizer import GaussianRasterizer
-    from oracle import gaussians as og
-    cov = og.build_covariance(sc["scales"], sc["rots"])
-    d = scene_to(sc, DEV)
-    R = GaussianRasterizer(d["xyz"], None, d["opacities"], colors_precomp=d["colours"].float(),
-                           cov3D_precomp=cov.to(DEV), calculate_surface_distance=surf)
-    return R, d, cov
+    return th.cuda_setup(sc, surf)
 
 
 def _tiles_camera(R, rs):
-    n = R._n
-    contrib = torch.zeros((n,), dtype=torch.float32, device=DEV)
-    pixels = torch.zeros((n,), dtype=torch.int32, device=DEV)
-    surf = torch.full((n,), torch.finfo(torch.float).max, dtype=torch.float32, device=DEV)
-    R._per_camera = (contrib, pixels, surf)
-    img, _, _, dep = R(rs)
-    R._per_camera = None
-    sl = R._slots[R._last_slot]
-    ok = sl["depth_key"].cpu().numpy().view(np.uint32) != 0xFFFFFFFF
-    return img.cpu().numpy(), dep.cpu().numpy()[0], sl["proj"].cpu().numpy(), ok, contrib.cpu().numpy(), \
-        pixels.cpu().numpy(), surf.cpu().numpy()
+    o = th.tiles_camera(R, rs)
+    return tuple(o[k] for k in ("image", "depth", "rec", "ok", "contrib", "pixel", "surface"))
 
 
 @pytest.mark.parametrize("family", ["huge", "ties", "inside"])
