@@ -18,6 +18,8 @@
 // not nearer than the current k-th distance is skipped without touching memory; otherwise its range is found by
 // galloping search from the previous position, and it is scanned if it holds <= LEAF_T points (or is a 42-bit cell),
 // else entered.  The k smallest d2 live in registers; indices are not needed (only the multiset of distances matters).
+// g2pc_knn_ids (the normal orientation, N7) runs the same index and walk with a register list of (d2, row id) pairs
+// instead, ordered lexicographically over the other points, and writes the ids.
 // Box distances are lowered by a margin of E * 2^-48, which covers the rounding of the quantisation and of the distance
 // arithmetic, so a cell is skipped only when no point in it can enter the list: the result is exact.
 #include <cub/cub.cuh>
@@ -112,7 +114,7 @@ __global__ void __launch_bounds__(BB) gather_u64_kernel(const uint64_t* __restri
     if (j < n) dst[j] = src[idx[j]];
 }
 
-// sorted index -> (lo, hi) key pair and the point as float4
+// sorted index -> (lo, hi) key pair and the point as float4, its row id in the bits of w
 __global__ void __launch_bounds__(BB) gather_sorted_kernel(const uint64_t* __restrict__ hi_sorted,
                                                            const uint64_t* __restrict__ lo, const uint32_t* __restrict__ idx,
                                                            const float* __restrict__ xyz, int64_t n,
@@ -121,7 +123,7 @@ __global__ void __launch_bounds__(BB) gather_sorted_kernel(const uint64_t* __res
     if (j >= n) return;
     const uint32_t i = idx[j];
     keys[j] = make_ulonglong2(lo[i], hi_sorted[j]);
-    pts[j] = make_float4(xyz[3 * (int64_t)i], xyz[3 * (int64_t)i + 1], xyz[3 * (int64_t)i + 2], 0.f);
+    pts[j] = make_float4(xyz[3 * (int64_t)i], xyz[3 * (int64_t)i + 1], xyz[3 * (int64_t)i + 2], __uint_as_float(i));
 }
 
 __device__ __forceinline__ u128 key_at(const ulonglong2* __restrict__ keys, int j) {
@@ -147,22 +149,74 @@ __device__ __forceinline__ int lower_bound_from(const ulonglong2* __restrict__ k
     return hi;
 }
 
-// best[] holds the k smallest d2 ascending in its LAST k slots (the others are -inf), so the k-th distance is always
-// best[K_MAX - 1] and every index below is a compile-time constant (the list stays in registers)
-__device__ __forceinline__ void consider(double (&best)[K_MAX], const float4 q, const float4 p) {
+// float64 d2 of two float32 points, in the order of the restatements: (dx*dx + dy*dy) + dz*dz
+__device__ __forceinline__ double dist2(const float4 q, const float4 p) {
     const double dx = __dsub_rn((double)q.x, (double)p.x), dy = __dsub_rn((double)q.y, (double)p.y),
                  dz = __dsub_rn((double)q.z, (double)p.z);
-    const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-    if (d2 < best[K_MAX - 1]) {  // insert, dropping the largest: new[j] = max(old[j-1], min(old[j], d2))
-#pragma unroll
-        for (int j = K_MAX - 1; j > 0; --j) best[j] = fmax(best[j - 1], fmin(best[j], d2));
-        best[0] = fmin(best[0], d2);
-    }
+    return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
 }
 
-__device__ __forceinline__ void scan_range(double (&best)[K_MAX], const float4 q, const float4* __restrict__ pts, int j0,
-                                           int j1) {
-    for (int j = j0; j < j1; ++j) consider(best, q, pts[j]);
+// The register list of a query: the k smallest d2 (N5, the query itself included).  d[] holds them ascending in its
+// LAST k slots (the others are -inf), so the k-th distance is always d[K_MAX - 1] and every index below is a
+// compile-time constant (the list stays in registers).
+struct DistList {
+    double d[K_MAX];
+    __device__ __forceinline__ void init(int kp) {
+#pragma unroll
+        for (int j = 0; j < K_MAX; ++j) d[j] = j >= K_MAX - kp ? INFINITY : -INFINITY;
+    }
+    __device__ __forceinline__ double kth() const { return d[K_MAX - 1]; }
+    __device__ __forceinline__ void consider(const float4 q, const float4 p) {
+        const double d2 = dist2(q, p);
+        if (d2 < d[K_MAX - 1]) {  // insert, dropping the largest: new[j] = max(old[j-1], min(old[j], d2))
+#pragma unroll
+            for (int j = K_MAX - 1; j > 0; --j) d[j] = fmax(d[j - 1], fmin(d[j], d2));
+            d[0] = fmin(d[0], d2);
+        }
+    }
+};
+
+// The k smallest (d2, id) pairs in lexicographic order over the other points (g2pc_knn_ids): ties of d2 go to the
+// smaller row id, so the list is unique.  The row id of every sorted point travels in the bits of its float4's w.
+struct IdList {
+    double d[K_MAX];
+    uint32_t id[K_MAX];
+    uint32_t self;
+    __device__ __forceinline__ void init(int kp) {
+#pragma unroll
+        for (int j = 0; j < K_MAX; ++j) { d[j] = j >= K_MAX - kp ? INFINITY : -INFINITY; id[j] = 0xFFFFFFFFu; }
+    }
+    __device__ __forceinline__ double kth() const { return d[K_MAX - 1]; }
+    static __device__ __forceinline__ bool less(double ad, uint32_t ai, double bd, uint32_t bi) {
+        return ad < bd || (ad == bd && ai < bi);
+    }
+    __device__ __forceinline__ bool contains(uint32_t j) const {
+        bool c = false;
+#pragma unroll
+        for (int s = 0; s < K_MAX; ++s) c |= id[s] == j && d[s] != -INFINITY;
+        return c;
+    }
+    __device__ __forceinline__ void consider(const float4 q, const float4 p) {
+        const uint32_t j = __float_as_uint(p.w);
+        if (j == self) return;
+        const double d2 = dist2(q, p);
+        if (!less(d2, j, d[K_MAX - 1], id[K_MAX - 1])) return;
+#pragma unroll
+        for (int s = K_MAX - 1; s > 0; --s) {
+            const bool lo = less(d2, j, d[s], id[s]);  // min(old[s], x)
+            const double md = lo ? d2 : d[s];
+            const uint32_t mi = lo ? j : id[s];
+            const bool up = less(d[s - 1], id[s - 1], md, mi);  // max(old[s-1], that)
+            d[s] = up ? md : d[s - 1];
+            id[s] = up ? mi : id[s - 1];
+        }
+        if (less(d2, j, d[0], id[0])) { d[0] = d2; id[0] = j; }
+    }
+};
+
+template <class List>
+__device__ __forceinline__ void scan_range(List& best, const float4 q, const float4* __restrict__ pts, int j0, int j1) {
+    for (int j = j0; j < j1; ++j) best.consider(q, pts[j]);
 }
 
 // distance of the shifted query s from the cell [c*w, (c+1)*w] along one axis, lowered by the margin
@@ -172,19 +226,10 @@ __device__ __forceinline__ double axis_gap(double s, uint64_t c, double w, doubl
     return fmax(g - margin, 0.0);
 }
 
-__global__ void __launch_bounds__(QB) knn_kernel(const ulonglong2* __restrict__ keys, const float4* __restrict__ pts,
-                                                 const uint32_t* __restrict__ order, const Frame* __restrict__ frp, int n,
-                                                 int k, double* __restrict__ avg) {
-    const int t = blockIdx.x * QB + threadIdx.x;
-    if (t >= n) return;
-    const float4 q = pts[t];
-    if (!finite3(q.x, q.y, q.z)) { avg[order[t]] = __longlong_as_double(0x7ff8000000000000ll); return; }
-    const Frame fr = *frp;
-    const int kp = k < n ? k : n;
-    double best[K_MAX];
-#pragma unroll
-    for (int j = 0; j < K_MAX; ++j) best[j] = j >= K_MAX - kp ? INFINITY : -INFINITY;
-
+// The search of sorted point t: its window, then the stackless octree walk.  One copy for both lists.
+template <class List>
+__device__ __forceinline__ void knn_query(List& best, const ulonglong2* __restrict__ keys, const float4* __restrict__ pts,
+                                          const Frame& fr, int n, int t, const float4 q) {
     const int W = n < WIN ? n : WIN;
     int w0 = t - WIN / 2;
     w0 = w0 < 0 ? 0 : (w0 > n - W ? n - W : w0);
@@ -199,7 +244,7 @@ __global__ void __launch_bounds__(QB) knn_kernel(const ulonglong2* __restrict__ 
     for (;;) {
         const double gx = axis_gap(sx, cx, w, fr.margin), gy = axis_gap(sy, cy, w, fr.margin),
                      gz = axis_gap(sz, cz, w, fr.margin);
-        if (gx * gx + gy * gy + gz * gz < best[K_MAX - 1]) {
+        if (gx * gx + gy * gy + gz * gz < best.kth()) {
             const int sh = QBITS - L;
             const u128 start = key126(cx << sh, cy << sh, cz << sh);
             const int a0 = lower_bound_from(keys, a, n, start);
@@ -218,12 +263,71 @@ __global__ void __launch_bounds__(QB) knn_kernel(const ulonglong2* __restrict__ 
         const uint32_t d = (uint32_t)((cx & 1) << 2 | (cy & 1) << 1 | (cz & 1)) + 1;
         cx = (cx & ~1ull) | (d >> 2); cy = (cy & ~1ull) | ((d >> 1) & 1); cz = (cz & ~1ull) | (d & 1);
     }
+}
 
+__global__ void __launch_bounds__(QB) knn_kernel(const ulonglong2* __restrict__ keys, const float4* __restrict__ pts,
+                                                 const uint32_t* __restrict__ order, const Frame* __restrict__ frp, int n,
+                                                 int k, double* __restrict__ avg) {
+    const int t = blockIdx.x * QB + threadIdx.x;
+    if (t >= n) return;
+    const float4 q = pts[t];
+    if (!finite3(q.x, q.y, q.z)) { avg[order[t]] = __longlong_as_double(0x7ff8000000000000ll); return; }
+    const Frame fr = *frp;
+    const int kp = k < n ? k : n;
+    DistList best;
+    best.init(kp);
+    knn_query(best, keys, pts, fr, n, t, q);
     double s = 0.0;
 #pragma unroll
     for (int j = 0; j < K_MAX; ++j)
-        if (j >= K_MAX - kp) s = __dadd_rn(s, sqrt(best[j]));
+        if (j >= K_MAX - kp) s = __dadd_rn(s, sqrt(best.d[j]));
     avg[order[t]] = s / (double)kp;
+}
+
+// ids[row * k + r], d2[row * k + r] for r < k' = min(k, n - 1): the neighbours of `row` by ascending (d2, id); the
+// slots r >= k' hold id -1 and d2 +inf.  A non-finite row gets id -1 and d2 NaN in every slot.
+__global__ void __launch_bounds__(QB) knn_ids_kernel(const ulonglong2* __restrict__ keys, const float4* __restrict__ pts,
+                                                     const Frame* __restrict__ frp, int n, int k,
+                                                     int32_t* __restrict__ ids, double* __restrict__ d2) {
+    const int t = blockIdx.x * QB + threadIdx.x;
+    if (t >= n) return;
+    const float4 q = pts[t];
+    const uint32_t row = __float_as_uint(q.w);
+    const int kp = k < n - 1 ? k : n - 1;
+    if (!finite3(q.x, q.y, q.z)) {
+        for (int r = 0; r < k; ++r) {
+            ids[(int64_t)row * k + r] = -1;
+            if (d2) d2[(int64_t)row * k + r] = __longlong_as_double(0x7ff8000000000000ll);
+        }
+        return;
+    }
+    const Frame fr = *frp;
+    IdList best;
+    best.self = row;
+    best.init(kp);
+    knn_query(best, keys, pts, fr, n, t, q);
+    // k' exact copies of the query fill the list at distance 0, and the walk then prunes every cell; copies with
+    // smaller ids may still be missing.  Copies share the query's key, and equal keys keep their row order through the
+    // stable sorts, so the key run's first copies (up to k' of them besides the query) are the smallest ids.
+    if (kp > 0 && best.kth() == 0.0) {
+        const u128 K = key_at(keys, t);
+        int found = 0;
+        for (int j = lower_bound_from(keys, 0, n, K); j < n && found < kp && key_at(keys, j) == K; ++j) {
+            const float4 p = pts[j];
+            const uint32_t jid = __float_as_uint(p.w);
+            if (jid == row) continue;
+            if (dist2(q, p) == 0.0) ++found;
+            if (!best.contains(jid)) best.consider(q, p);
+        }
+    }
+    int32_t* out = ids + (int64_t)row * k;
+    double* od = d2 ? d2 + (int64_t)row * k : nullptr;
+#pragma unroll
+    for (int j = 0; j < K_MAX; ++j) {
+        const int r = j - (K_MAX - kp);
+        if (r >= 0) { out[r] = (int32_t)best.id[j]; if (od) od[r] = best.d[j]; }
+    }
+    for (int r = kp; r < k; ++r) { out[r] = -1; if (od) od[r] = INFINITY; }
 }
 
 // ---- statistics and keep mask ------------------------------------------------------------------------------------
@@ -307,6 +411,31 @@ KnnWs knn_ws(void* base, int64_t n) {
     return l;
 }
 
+// The index of both k-NN entry points: frame, keys, the two stable sorts, the sorted key pairs and points.  Returns the
+// key pairs; the sorted points are in l.pts and their rows in l.idx_a.
+int build_index(const float* xyz, int64_t n, int32_t* status, const KnnWs& l, cudaStream_t st, ulonglong2** keys_out) {
+    uint64_t* hi_sorted = l.hi;                          // sort 2 output keys (hi is dead by then)
+    ulonglong2* keys = (ulonglong2*)l.lo_by_lo;          // both sort 1 buffers are dead by then
+    const int nbox = bbox_blocks(n);
+    const unsigned g = (unsigned)((n + BB - 1) / BB);
+    bbox_kernel<<<nbox, BBOX_THREADS, 0, st>>>(xyz, n, l.part);
+    G2PC_CHECK_LAUNCH();
+    frame_kernel<<<1, 1, 0, st>>>(l.part, nbox, l.fr);
+    G2PC_CHECK_LAUNCH();
+    key_kernel<<<g, BB, 0, st>>>(xyz, n, l.fr, l.hi, l.lo, l.idx_a, status);
+    G2PC_CHECK_LAUNCH();
+    size_t b = l.tmp_bytes;
+    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, l.lo, l.lo_by_lo, l.idx_a, l.idx_b, n, 0, 63, st));
+    gather_u64_kernel<<<g, BB, 0, st>>>(l.hi, l.idx_b, n, l.hi_by_lo);
+    G2PC_CHECK_LAUNCH();
+    b = l.tmp_bytes;  // stable: points with equal hi keep their lo order
+    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, l.hi_by_lo, hi_sorted, l.idx_b, l.idx_a, n, 0, 63, st));
+    gather_sorted_kernel<<<g, BB, 0, st>>>(hi_sorted, l.lo, l.idx_a, xyz, n, keys, l.pts);
+    G2PC_CHECK_LAUNCH();
+    *keys_out = keys;
+    return G2PC_OK;
+}
+
 }  // namespace
 
 extern "C" int64_t g2pc_knn_workspace_bytes(int64_t n) { return n <= 0 ? 0 : (int64_t)knn_ws(nullptr, n).bytes; }
@@ -323,26 +452,30 @@ extern "C" int g2pc_knn_mean_dist(const float* xyz, int64_t n, int32_t k, double
     G2PC_CHECK_ARG(xyz && avg && workspace, "null pointer");
     const KnnWs l = knn_ws(workspace, n);
     G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
-    uint64_t* hi_sorted = l.hi;                          // sort 2 output keys (hi is dead by then)
-    ulonglong2* keys = (ulonglong2*)l.lo_by_lo;          // both sort 1 buffers are dead by then
-    const int nbox = bbox_blocks(n);
-    const unsigned g = (unsigned)((n + BB - 1) / BB);
-
-    bbox_kernel<<<nbox, BBOX_THREADS, 0, st>>>(xyz, n, l.part);
-    G2PC_CHECK_LAUNCH();
-    frame_kernel<<<1, 1, 0, st>>>(l.part, nbox, l.fr);
-    G2PC_CHECK_LAUNCH();
-    key_kernel<<<g, BB, 0, st>>>(xyz, n, l.fr, l.hi, l.lo, l.idx_a, status);
-    G2PC_CHECK_LAUNCH();
-    size_t b = l.tmp_bytes;
-    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, l.lo, l.lo_by_lo, l.idx_a, l.idx_b, n, 0, 63, st));
-    gather_u64_kernel<<<g, BB, 0, st>>>(l.hi, l.idx_b, n, l.hi_by_lo);
-    G2PC_CHECK_LAUNCH();
-    b = l.tmp_bytes;  // stable: points with equal hi keep their lo order
-    G2PC_CUDA(cub::DeviceRadixSort::SortPairs(l.tmp, b, l.hi_by_lo, hi_sorted, l.idx_b, l.idx_a, n, 0, 63, st));
-    gather_sorted_kernel<<<g, BB, 0, st>>>(hi_sorted, l.lo, l.idx_a, xyz, n, keys, l.pts);
-    G2PC_CHECK_LAUNCH();
+    ulonglong2* keys = nullptr;
+    const int rc = build_index(xyz, n, status, l, st, &keys);
+    if (rc != G2PC_OK) return rc;
     knn_kernel<<<(unsigned)((n + QB - 1) / QB), QB, 0, st>>>(keys, l.pts, l.idx_a, l.fr, (int)n, k, avg);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
+extern "C" int g2pc_knn_ids(const float* xyz, int64_t n, int32_t k, int32_t* ids, double* d2, int32_t* status,
+                            void* workspace, int64_t workspace_bytes, void* stream) {
+    G2PC_CHECK_ARG(n >= 0, "n < 0");
+    G2PC_CHECK_ARG(n < 0x7FFFFFFFll, "n must fit int32 indices");
+    G2PC_CHECK_ARG(k >= 1 && k <= G2PC_ORIENT_K_MAX, "k must be in 1..G2PC_ORIENT_K_MAX");
+    G2PC_CHECK_ARG(status, "null status");
+    cudaStream_t st = (cudaStream_t)stream;
+    G2PC_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+    if (n == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(xyz && ids && workspace, "null pointer");
+    const KnnWs l = knn_ws(workspace, n);
+    G2PC_CHECK_WORKSPACE(workspace, workspace_bytes, l.bytes, 256);
+    ulonglong2* keys = nullptr;
+    const int rc = build_index(xyz, n, status, l, st, &keys);
+    if (rc != G2PC_OK) return rc;
+    knn_ids_kernel<<<(unsigned)((n + QB - 1) / QB), QB, 0, st>>>(keys, l.pts, l.fr, (int)n, k, ids, d2);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }

@@ -41,6 +41,7 @@ SIGNATURES = {
     "g2pc_ppg_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_knn_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_knn_mean_dist": ([_c_void_p, _i64, _i32, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_knn_ids": ([_c_void_p, _i64, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_sor_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_sor_mask": ([_c_void_p, _i64, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_mesh_splat_workspace_bytes": ([_i64], ctypes.c_int64),
@@ -67,6 +68,18 @@ SIGNATURES = {
     "g2pc_mesh_normals_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
     "g2pc_mesh_normals": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
                           ctypes.c_int),
+    "g2pc_orient_prepare_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_orient_prepare": ([_c_void_p, _c_void_p, ctypes.c_int, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                             _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_orient_edges_workspace_bytes": ([_i64, _i32], ctypes.c_int64),
+    "g2pc_orient_edges": ([_c_void_p, _i64, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                           _i64, _c_void_p], ctypes.c_int),
+    "g2pc_orient_round_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_orient_round": ([_c_void_p, _c_void_p, _c_void_p, _i64, _i64, _i32, _i64, _c_void_p, _c_void_p, _c_void_p,
+                           _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_orient_finish_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_orient_finish": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, ctypes.c_int, _i64, _c_void_p, _c_void_p,
+                            _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_points_per_gaussian": ([_c_void_p, _c_void_p, _i64, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _i64,
                                   _c_void_p], ctypes.c_int),
     "g2pc_pack_geometry": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p], ctypes.c_int),
@@ -150,12 +163,13 @@ def load(path=None):
 LAUNCHES = 0      # number of hand-written g2pc kernels launched since the last reset
 TIMING = None     # None, or a dict filled as {entry point name: [(start_event, end_event), ...]}: every launch is
                   # bracketed with CUDA events on the current stream (bench.py)
-# hand-written kernels launched per entry point (default 1); the radix sorts inside g2pc_depth_sort and
-# g2pc_knn_mean_dist are cub's (library)
+# hand-written kernels launched per entry point (default 1); the radix sorts and selections inside g2pc_depth_sort,
+# the k-NN and the orientation entry points are cub's (library)
 _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
-                "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_sor_mask": 5, "g2pc_mesh_splat": 5,
+                "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_knn_ids": 6, "g2pc_sor_mask": 5, "g2pc_mesh_splat": 5,
                 "g2pc_mesh_iso": 7, "g2pc_mesh_extract_count": 2, "g2pc_mesh_extract_emit": 2, "g2pc_mesh_gather": 3,
-                "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3}
+                "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
+                "g2pc_orient_round": 5, "g2pc_orient_finish": 3}
 # host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",
                 "g2pc_multisplit_rows", "g2pc_blend_set_compact"}

@@ -2,10 +2,12 @@
 trim and Laplacian smoothing (g2pc/mesh.py).
 
     python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10]
-                      [--laplacian_iterations 10] [--quiet]
+                      [--laplacian_iterations 10] [--orient_normals] [--quiet]
 
 The cloud must carry normals (nx ny nz), as gauss_to_pc.py writes them by default; its colours (red green blue) are
-carried over to the mesh's vertices.  The normals are used as they are: a mesh faces the way its normals point."""
+carried over to the mesh's vertices.  A mesh faces the way its normals point.  By default the normals are used as they
+are; --orient_normals first gives them a consistent sign (g2pc/orient.py, k = 10), which the normals of a cloud sampled
+from Gaussians lack: each takes its sign from its Gaussian's rotation."""
 import argparse
 import time
 
@@ -13,7 +15,7 @@ import numpy as np
 import torch
 
 import gauss_dataloader
-from g2pc import build, mesh
+from g2pc import build, mesh, orient
 
 
 def _depth(s):
@@ -37,6 +39,8 @@ def config_parser(argv=None):
     p.add_argument("--poisson_depth", type=_depth, default=10,
                    help=f"grid of 2^depth nodes per axis, {mesh.DEPTH_MIN}..{mesh.DEPTH_MAX}")
     p.add_argument("--laplacian_iterations", type=_iterations, default=10, help="Laplacian smoothing steps (0: none)")
+    p.add_argument("--orient_normals", action="store_true",
+                   help=f"orient the normals consistently (k = {orient.K_DEFAULT} nearest neighbours) before meshing")
     p.add_argument("--quiet", action="store_true", help="print nothing")
     return p.parse_args(argv)
 
@@ -59,6 +63,10 @@ def main(argv=None):
     points, normals, colours = load_cloud(args.input_path)
     if not args.quiet:
         print(f"Meshing {points.shape[0]} points at depth {args.poisson_depth}")
+    if args.orient_normals:
+        normals, st = orient.orient_normals(points, normals, k=orient.K_DEFAULT)
+        if not args.quiet:
+            print(f"Oriented the normals: {st.flipped} flipped, {st.components} component(s), {st.skipped} skipped")
     m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations)
     mesh.write_mesh_ply(args.mesh_output_path, m)
     if not args.quiet:

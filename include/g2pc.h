@@ -170,6 +170,14 @@ int g2pc_points_per_gaussian(const float* cov, const float* contrib, int64_t n, 
 int64_t g2pc_knn_workspace_bytes(int64_t n);
 int g2pc_knn_mean_dist(const float* xyz, int64_t n, int32_t k, double* avg, int32_t* status, void* workspace,
                        int64_t workspace_bytes, void* stream);
+/* The neighbour lists of a cloud, for the normal orientation (N7).  ids (n,k int32), d2 (n,k float64, or NULL): the k' =
+ * min(k, n - 1) nearest OTHER points of every row by ascending (d2, id) (d2 as for g2pc_knn_mean_dist, ties of d2 to the
+ * smaller row id; exact), in slots 0..k'-1; slots k'..k-1 hold id -1 and d2 +inf.  A row with a non-finite coordinate
+ * gets id -1 and d2 NaN everywhere and is nobody's neighbour; status counts such rows.  1 <= k <= G2PC_ORIENT_K_MAX.
+ * workspace: g2pc_knn_workspace_bytes(n), 256-byte aligned. */
+#define G2PC_ORIENT_K_MAX 31 /* largest k of g2pc_knn_ids: k + the point itself fit the 32-entry list of N5 */
+int g2pc_knn_ids(const float* xyz, int64_t n, int32_t k, int32_t* ids, double* d2, int32_t* status, void* workspace,
+                 int64_t workspace_bytes, void* stream);
 /* stats (3 float64): mean = (sum of avg over avg > 0) / n, std = sqrt((sum of (avg - mean)^2 over avg > 0) / (n - 1)),
  * threshold = mean + std_ratio * std, each sum reduced in a fixed order (bit-identical re-runs); keep (n uint8) =
  * avg > 0 && avg < threshold.  std_ratio > 0.  workspace: g2pc_sor_workspace_bytes(n), 8-byte aligned.  n == 0 writes
@@ -258,6 +266,49 @@ int g2pc_mesh_smooth(double* vpos, int64_t m, const int32_t* faces, int64_t t, i
 int64_t g2pc_mesh_normals_workspace_bytes(int64_t m, int64_t t);
 int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* faces, int64_t t, float* vertices, float* normals,
                       void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- N7: consistent orientation of point-cloud normals (s11_orient.cu, g2pc/orient.py) -------------------------- */
+/* Hoppe et al. 1992 (the rule behind Open3D's orient_normals_consistent_tangent_plane) with this project's own rules
+ * (DESIGN.md §2): k-NN graph, edge weight 1 - |n_i . n_j|, minimum spanning forest, sign propagated from one seed per
+ * tree (its largest z) so that the seed's normal points to +z.  Order of calls: g2pc_orient_prepare, g2pc_knn_ids on the
+ * m usable points, g2pc_orient_edges, g2pc_orient_round for round = 0, 1, ... until a round hooks nothing (one host read
+ * of its counts per round), g2pc_orient_finish. */
+
+/* The usable rows (finite coordinate; finite, non-zero float64 normal length), ascending: rows[0..m), their points
+ * uxyz (m,3 float32) and unit normals unh (m,3 float64, n / sqrt((nx*nx + ny*ny) + nz*nz) without FMA).  Every buffer has
+ * room for n rows; count (one int64) = m.  workspace: g2pc_orient_prepare_workspace_bytes(n), 256-byte aligned. */
+int64_t g2pc_orient_prepare_workspace_bytes(int64_t n);
+int g2pc_orient_prepare(const float* xyz, const void* normals, int normal_dtype, int64_t n, int32_t* rows, float* uxyz,
+                        double* unh, int64_t* count, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* The undirected edges of the k-NN graph of g2pc_knn_ids(uxyz, m, k): edges (E uint64, min << 32 | max) ascending and
+ * unique; keys (c uint64): keys[e] = (float32 bits of max(0, 1 - |dot|)) << 32 | e for e < E, UINT64_MAX after;
+ * flips (E uint8) = dot < 0, dot = (ax*bx + ay*by) + az*bz of the unit normals in float64 without FMA.  Capacity of
+ * every buffer: c = m * min(k, m - 1) entries (below 2^32).  count (one int64) = E.  workspace:
+ * g2pc_orient_edges_workspace_bytes(m, k), 256-byte aligned. */
+int64_t g2pc_orient_edges_workspace_bytes(int64_t m, int32_t k);
+int g2pc_orient_edges(const int32_t* ids, int64_t m, int32_t k, const double* unh, uint64_t* edges, uint64_t* keys,
+                      uint8_t* flips, int64_t* count, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* One Borůvka round over the keys: every component hooks along its smallest outgoing key (in a mutual pair the smaller
+ * representative stays the root) and mst[e] = 1 for each edge used.  comp (m int32): representative of each point;
+ * rel (m uint8): XOR of the flip bits along the tree path to it.  Round 0 initialises comp, rel and mst (c bytes) and
+ * needs active = c; later rounds take active = counts[1] of the round before.  counts (2 int64) = components hooked,
+ * active edges left.  The workspace carries the active edges from round to round: the same buffer for every round,
+ * g2pc_orient_round_workspace_bytes(m, c), 256-byte aligned. */
+int64_t g2pc_orient_round_workspace_bytes(int64_t m, int64_t c);
+int g2pc_orient_round(const uint64_t* edges, const uint64_t* keys, const uint8_t* flips, int64_t m, int64_t c,
+                      int32_t round_index, int64_t active, int32_t* comp, uint8_t* rel, uint8_t* mst, int64_t* counts,
+                      void* workspace, int64_t workspace_bytes, void* stream);
+
+/* out (n,3, the normals' dtype) = normals, with the rows rows[v] of every flipped point v negated: flip(v) = rel(v) ^
+ * rel(s) ^ (unh[s].z < 0), s = the seed of v's component (largest z of uxyz, then smallest index).  seed (m int32) and
+ * seed_rel (m uint8, rel(v) ^ rel(s)) may be NULL.  stats (2 int64) = components, flipped points.  workspace:
+ * g2pc_orient_finish_workspace_bytes(m), 256-byte aligned. */
+int64_t g2pc_orient_finish_workspace_bytes(int64_t m);
+int g2pc_orient_finish(const float* uxyz, const double* unh, const int32_t* rows, int64_t m, const void* normals,
+                       int normal_dtype, int64_t n, const int32_t* comp, const uint8_t* rel, void* out, int32_t* seed,
+                       uint8_t* seed_rel, int64_t* stats, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- S3-S6: colour stage, renderer_type=python semantics (gauss_render.py:101-465) ------------------------------ */
 /* Replaces GaussPythonRenderer.__call__/render (gauss_render.py:266-465) and — as the native op boundary — the role
