@@ -5,6 +5,7 @@ This is the stub a maintainer of the reference would add in place of
 the torch call chains in gauss_to_pc.py:140-275.  There is NO fallback: if the library is missing or a call
 fails, an exception is raised.
 """
+import contextlib
 import ctypes
 import os
 
@@ -180,16 +181,27 @@ def call(name, *args):
     dict — bracket it with CUDA events on the current stream."""
     global LAUNCHES
     fn = getattr(load(), name)
-    if TIMING is not None and name not in _NOT_KERNELS and not name.endswith("_workspace_bytes"):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
+    if TIMING is None or name in _NOT_KERNELS or name.endswith("_workspace_bytes"):
         status = fn(*args)
-        b.record()
-        TIMING.setdefault(name, []).append((a, b))
     else:
-        status = fn(*args)
+        with phase(TIMING, name):
+            status = fn(*args)
     LAUNCHES += _OWN_KERNELS.get(name, 1)
     check(status, name)
+
+
+@contextlib.contextmanager
+def phase(timings, name):
+    """Brackets the block with CUDA events on the current stream and appends the pair to timings[name] when `timings` is
+    a dict; does nothing when it is None."""
+    if timings is None:
+        yield
+        return
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    yield
+    b.record()
+    timings.setdefault(name, []).append((a, b))
 
 
 def check(status, what):
@@ -228,3 +240,38 @@ def require_cuda(*tensors):
         if t is not None and not t.is_cuda:
             raise G2pcError("g2pc kernels need CUDA tensors; there is no CPU fallback "
                             f"(got a tensor on {t.device})")
+
+
+def check_cloud(points, normals=None, colours=None, what=None):
+    """Refuses a point cloud the point-cloud kernels cannot take: points (n, 3) float32; normals, when given, (n, 3)
+    float32 or float64; colours, when given, (n, 3); all CUDA tensors on one device.  `what` names an operation that
+    needs the normals (e.g. "Poisson meshing"): with it, missing normals are refused too."""
+    if what is not None and normals is None:
+        raise G2pcError(f"{what} needs normals (the cloud has none)")
+    if points is None:
+        raise G2pcError(f"{what or 'the point-cloud kernels'} needs the points")
+    require_cuda(points, normals, colours)
+    if points.dim() != 2 or points.shape[1] != 3 or points.dtype != torch.float32:
+        raise G2pcError(f"points must be (n, 3) float32, got {tuple(points.shape)} {points.dtype}")
+    if normals is not None and (normals.shape != points.shape or normals.dtype not in (torch.float32, torch.float64)):
+        raise G2pcError(f"normals must be (n, 3) float32 or float64 like the points, got {tuple(normals.shape)} "
+                        f"{normals.dtype}")
+    if colours is not None and colours.shape != points.shape:
+        raise G2pcError(f"colours must be (n, 3) like the points, got {tuple(colours.shape)}")
+    devices = [str(t.device) for t in (points, normals, colours) if t is not None]
+    if len(set(devices)) > 1:
+        raise G2pcError(f"the points, normals and colours are on different devices ({', '.join(devices)})")
+
+
+def gather_rows(index, m, tensors):
+    """Rows index[:m] (int32 CUDA) of every tensor in `tensors`, compacted by one g2pc_gather_rows call: a list of new
+    (m, ...) tensors with the sources' dtypes, in the order of `tensors`."""
+    dev = index.device
+    srcs = [t.contiguous() for t in tensors]
+    dsts = [torch.empty((m,) + tuple(s.shape[1:]), dtype=s.dtype, device=dev) for s in srcs]
+    if m > 0:
+        k = len(srcs)
+        call("g2pc_gather_rows", ptr(index), m, k, (ctypes.c_void_p * k)(*[s.data_ptr() for s in srcs]),
+             (ctypes.c_void_p * k)(*[d.data_ptr() for d in dsts]),
+             (ctypes.c_int32 * k)(*[s[0].numel() * s.element_size() for s in srcs]), stream_ptr(dev))
+    return dsts

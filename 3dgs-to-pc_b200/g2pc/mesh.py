@@ -8,7 +8,6 @@ cycles -> g2pc_mesh_iso -> g2pc_mesh_extract_count / _emit (marching tetrahedra)
 residual once per cycle, the vertex / triangle counts before and after the trim.
 """
 import collections
-import contextlib
 import math
 
 import numpy as np
@@ -23,19 +22,6 @@ TOLERANCE = 1e-5
 NB_NEIGHBORS = 20
 
 Mesh = collections.namedtuple("Mesh", ["vertices", "faces", "colours", "normals", "densities"])
-
-
-@contextlib.contextmanager
-def _phase(timings, name):
-    """Brackets a phase with CUDA events on the current stream when `timings` is a dict."""
-    if timings is None:
-        yield
-        return
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    yield
-    b.record()
-    timings.setdefault(name, []).append((a, b))
 
 
 def splat(points, normals, depth):
@@ -161,26 +147,6 @@ def vertex_normals(vpos, faces):
     return v, nrm
 
 
-def _check_inputs(points, normals, colours, depth, laplacian_iters):
-    if normals is None:
-        raise capi.G2pcError("Poisson meshing needs normals (the cloud has none)")
-    capi.require_cuda(points, normals, colours)
-    if points.dim() != 2 or points.shape[1] != 3 or points.dtype != torch.float32:
-        raise capi.G2pcError(f"points must be (n, 3) float32, got {tuple(points.shape)} {points.dtype}")
-    if normals.shape != points.shape or normals.dtype not in (torch.float32, torch.float64):
-        raise capi.G2pcError(f"normals must be (n, 3) float32 or float64 like the points, got {tuple(normals.shape)} "
-                             f"{normals.dtype}")
-    if colours is not None and colours.shape != points.shape:
-        raise capi.G2pcError(f"colours must be (n, 3) like the points, got {tuple(colours.shape)}")
-    if int(depth) != depth or not DEPTH_MIN <= depth <= DEPTH_MAX:
-        raise capi.G2pcError(f"depth must be an integer in {DEPTH_MIN}..{DEPTH_MAX} (the dense int64 right-hand side "
-                             f"alone is 69 GB at depth 11), got {depth}")
-    if int(laplacian_iters) != laplacian_iters or laplacian_iters < 0:
-        raise capi.G2pcError(f"laplacian_iters must be an integer >= 0, got {laplacian_iters}")
-    if points.shape[0] == 0:
-        raise capi.G2pcError("the point cloud is empty")
-
-
 def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, std_ratio=3.0, return_debug=False,
                  timings=None):
     """Mesh of an oriented point cloud.  points (n,3) float32 CUDA; normals (n,3) float32 / float64 (outward for an
@@ -189,15 +155,22 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     (R^3 float32, mean-free), iso, B (R^3 int64), frame, cycles, ratio (final |r| / |b|), skipped (points whose normal is
     zero or not finite), keep (vertex trim mask), threshold.  `timings`: a dict that receives CUDA event pairs per phase
     (clean, splat, solve, extract, gather_trim, smooth, normals)."""
-    _check_inputs(points, normals, colours, depth, laplacian_iters)
+    capi.check_cloud(points, normals, colours, what="Poisson meshing")
+    if int(depth) != depth or not DEPTH_MIN <= depth <= DEPTH_MAX:
+        raise capi.G2pcError(f"depth must be an integer in {DEPTH_MIN}..{DEPTH_MAX} (the dense int64 right-hand side "
+                             f"alone is 69 GB at depth 11), got {depth}")
+    if int(laplacian_iters) != laplacian_iters or laplacian_iters < 0:
+        raise capi.G2pcError(f"laplacian_iters must be an integer >= 0, got {laplacian_iters}")
+    if points.shape[0] == 0:
+        raise capi.G2pcError("the point cloud is empty")
     depth, dev = int(depth), points.device
-    with _phase(timings, "clean"):
+    with capi.phase(timings, "clean"):
         pts, cols, nrm = outliers.remove_statistical_outliers(points, colours, normals, NB_NEIGHBORS, std_ratio)
         pts, nrm = pts.contiguous(), nrm.contiguous()
         cols = cols.contiguous() if cols is not None else None
     if pts.shape[0] == 0:
         raise capi.G2pcError("no point is left after the outlier removal")
-    with _phase(timings, "splat"):
+    with capi.phase(timings, "splat"):
         frame, B, cell, status = splat(pts, nrm, depth)
         host = torch.cat([frame, status.to(torch.float64)]).tolist()
     extent, skipped, bad = host[6], int(host[FRAME_WORDS]), int(host[FRAME_WORDS + 1])
@@ -207,23 +180,23 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
         raise capi.G2pcError("the point cloud has zero extent: every point is at the same place")
     if skipped == pts.shape[0]:
         raise capi.G2pcError("no point has a usable normal (all are zero or not finite)")
-    with _phase(timings, "solve"):
+    with capi.phase(timings, "solve"):
         chi, cycles, ratio = solve(B, frame, depth)
         iso = iso_value(pts, cell, frame, depth, chi)
     debug = {}
     if return_debug:
         debug = {"B": B.clone(), "frame": frame, "cycles": cycles, "ratio": ratio, "skipped": skipped}
-    with _phase(timings, "extract"):
+    with capi.phase(timings, "extract"):
         # B is dead after the solve: its memory holds the node lists of the extraction and the cell lists of the gather
         vkey, vt, vpos, faces = extract(chi, depth, frame, iso, B)
     if vkey.shape[0] == 0:
         raise capi.G2pcError("no surface: the indicator function does not cross its iso-value")
-    with _phase(timings, "gather_trim"):
+    with capi.phase(timings, "gather_trim"):
         dens, vcol = gather(pts, cols.to(torch.int32) if cols is not None else None, cell, frame, depth, vkey, vt, B)
         dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
-    with _phase(timings, "smooth"):
+    with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
-    with _phase(timings, "normals"):
+    with capi.phase(timings, "normals"):
         v, vn = vertex_normals(vpos, faces)
     out = Mesh(v, faces, vcol, vn, dens)
     if return_debug:

@@ -8,7 +8,6 @@ g2pc_orient_finish (seed per component, flips, output).  Host reads: the usable 
 counts once per round, the stats at the end.
 """
 import collections
-import contextlib
 
 import torch
 
@@ -18,18 +17,6 @@ K_MAX = 31  # G2PC_ORIENT_K_MAX in include/g2pc.h
 K_DEFAULT = 10
 
 OrientStats = collections.namedtuple("OrientStats", ["components", "flipped", "skipped", "rounds"])
-
-
-@contextlib.contextmanager
-def _phase(timings, name):
-    if timings is None:
-        yield
-        return
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    yield
-    b.record()
-    timings.setdefault(name, []).append((a, b))
 
 
 def knn_ids(xyz, k):
@@ -45,23 +32,6 @@ def knn_ids(xyz, k):
     return ids, d2, status
 
 
-def _check_inputs(points, normals, k):
-    if normals is None:
-        raise capi.G2pcError("orienting normals needs normals (the cloud has none)")
-    if points is None:
-        raise capi.G2pcError("orienting normals needs the points")
-    capi.require_cuda(points, normals)
-    if points.dim() != 2 or points.shape[1] != 3 or points.dtype != torch.float32:
-        raise capi.G2pcError(f"points must be (n, 3) float32, got {tuple(points.shape)} {points.dtype}")
-    if normals.shape != points.shape or normals.dtype not in (torch.float32, torch.float64):
-        raise capi.G2pcError(f"normals must be (n, 3) float32 or float64 like the points, got {tuple(normals.shape)} "
-                             f"{normals.dtype}")
-    if isinstance(k, bool) or int(k) != k or not 1 <= k <= K_MAX:
-        raise capi.G2pcError(f"k must be an integer in 1..{K_MAX}, got {k}")
-    if points.device != normals.device:
-        raise capi.G2pcError(f"points and normals are on different devices ({points.device}, {normals.device})")
-
-
 def orient_normals(points, normals, k=K_DEFAULT, return_debug=False, timings=None):
     """Normals with a consistent sign.  points (n,3) float32 CUDA; normals (n,3) float32 / float64 CUDA (not modified).
     Returns (oriented normals: the input's dtype, values and magnitudes, with the sign of every flipped row negated;
@@ -72,11 +42,13 @@ def orient_normals(points, normals, k=K_DEFAULT, return_debug=False, timings=Non
     spanning forest's edge numbers, ascending), rel (m,) uint8 (flip parity to the component's seed), seed (m,) int32
     (the seed of each point's component).  `timings`: a dict that receives CUDA event pairs per phase (prepare, knn,
     edges, rounds, finish)."""
-    _check_inputs(points, normals, k)
+    capi.check_cloud(points, normals, what="orienting normals")
+    if isinstance(k, bool) or int(k) != k or not 1 <= k <= K_MAX:
+        raise capi.G2pcError(f"k must be an integer in 1..{K_MAX}, got {k}")
     k, dev, n = int(k), points.device, points.shape[0]
     pts, nrm = points.contiguous(), normals.contiguous()
     lib, st = capi.load(), capi.stream_ptr(dev)
-    with _phase(timings, "prepare"):
+    with capi.phase(timings, "prepare"):
         rows = torch.empty((n,), dtype=torch.int32, device=dev)
         uxyz = torch.empty((n, 3), dtype=torch.float32, device=dev)
         unh = torch.empty((n, 3), dtype=torch.float64, device=dev)
@@ -86,12 +58,12 @@ def orient_normals(points, normals, k=K_DEFAULT, return_debug=False, timings=Non
                   capi.ptr(uxyz), capi.ptr(unh), capi.ptr(count), capi.ptr(ws), ws.numel(), st)
         del ws
         m = int(count.item())
-    with _phase(timings, "knn"):
+    with capi.phase(timings, "knn"):
         ids, d2, _ = knn_ids(uxyz[:m], k) if m else (torch.empty((0, k), dtype=torch.int32, device=dev),
                                                      torch.empty((0, k), dtype=torch.float64, device=dev), None)
     kp = min(k, m - 1) if m > 1 else 0
     c = m * kp
-    with _phase(timings, "edges"):
+    with capi.phase(timings, "edges"):
         edges = torch.empty((max(c, 1),), dtype=torch.int64, device=dev)
         keys = torch.empty((max(c, 1),), dtype=torch.int64, device=dev)
         flips = torch.empty((max(c, 1),), dtype=torch.uint8, device=dev)
@@ -105,7 +77,7 @@ def orient_normals(points, normals, k=K_DEFAULT, return_debug=False, timings=Non
     rel = torch.empty((max(m, 1),), dtype=torch.uint8, device=dev)
     mst = torch.empty((max(c, 1),), dtype=torch.uint8, device=dev)
     rounds = 0
-    with _phase(timings, "rounds"):
+    with capi.phase(timings, "rounds"):
         if m:
             counts = torch.empty((2,), dtype=torch.int64, device=dev)
             ws = capi.workspace(lib.g2pc_orient_round_workspace_bytes(m, c), dev)
@@ -118,7 +90,7 @@ def orient_normals(points, normals, k=K_DEFAULT, return_debug=False, timings=Non
                 if hooked == 0 or active == 0:
                     break
             del ws
-    with _phase(timings, "finish"):
+    with capi.phase(timings, "finish"):
         out = torch.empty_like(nrm)
         seed = torch.empty((max(m, 1),), dtype=torch.int32, device=dev) if return_debug else None
         srel = torch.empty((max(m, 1),), dtype=torch.uint8, device=dev) if return_debug else None

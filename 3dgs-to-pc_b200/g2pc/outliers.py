@@ -5,8 +5,6 @@ The reference cleans the finished cloud with Open3D's remove_statistical_outlier
 statistics and keep rule), then the existing compaction, g2pc_cull_select with the keep mask as its extra mask and
 g2pc_gather_rows.  One host read: the kept count and the non-finite-point count, together.
 """
-import ctypes
-
 import torch
 
 from . import capi
@@ -42,19 +40,13 @@ def remove_statistical_outliers(points, colours, normals, nb_neighbors=20, std_r
     or None, returned as clamp(colours, 0, 255) truncated to int32 like the reference's Open3D round trip; normals (n,3)
     or None (None stays None).  The kept rows keep their order.  With return_debug, also returns
     {"avg", "keep", "stats"}."""
-    capi.require_cuda(points, colours, normals)
-    if points.dim() != 2 or points.shape[1] != 3 or points.dtype != torch.float32:
-        raise capi.G2pcError(f"points must be (n, 3) float32, got {tuple(points.shape)} {points.dtype}")
+    capi.check_cloud(points, normals, colours)
     k = int(nb_neighbors)
     if not 1 <= k <= K_MAX:
         raise capi.G2pcError(f"nb_neighbors must be in 1..{K_MAX}, got {nb_neighbors}")
     if not float(std_ratio) > 0.0:
         raise capi.G2pcError(f"std_ratio must be > 0, got {std_ratio}")
-    n = points.shape[0]
-    for name, t in (("colours", colours), ("normals", normals)):
-        if t is not None and (t.dim() != 2 or t.shape[0] != n or t.shape[1] != 3):
-            raise capi.G2pcError(f"{name} must be (n, 3) like the points, got {tuple(t.shape)}")
-    dev = points.device
+    n, dev = points.shape[0], points.device
     if colours is not None:
         colours = torch.clamp(colours, min=0, max=255).to(torch.int32)  # mesh_handler.py:45 of the reference
     xyz = points.contiguous()
@@ -70,15 +62,7 @@ def remove_statistical_outliers(points, colours, normals, nb_neighbors=20, std_r
     m, bad = torch.cat([count, status.to(torch.int64)]).tolist()  # the one host read
     if bad:
         raise capi.G2pcError(f"{bad} point(s) have a non-finite coordinate; the outlier statistics are undefined")
-    index = index[:m]
-    srcs = [t.contiguous() for t in (xyz, colours, normals) if t is not None]
-    dsts = [torch.empty((m, 3), dtype=s.dtype, device=dev) for s in srcs]
-    if m > 0:
-        c = len(srcs)
-        capi.call("g2pc_gather_rows", capi.ptr(index), m, c, (ctypes.c_void_p * c)(*[s.data_ptr() for s in srcs]),
-                  (ctypes.c_void_p * c)(*[d.data_ptr() for d in dsts]),
-                  (ctypes.c_int32 * c)(*[3 * s.element_size() for s in srcs]), st)
-    it = iter(dsts)
+    it = iter(capi.gather_rows(index, m, [t for t in (xyz, colours, normals) if t is not None]))
     out = tuple(next(it) if t is not None else None for t in (xyz, colours, normals))
     if return_debug:
         return out + ({"avg": avg, "keep": keep, "stats": stats},)

@@ -1,7 +1,8 @@
 """Deterministic synthetic 3DGS scenes and camera rigs (BASELINE.md §3.2) for tests and bench.py.
 
 Everything is generated on the CPU with a seeded torch.Generator and moved to the device by the caller, so the
-same scene is seen by the GPU path and by the CPU oracle.
+same scene is seen by the GPU path and by the CPU oracle; sampled_cloud is the exception, a point cloud sampled on the
+device from such a scene.
 """
 import math
 
@@ -41,6 +42,24 @@ def make_scene(n, seed=1234, sh_degree=3, dtype_like_ply=True):
         "colours": colours,
     }
     return out
+
+
+def sampled_cloud(n_gaussians, num_points, seed, device):
+    """PointCloudData of make_scene(n_gaussians, seed) sampled on `device` the way the CLI samples with
+    --no_render_colours; with 3 M Gaussians and 10 M points, the C3-like cloud of the point-cloud benchmarks."""
+    import gauss_to_pc as g2p
+    from . import sampler
+    sc = {k: v.to(device) for k, v in make_scene(n_gaussians, seed=seed).items()}
+    st = g2p.GaussPointCloudSettings(
+        renderer_type="python", num_points=num_points, prioritise_visible_gaussians=True, mahalanobis_distance_std=2.0,
+        camera_skip_rate=0, render_colours=False, min_opacity=0.0, bounding_box_min=None, bounding_box_max=None,
+        calculate_normals=True, cull_large_percentage=0.0, remove_unrendered_gaussians=True, colour_resolution=None,
+        max_sh_degree=3, exact_num_points=False, visibility_threshold=0.05, surface_distance_std=None,
+        generate_mesh=False, quiet=True, device=device)
+    sampler.reset_call_counter(0)
+    pc, _ = g2p.convert_gaussians_to_pc(sc["xyz"], sc["scales"], sc["rots"], sc["colours"].clone() * 255,
+                                        sc["opacities"], sc["shs"], None, None, None, st)
+    return pc
 
 
 def look_at_c2w(eye, target=(0.0, 0.0, 0.0), up=(0.0, 0.0, 1.0)):

@@ -162,15 +162,7 @@ class Gaussians():
         m = int(count.item())  # the one host read: output sizes
         index = index[:m]
         names = [k for k in ("xyz", "colours", "opacities", "covariances", "normals", "ids") if getattr(self, k) is not None]
-        srcs = [getattr(self, k).contiguous() for k in names]
-        dsts = [torch.empty((m,) + tuple(s.shape[1:]), dtype=s.dtype, device=dev) for s in srcs]
-        if m > 0:
-            k = len(srcs)
-            sp = (ctypes.c_void_p * k)(*[s.data_ptr() for s in srcs])
-            dp = (ctypes.c_void_p * k)(*[d.data_ptr() for d in dsts])
-            rb = (ctypes.c_int32 * k)(*[int(s[0].numel() * s.element_size()) if s.dim() > 1 else int(s.element_size()) for s in srcs])
-            capi.call("g2pc_gather_rows", capi.ptr(index), m, k, sp, dp, rb, st)
-        for name, d in zip(names, dsts):
+        for name, d in zip(names, capi.gather_rows(index, m, [getattr(self, k) for k in names])):
             setattr(self, name, d)
         index64 = index.to(torch.int64)
         self._lazy_filter(index64)

@@ -37,52 +37,40 @@ def card():
     return name, out
 
 
-def sampled_cloud(num_points, seed):
-    import gauss_to_pc as g2p
-    from g2pc import sampler, synth
-    sc = {k: v.to(DEV) for k, v in synth.make_scene(3_000_000, seed=seed).items()}
-    st = g2p.GaussPointCloudSettings(
-        renderer_type="python", num_points=num_points, prioritise_visible_gaussians=True, mahalanobis_distance_std=2.0,
-        camera_skip_rate=0, render_colours=False, min_opacity=0.0, bounding_box_min=None, bounding_box_max=None,
-        calculate_normals=True, cull_large_percentage=0.0, remove_unrendered_gaussians=True, colour_resolution=None,
-        max_sh_degree=3, exact_num_points=False, visibility_threshold=0.05, surface_distance_std=None,
-        generate_mesh=False, quiet=True, device=DEV)
-    sampler.reset_call_counter(0)
-    pc, _ = g2p.convert_gaussians_to_pc(sc["xyz"], sc["scales"], sc["rots"], sc["colours"].clone() * 255,
-                                        sc["opacities"], sc["shs"], None, None, None, st)
-    del sc
-    return pc
+def timed_runs(call, phases, runs):
+    """`runs` calls of call(timings), each between two device synchronisations, with the peak-memory statistics reset
+    first.  Returns the CUDA-event time of every whole call and, for each name in `phases`, the sum of the event pairs
+    the call put under that name in `timings`, per run (ms)."""
+    torch.cuda.reset_peak_memory_stats()
+    total, per_phase = [], {p: [] for p in phases}
+    for _ in range(runs):
+        timings = {}
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        a.record()
+        call(timings)
+        b.record()
+        torch.cuda.synchronize()
+        total.append(a.elapsed_time(b))
+        for p in phases:
+            per_phase[p].append(sum(s.elapsed_time(e) for s, e in timings[p]))
+    return total, per_phase
+
+
+def spread(ms, digits):
+    """Median and range of a list of times, rounded to `digits` decimals."""
+    return {"median_ms": round(float(np.median(ms)), digits), "min_ms": round(min(ms), digits),
+            "max_ms": round(max(ms), digits)}
 
 
 def time_clean(pc, runs):
     from g2pc import outliers
-    clean = lambda: outliers.remove_statistical_outliers(pc.points, pc.colours, pc.normals, 20, 10.0)
-    out = clean()  # warm-up
-    kept = int(out[0].shape[0])
-    del out
-    ms = []
-    for _ in range(runs):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        a.record()
-        out = clean()
-        b.record()
-        torch.cuda.synchronize()
-        ms.append(a.elapsed_time(b))
-        del out
+    clean = lambda timings=None: outliers.remove_statistical_outliers(pc.points, pc.colours, pc.normals, 20, 10.0)
+    kept = int(clean()[0].shape[0])  # warm-up
+    ms, _ = timed_runs(clean, (), runs)
     # the k-NN kernels alone (index build + queries), same warm state
-    from g2pc import outliers as o
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    knn = []
-    for _ in range(runs):
-        torch.cuda.synchronize()
-        a.record()
-        o.mean_distances(pc.points, 20)
-        b.record()
-        torch.cuda.synchronize()
-        knn.append(a.elapsed_time(b))
-    return {"points": int(pc.points.shape[0]), "kept": kept, "median_ms": round(float(np.median(ms)), 2),
-            "min_ms": round(min(ms), 2), "max_ms": round(max(ms), 2), "runs": runs,
+    knn, _ = timed_runs(lambda timings: outliers.mean_distances(pc.points, 20), (), runs)
+    return {"points": int(pc.points.shape[0]), "kept": kept, **spread(ms, 2), "runs": runs,
             "knn_median_ms": round(float(np.median(knn)), 2)}
 
 
@@ -112,14 +100,14 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_clean.py needs a CUDA device")
-    from g2pc import build
+    from g2pc import build, synth
     build.build()
     name, power = card()
     res = {"metric": "statistical outlier removal (k = 20, std_ratio = 10), whole clean", "card": name,
            "power_limit": power, "gpu": []}
     cpu_done = False
     for n in [int(s) for s in args.sizes.split(",")]:
-        pc = sampled_cloud(n, seed=1234 + (2 if n <= 10_000_000 else 3))
+        pc = synth.sampled_cloud(3_000_000, n, 1234 + (2 if n <= 10_000_000 else 3), DEV)
         r = time_clean(pc, args.runs)
         res["gpu"].append(r)
         print(f"[clean] {r}", file=sys.stderr)

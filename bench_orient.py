@@ -21,7 +21,7 @@ sys.path.insert(0, os.path.join(ROOT, "3dgs-to-pc_b200"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from bench_clean import card, sampled_cloud  # noqa: E402
+from bench_clean import DEV, card, spread, timed_runs  # noqa: E402
 
 PHASES = ("prepare", "knn", "edges", "rounds", "finish")
 
@@ -33,35 +33,21 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_orient.py needs a CUDA device")
-    from g2pc import build, orient
+    from g2pc import build, orient, synth
     build.build()
     name, power = card()
-    pc = sampled_cloud(args.points, seed=1236)
+    pc = synth.sampled_cloud(3_000_000, args.points, 1236, DEV)
     pts, nrm = pc.points, pc.normals
     del pc
     torch.cuda.empty_cache()
-    orient.orient_normals(pts, nrm, k=10)  # warm-up
+    stats = orient.orient_normals(pts, nrm, k=10)[1]  # warm-up
     torch.cuda.synchronize()
     base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    total, phases, stats = [], {p: [] for p in PHASES}, None
-    for _ in range(args.runs):
-        timings = {}
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        a.record()
-        out, stats = orient.orient_normals(pts, nrm, k=10, timings=timings)
-        b.record()
-        torch.cuda.synchronize()
-        total.append(a.elapsed_time(b))
-        for p in PHASES:
-            phases[p].append(sum(s.elapsed_time(e) for s, e in timings[p]))
-        del out
+    total, phases = timed_runs(lambda timings: orient.orient_normals(pts, nrm, k=10, timings=timings), PHASES, args.runs)
     peak = (torch.cuda.max_memory_allocated() - base) / 2 ** 30
-    r = lambda v: round(float(v), 2)
     res = {"metric": "normal orientation (k = 10), whole call", "card": name, "power_limit": power,
-           "points": int(pts.shape[0]), "runs": args.runs, "median_ms": r(np.median(total)), "min_ms": r(min(total)),
-           "max_ms": r(max(total)), "phase_median_ms": {p: r(np.median(v)) for p, v in phases.items()},
+           "points": int(pts.shape[0]), "runs": args.runs, **spread(total, 2),
+           "phase_median_ms": {p: round(float(np.median(v)), 2) for p, v in phases.items()},
            "rounds": stats.rounds, "components": stats.components, "flipped": stats.flipped, "skipped": stats.skipped,
            "peak_gib_above_inputs": round(peak, 2)}
     print(json.dumps(res))

@@ -14,20 +14,19 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from g2pc import outliers  # noqa: E402
-from sanitizer_harness import poison_allocator  # noqa: E402
+from sanitizer_harness import target_main  # noqa: E402
 
-dev = "cuda:0"
-if os.environ.get("G2PC_TARGET_POISON") is not None:
-    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
-rng = np.random.default_rng(3)
-p = np.concatenate([rng.random((3000, 3)), np.repeat(rng.random((1, 3)), 25, 0), [[40.0, 40.0, 40.0]],
-                    0.5 + 1e-6 * rng.random((500, 3))]).astype(np.float32)
-xyz = torch.from_numpy(p).to(dev)
-cols = torch.from_numpy(rng.uniform(-10, 300, p.shape).astype(np.float32)).to(dev)
-nrm = torch.from_numpy(rng.normal(size=p.shape).astype(np.float32)).to(dev)
-pts, c, n, dbg = outliers.remove_statistical_outliers(xyz, cols, nrm, 20, 3.0, return_debug=True)
-torch.cuda.synchronize()
-if os.environ.get("G2PC_TARGET_OUT"):
-    outputs = dict(points=pts, colours=c, normals=n, **dbg)
-    np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
-print("CLEAN_TARGET_OK", pts.shape[0])
+
+def run():
+    dev = "cuda:0"
+    rng = np.random.default_rng(3)
+    p = np.concatenate([rng.random((3000, 3)), np.repeat(rng.random((1, 3)), 25, 0), [[40.0, 40.0, 40.0]],
+                        0.5 + 1e-6 * rng.random((500, 3))]).astype(np.float32)
+    xyz = torch.from_numpy(p).to(dev)
+    cols = torch.from_numpy(rng.uniform(-10, 300, p.shape).astype(np.float32)).to(dev)
+    nrm = torch.from_numpy(rng.normal(size=p.shape).astype(np.float32)).to(dev)
+    pts, c, n, dbg = outliers.remove_statistical_outliers(xyz, cols, nrm, 20, 3.0, return_debug=True)
+    return dict(points=pts, colours=c, normals=n, **dbg), (pts.shape[0],)
+
+
+target_main("CLEAN_TARGET_OK", run)

@@ -14,21 +14,21 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from g2pc import mesh  # noqa: E402
-from sanitizer_harness import poison_allocator  # noqa: E402
+from sanitizer_harness import target_main  # noqa: E402
 
-dev = "cuda:0"
-if os.environ.get("G2PC_TARGET_POISON") is not None:
-    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
-rng = np.random.default_rng(3)
-d = rng.normal(size=(3000, 3))
-d /= np.linalg.norm(d, axis=1, keepdims=True)
-p = np.concatenate([0.8 * d, [[0.0, 0.0, 0.0]]]).astype(np.float32)
-nrm = np.concatenate([d, [[0.0, 0.0, 0.0]]]).astype(np.float32)
-cols = rng.uniform(0, 255, p.shape).astype(np.float32)
-m, dbg = mesh.poisson_mesh(torch.from_numpy(p).to(dev), torch.from_numpy(nrm).to(dev), torch.from_numpy(cols).to(dev),
-                           depth=4, laplacian_iters=2, return_debug=True)
-torch.cuda.synchronize()
-if os.environ.get("G2PC_TARGET_OUT"):
+
+def run():
+    dev = "cuda:0"
+    rng = np.random.default_rng(3)
+    d = rng.normal(size=(3000, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    p = np.concatenate([0.8 * d, [[0.0, 0.0, 0.0]]]).astype(np.float32)
+    nrm = np.concatenate([d, [[0.0, 0.0, 0.0]]]).astype(np.float32)
+    cols = rng.uniform(0, 255, p.shape).astype(np.float32)
+    m, dbg = mesh.poisson_mesh(torch.from_numpy(p).to(dev), torch.from_numpy(nrm).to(dev),
+                               torch.from_numpy(cols).to(dev), depth=4, laplacian_iters=2, return_debug=True)
     outputs = dict(m._asdict(), **{k: dbg[k] for k in ("chi", "iso", "B", "keep", "threshold")})
-    np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
-print("MESH_TARGET_OK", m.vertices.shape[0], m.faces.shape[0])
+    return outputs, (m.vertices.shape[0], m.faces.shape[0])
+
+
+target_main("MESH_TARGET_OK", run)

@@ -14,23 +14,22 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from g2pc import orient  # noqa: E402
-from sanitizer_harness import poison_allocator  # noqa: E402
+from sanitizer_harness import target_main  # noqa: E402
 
-dev = "cuda:0"
-if os.environ.get("G2PC_TARGET_POISON") is not None:
-    poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0))
-rng = np.random.default_rng(3)
-d = rng.normal(size=(3000, 3))
-d /= np.linalg.norm(d, axis=1, keepdims=True)
-p = np.concatenate([d, np.repeat(rng.random((1, 3)), 25, 0), [[40.0, 40.0, 40.0]],
-                    0.5 + 1e-6 * rng.random((500, 3))]).astype(np.float32)
-n = rng.normal(size=p.shape).astype(np.float32)
-n[:3000] = d * np.where(rng.random(3000) < 0.5, -1.0, 1.0)[:, None]
-n[5] = 0.0
-n[6, 1] = np.nan
-out, st, dbg = orient.orient_normals(torch.from_numpy(p).to(dev), torch.from_numpy(n).to(dev), return_debug=True)
-torch.cuda.synchronize()
-if os.environ.get("G2PC_TARGET_OUT"):
-    outputs = dict(normals=out, stats=torch.tensor(list(st)), **dbg)
-    np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
-print("ORIENT_TARGET_OK", st.components, st.flipped)
+
+def run():
+    dev = "cuda:0"
+    rng = np.random.default_rng(3)
+    d = rng.normal(size=(3000, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    p = np.concatenate([d, np.repeat(rng.random((1, 3)), 25, 0), [[40.0, 40.0, 40.0]],
+                        0.5 + 1e-6 * rng.random((500, 3))]).astype(np.float32)
+    n = rng.normal(size=p.shape).astype(np.float32)
+    n[:3000] = d * np.where(rng.random(3000) < 0.5, -1.0, 1.0)[:, None]
+    n[5] = 0.0
+    n[6, 1] = np.nan
+    out, st, dbg = orient.orient_normals(torch.from_numpy(p).to(dev), torch.from_numpy(n).to(dev), return_debug=True)
+    return dict(normals=out, stats=torch.tensor(list(st)), **dbg), (st.components, st.flipped)
+
+
+target_main("ORIENT_TARGET_OK", run)

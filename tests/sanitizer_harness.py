@@ -1,4 +1,5 @@
-"""Runs a GPU test target under compute-sanitizer, and the allocator poisoning the targets and tests use.
+"""Runs a GPU test target under compute-sanitizer; the allocator poisoning the targets and tests use, the body every
+target shares (target_main) and the tests' check that a run repeats bit for bit on poisoned memory (assert_repeatable).
 
 A target is a small script that prints a marker line when it finishes and, with G2PC_TARGET_OUT=<file.npz>, saves every
 output of its run there.  Where compute-sanitizer is missing or does not support the GPU, the target runs without it and
@@ -14,6 +15,8 @@ import sys
 
 import numpy as np
 import pytest
+
+from util import same
 
 DEV = "cuda:0"
 
@@ -46,6 +49,34 @@ def poison_allocator(byte, large_bytes=64 << 20, large_blocks=4):
         probe = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
         assert bool((probe == byte).all()), f"allocator memory not poisoned ({nbytes} B block)"
         del probe
+
+
+def assert_repeatable(run, **poison_kwargs):
+    """Two runs of run() (a list of host outputs: arrays, or plain values such as cycle counts), then a third on
+    allocator memory filled by poison_allocator(**poison_kwargs); all three must agree bit for bit.  Returns the first
+    run's outputs."""
+    runs = [run() for _ in range(2)]
+    poison_allocator(**poison_kwargs)
+    runs.append(run())
+    for r in runs[1:]:
+        assert len(r) == len(runs[0])
+        for a, b in zip(runs[0], r):
+            assert same(a, b) if isinstance(a, np.ndarray) else a == b
+    return runs[0]
+
+
+def target_main(marker, run, **poison_kwargs):
+    """The body of a target script: poisons the allocator with poison_allocator(G2PC_TARGET_POISON, **poison_kwargs)
+    when that variable is set, calls run() -> (dict of output tensors, values to print), saves the outputs to
+    G2PC_TARGET_OUT when that is set, and prints the marker line with the values."""
+    import torch
+    if os.environ.get("G2PC_TARGET_POISON") is not None:
+        poison_allocator(int(os.environ["G2PC_TARGET_POISON"], 0), **poison_kwargs)
+    outputs, values = run()
+    torch.cuda.synchronize()
+    if os.environ.get("G2PC_TARGET_OUT"):
+        np.savez(os.environ["G2PC_TARGET_OUT"], **{k: v.detach().cpu().numpy() for k, v in outputs.items()})
+    print(marker, *values)
 
 
 def _sanitizer():

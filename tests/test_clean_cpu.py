@@ -3,25 +3,20 @@ pinned against all pairs on small and degenerate clouds, and the CLI accepting -
 import numpy as np
 import pytest
 
+import clouds
 import f64ref_outliers
 
 K = 20
 
 
-def _lattice(m):
-    g = np.arange(m, dtype=np.float32)
-    return np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3)
-
-
 def _clouds():
     rng = np.random.default_rng(5)
-    u = lambda n: rng.random((n, 3)).astype(np.float32)
+    u = lambda n: clouds.uniform(n, rng)
     out = {f"n{n}": u(n) for n in (0, 1, 2, K - 1, K, K + 1)}
     for run in (K - 2, K - 1, K):  # exact duplicates
         out[f"dup{run}"] = np.concatenate([np.repeat(u(1), run, 0), u(40), np.repeat(u(1), run, 0)])
-    out["lattice"] = _lattice(5)  # 6 neighbours at 1, 12 at sqrt 2, 8 at sqrt 3: ties at the 20th slot
-    plane = u(300); plane[:, 2] = 0.25
-    out["plane"] = plane
+    out["lattice"] = clouds.lattice(5)  # 6 neighbours at 1, 12 at sqrt 2, 8 at sqrt 3: ties at the 20th slot
+    out["plane"] = clouds.plane(300, rng, 0.0, 1.0, 0.25)
     t = rng.random(200).astype(np.float32)
     out["line"] = np.stack([t, 2 * t, np.full_like(t, -1)], 1).astype(np.float32)
     return out

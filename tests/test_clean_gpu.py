@@ -13,8 +13,10 @@ import numpy as np
 import pytest
 import torch
 
+import clouds
 import f64ref_outliers
-from sanitizer_harness import check_target, poison_allocator
+from sanitizer_harness import assert_repeatable, check_target
+from util import same
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -24,49 +26,25 @@ K_MAX = 32
 BAND = 1e-12
 
 
-def _sampled_cloud(n_gaussians, num_points, seed):
-    """Point cloud of a synthetic scene sampled the way the CLI does with --no_render_colours."""
-    import gauss_to_pc as g2p
-    from g2pc import sampler, synth
-    sc = {k: v.to(DEV) for k, v in synth.make_scene(n_gaussians, seed=seed).items()}
-    st = g2p.GaussPointCloudSettings(
-        renderer_type="python", num_points=num_points, prioritise_visible_gaussians=True, mahalanobis_distance_std=2.0,
-        camera_skip_rate=0, render_colours=False, min_opacity=0.0, bounding_box_min=None, bounding_box_max=None,
-        calculate_normals=True, cull_large_percentage=0.0, remove_unrendered_gaussians=True, colour_resolution=None,
-        max_sh_degree=3, exact_num_points=False, visibility_threshold=0.05, surface_distance_std=None,
-        generate_mesh=False, quiet=True, device=DEV)
-    sampler.reset_call_counter(0)
-    pc, _ = g2p.convert_gaussians_to_pc(sc["xyz"], sc["scales"], sc["rots"], sc["colours"].clone() * 255,
-                                        sc["opacities"], sc["shs"], None, None, None, st)
-    return pc
-
-
 def _scene(name, rng):
-    u = lambda n, lo=0.0, hi=1.0: rng.uniform(lo, hi, (n, 3)).astype(np.float32)
+    u = lambda n: clouds.uniform(n, rng)
     if name == "sampled":
-        return _sampled_cloud(60_000, 200_000, seed=71).points.cpu().numpy()
+        from g2pc import synth
+        return synth.sampled_cloud(60_000, 200_000, 71, DEV).points.cpu().numpy()
     if name == "cube":
         return u(100_000)
     if name == "plane":
-        p = u(100_000, -2.0, 2.0)
-        p[:, 2] = np.float32(0.5) + rng.normal(0, 1e-6, p.shape[0]).astype(np.float32)
-        return p
+        return clouds.plane(100_000, rng, -2.0, 2.0, 0.5, jitter=1e-6)
     if name == "dense_sparse":
-        return np.concatenate([np.float32(0.3) + u(50_000, 0.0, 1e-4), u(5_000)])
+        return np.concatenate([clouds.clusters(rng, [0.3], [50_000], 1e-4), u(5_000)])
     if name == "isolated":
         return np.concatenate([u(20_000), np.float32([[1e3, 1e3, 1e3], [-1e3, 0, 0], [0, 1e3, -1e3], [2e3, 2e3, 2e3]])])
     if name == "far_clusters":
-        centres = np.float32([[1e4, 1e4, 1e4], [-1e4, 1e4, -1e4], [1e4, -1e4, 0], [-1e4, -1e4, -1e4]])
-        return np.concatenate([c + u(5_000, 0.0, 1e-3) for c in centres]).astype(np.float32)
+        return clouds.clusters(rng, clouds.FAR, [5_000] * 4, 1e-3)
     if name == "dup_runs":
-        parts = [u(3_000)]
-        for r in (18, 19, 20, 21, 30, 31, 32, 33, 40):
-            parts += [np.repeat(u(1), r, 0), u(7)]
-        p = np.concatenate(parts)
-        return p[rng.permutation(p.shape[0])]
+        return clouds.dup_runs(3_000, rng, (18, 19, 20, 21, 30, 31, 32, 33, 40), 7)
     if name == "lattice":  # every point on an octree cell boundary
-        g = np.arange(32, dtype=np.float32)
-        return np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3)
+        return clouds.lattice(32)
     if name.startswith("small"):
         return u(int(name[5:]))
     raise KeyError(name)
@@ -82,11 +60,6 @@ def _avg(p, k):
     avg, status = outliers.mean_distances(xyz, k)
     assert int(status.item()) == 0
     return avg.cpu().numpy()
-
-
-def _same(a, b):
-    """Bit-for-bit equality as a plain bool (keeps pytest from diffing megabytes of bytes on a failure)."""
-    return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
 
 
 def _ulps(a, b):
@@ -147,10 +120,10 @@ def test_output_rows(lib):
     _, keep_o, _ = f64ref_outliers.statistical_outliers(p, 20, 3.0)
     keep = dbg["keep"].cpu().numpy().astype(bool)
     assert np.array_equal(keep, keep_o) and not keep[20_000:].all()
-    assert pts.dtype == torch.float32 and _same(pts.cpu().numpy(), p[keep])
+    assert pts.dtype == torch.float32 and same(pts.cpu().numpy(), p[keep])
     want_c = np.clip(cols.cpu().numpy(), 0, 255).astype(np.int32)[keep]
     assert c.dtype == torch.int32 and np.array_equal(c.cpu().numpy(), want_c)
-    assert _same(nn.cpu().numpy(), nrm.cpu().numpy()[keep])
+    assert same(nn.cpu().numpy(), nrm.cpu().numpy()[keep])
     pts2, c2, nn2 = outliers.remove_statistical_outliers(xyz, None, None, 20, 3.0)
     assert c2 is None and nn2 is None and torch.equal(pts2, pts)
     import mesh_handler
@@ -172,28 +145,24 @@ def test_scale_c3_cloud(lib):
     """A 10 M-point cloud sampled like C3: avg on a 20 k subset bit-identical to the oracle over all 10 M points, the
     statistics recomputed on the host from the kernel's avg, the keep rule, and three bit-identical runs (the last one
     on poisoned allocator memory)."""
-    pc = _sampled_cloud(3_000_000, 10_000_000, seed=1236)
+    from g2pc import synth
+    pc = synth.sampled_cloud(3_000_000, 10_000_000, 1236, DEV)
     host = [t.cpu() for t in (pc.points, pc.colours, pc.normals)]
+    del pc
     n = host[0].shape[0]
     assert n > 9_000_000
-    runs = [_clean_to_host(pc.points, pc.colours, pc.normals) for _ in range(2)]
-    del pc
-    poison_allocator(0x5A, large_bytes=1 << 30)
-    runs.append(_clean_to_host(*[t.to(DEV) for t in host]))
-    for r in runs[1:]:
-        for a, b in zip(runs[0], r):
-            assert _same(a, b)
-    pts, _, _, avg, s, keep = runs[0]
+    pts, _, _, avg, s, keep = assert_repeatable(lambda: _clean_to_host(*[t.to(DEV) for t in host]), byte=0x5A,
+                                                large_bytes=1 << 30)
     keep = keep.astype(bool)
     p = host[0].numpy()
     sub = np.random.default_rng(4).choice(n, 20_000, replace=False)
     want = f64ref_outliers.knn_mean_distances(p, 20, query=sub)
-    assert _same(avg[sub], want), f"{int((avg[sub] != want).sum())} of 20000 differ"
+    assert same(avg[sub], want), f"{int((avg[sub] != want).sum())} of 20000 differ"
     mean, std, thr = f64ref_outliers.sor_statistics(avg, 10.0)
     for got, w in zip(s, (mean, std, thr)):
         assert abs(got - w) <= 1e-12 * abs(w), (s, (mean, std, thr))
     _check_keep(keep, avg, thr, "10M")
-    assert _same(pts, p[keep])
+    assert same(pts, p[keep])
 
 
 @pytest.mark.parametrize("case", ["copies", "tiny_cube"])
@@ -221,11 +190,11 @@ def test_bounded_work(lib, case):
         assert (avg[:1_000_000] == 0).all() and not dbg["keep"].cpu().numpy()[:1_000_000].any()
         # the k nearest of a scattered point hold at most k copies: the oracle over 20 copies + the sparse points
         want = f64ref_outliers.knn_mean_distances(np.concatenate([dense[:20], sparse]), 20)[20:]
-        assert _same(avg[1_000_000:], want)
+        assert same(avg[1_000_000:], want)
     else:
         sub = np.concatenate([np.arange(0, 1_000_000, 997), np.arange(1_000_000, p.shape[0])])
         want = f64ref_outliers.knn_mean_distances(p, 20, query=sub)
-        assert _same(avg[sub], want)
+        assert same(avg[sub], want)
 
 
 def test_cli_clean(lib, tmp_path):
@@ -252,7 +221,7 @@ def test_cli_clean(lib, tmp_path):
         avg, keep, (_, _, thr) = f64ref_outliers.statistical_outliers(p, 20, 10.0)
         assert int((np.abs(avg - thr) <= BAND * thr).sum()) == 0
         assert 0 < int(keep.sum()) < p.shape[0] or keep.all()
-        assert _same(c, v[keep])
+        assert same(c, v[keep])
     with open(outs["clean_nn"], "rb") as f:
         head = f.read(400).split(b"end_header")[0]
     assert b"nx" not in head and b"red" in head

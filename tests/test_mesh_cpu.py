@@ -5,19 +5,20 @@ import numpy as np
 import pytest
 import torch
 
+import clouds
 import f64ref_mesh as fm
 
 R = 32
 
 
-def _lattice(R):
-    g = np.arange(R) + 0.5
-    z, y, x = np.meshgrid(g, g, g, indexing="ij")
-    return x.reshape(-1), y.reshape(-1), z.reshape(-1)
+def _cell_centres(R):
+    """x, y, z of the centres of the R^3 unit cells in chi's order (x fastest), float64."""
+    z, y, x = (clouds.lattice(R).astype(np.float64) + 0.5).T
+    return x, y, z
 
 
 def _sphere_sdf(R, c, r):
-    x, y, z = _lattice(R)
+    x, y, z = _cell_centres(R)
     return np.sqrt((x - c[0]) ** 2 + (y - c[1]) ** 2 + (z - c[2]) ** 2) - r
 
 
@@ -39,7 +40,7 @@ def test_sphere_closed_genus0_volume():
 
 
 def test_torus_genus1():
-    x, y, z = _lattice(R)
+    x, y, z = _cell_centres(R)
     q = np.sqrt((x - 16) ** 2 + (y - 16) ** 2) - 9.0
     vkey, vt, vpos, faces = fm.marching_tetrahedra(np.sqrt(q ** 2 + (z - 16) ** 2) - 3.5, R, 0.0)
     _check_closed(faces)

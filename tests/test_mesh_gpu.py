@@ -12,8 +12,10 @@ import numpy as np
 import pytest
 import torch
 
+import clouds
 import f64ref_mesh as fm
-from sanitizer_harness import check_target, poison_allocator
+from sanitizer_harness import assert_repeatable, check_target
+from util import gpu, same
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -22,30 +24,15 @@ TARGET = os.path.join(HERE, "mesh_sanitizer_target.py")
 CHI_TOL = 2e-5  # |chi_gpu - chi_direct| <= CHI_TOL * range(chi_direct), both mean-free: measured <= 3.4e-6 (DESIGN.md §2)
 
 
-def _sphere(n, rng, r=1.0, centre=(0.0, 0.0, 0.0), noise=0.0):
-    d = rng.normal(size=(n, 3))
-    d /= np.linalg.norm(d, axis=1, keepdims=True)
-    p = np.asarray(centre) + r * d + noise * rng.normal(size=(n, 3))
-    return p.astype(np.float32), d.astype(np.float32)
-
-
-def _torus(n, rng, R0=1.0, r0=0.35):
-    u, v = rng.uniform(0, 2 * np.pi, n), rng.uniform(0, 2 * np.pi, n)
-    c = np.stack([np.cos(u), np.sin(u), np.zeros(n)], 1)
-    nrm = np.cos(v)[:, None] * c + np.sin(v)[:, None] * np.array([0, 0, 1.0])
-    return (R0 * c + r0 * nrm).astype(np.float32), nrm.astype(np.float32)
-
-
 def _cloud(name, rng, depth):
     if name == "sphere":
-        return _sphere(20_000, rng)
+        return clouds.sphere(20_000, rng)
     if name == "two_spheres":
-        a, na = _sphere(10_000, rng, 0.6, (-1, 0, 0))
-        b, nb = _sphere(10_000, rng, 0.5, (1, 0.2, 0))
+        a, na = clouds.sphere(10_000, rng, 0.6, (-1, 0, 0))
+        b, nb = clouds.sphere(10_000, rng, 0.5, (1, 0.2, 0))
         return np.r_[a, b], np.r_[na, nb]
     if name == "plane":
-        p = rng.uniform(-1, 1, (20_000, 3)).astype(np.float32)
-        p[:, 2] = 0.1
+        p = clouds.plane(20_000, rng, -1.0, 1.0, 0.1)
         return p, np.tile(np.float32([0, 0, 1]), (p.shape[0], 1))
     if name == "node_planes":  # bbox [0, 1]^3: points on the (float32-rounded) node planes, f = 0 and f = 1
         R = 1 << depth
@@ -67,21 +54,13 @@ def _cloud(name, rng, depth):
         n = np.r_[np.repeat(np.float32([[0.0, 0.6, 0.8]]), 1_000_000, 0), rng.normal(size=(100, 3))]
         return p.astype(np.float32), n.astype(np.float32)
     if name == "bad_normals":
-        p, n = _sphere(5_000, rng)
+        p, n = clouds.sphere(5_000, rng)
         n = n.astype(np.float64) * rng.uniform(1e-3, 1e3, (n.shape[0], 1))
         n[:50] = 0.0
         n[50:60, 1] = np.nan
         n[60:70, 2] = np.inf
         return p, n
     raise KeyError(name)
-
-
-def _t(a, dtype=None):
-    return torch.from_numpy(np.ascontiguousarray(a if dtype is None else a.astype(dtype))).to(DEV)
-
-
-def _same(a, b):
-    return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
 
 
 @pytest.mark.parametrize("name", ["sphere", "two_spheres", "plane", "node_planes", "cube_faces", "copies",
@@ -91,11 +70,11 @@ def test_splat_bit_identical(lib, name):
     rng = np.random.default_rng(len(name))
     for depth in range(2, 8):
         p, n = _cloud(name, rng, depth)
-        frame, B, cell, status = mesh.splat(_t(p), _t(n), depth)
+        frame, B, cell, status = mesh.splat(gpu(p), gpu(n), depth)
         B_o, cell_o, skipped_o, fr = fm.splat(p, n, depth)
         f = frame.cpu().numpy()
         assert f[0:3].tobytes() == fr["origin"].tobytes() and f[3] == fr["h"] and f[4] == fr["L"], (name, depth)
-        assert _same(B.cpu().numpy(), B_o), (name, depth)
+        assert same(B.cpu().numpy(), B_o), (name, depth)
         assert np.array_equal(cell.cpu().numpy().astype(np.int64), cell_o), (name, depth)
         st = status.cpu().numpy()
         assert st[0] == skipped_o and st[1] == 0, (name, depth, st)
@@ -109,8 +88,8 @@ def test_splat_bit_identical(lib, name):
 def _stages(p, n, depth, colours=None):
     """The mesher's stages one by one through the C ABI, keeping what each one produced."""
     from g2pc import mesh
-    pts, nrm = _t(p), _t(n)
-    col = _t(colours, np.int32) if colours is not None else None
+    pts, nrm = gpu(p), gpu(n)
+    col = gpu(colours, np.int32) if colours is not None else None
     frame, B, cell, status = mesh.splat(pts, nrm, depth)
     B_host = B.cpu().numpy()
     chi, cycles, ratio = mesh.solve(B, frame, depth)
@@ -137,7 +116,7 @@ def _fr(frame, depth):
 @pytest.mark.parametrize("depth", [4, 5, 6])
 def test_solve_against_direct(lib, depth):
     rng = np.random.default_rng(depth)
-    p, n = _sphere(20_000, rng)
+    p, n = clouds.sphere(20_000, rng)
     s = _stages(p, n, depth)
     fr = _fr(s["frame"], depth)
     b = fm.rhs(s["B"], fr)
@@ -152,8 +131,8 @@ def test_solve_against_direct(lib, depth):
 @pytest.mark.parametrize("depth", [2, 3, 7])
 def test_residual_ratio(lib, depth):
     from g2pc import mesh
-    p, n = _sphere(50_000, np.random.default_rng(7))
-    frame, B, cell, _ = mesh.splat(_t(p), _t(n), depth)
+    p, n = clouds.sphere(50_000, np.random.default_rng(7))
+    frame, B, cell, _ = mesh.splat(gpu(p), gpu(n), depth)
     chi, cycles, ratio = mesh.solve(B, frame, depth)
     b = fm.rhs(B.cpu().numpy(), _fr(frame.cpu().numpy(), depth))
     host = fm.residual_ratio(chi.cpu().numpy(), b, 1 << depth)
@@ -165,7 +144,7 @@ def test_residual_ratio(lib, depth):
 def test_extraction_against_restatement(lib, name, depth):
     rng = np.random.default_rng(11)
     if name == "torus":
-        p, n = _torus(60_000, rng)
+        p, n, _ = clouds.torus(60_000, rng)
     else:
         p, n = _cloud(name, rng, depth)
     colours = rng.integers(0, 256, p.shape)
@@ -178,19 +157,19 @@ def test_extraction_against_restatement(lib, name, depth):
     iso = s["iso"][1]
     vkey, vt, vpos, faces = fm.marching_tetrahedra(s["chi"], R, iso, fr["origin"], fr["h"])
     assert np.array_equal(s["vkey"], vkey)
-    assert _same(s["vt"], vt) and _same(s["vpos"], vpos)
+    assert same(s["vt"], vt) and same(s["vpos"], vpos)
     rot = lambda f: np.stack([np.roll(r, -int(np.argmin(r))) for r in f]) if len(f) else f
     assert np.array_equal(rot(s["faces"].astype(np.int64)), rot(faces))
     dens, vcol = fm.vertex_density_colour(p, colours, s["cell"], fr, vkey, vt)
-    assert _same(s["dens"], dens) and np.array_equal(s["vcol"], vcol)
+    assert same(s["dens"], dens) and np.array_equal(s["vcol"], vcol)
     d2, p2, c2, f2, keep, thr = fm.trim(dens, vpos, vcol, faces)
     assert np.array_equal(s["keep"], keep) and s["thr"] == thr
-    assert _same(s["tdens"], d2) and _same(s["tpos"], p2) and np.array_equal(s["tfaces"], f2)
+    assert same(s["tdens"], d2) and same(s["tpos"], p2) and np.array_equal(s["tfaces"], f2)
     sm = fm.smooth(p2, f2, 3)
     assert np.abs(s["spos"] - sm).max() <= 1e-12 * fr["L"]
     nr = fm.vertex_normals(s["spos"], f2)
     assert np.abs(s["normals"] - nr).max() <= 1e-6
-    assert _same(s["verts"], s["spos"].astype(np.float32))
+    assert same(s["verts"], s["spos"].astype(np.float32))
 
 
 def _closed_checks(vpos, faces, h, centre=None, radius=None):
@@ -203,24 +182,24 @@ def _closed_checks(vpos, faces, h, centre=None, radius=None):
 def test_end_to_end_shapes(lib):
     rng = np.random.default_rng(5)
     depth = 7
-    p, n = _sphere(200_000, rng, 1.0, (0.2, -0.1, 0.3))
+    p, n = clouds.sphere(200_000, rng, 1.0, (0.2, -0.1, 0.3))
     s = _stages(p, n, depth)
     _closed_checks(s["vpos"], s["faces"], s["frame"][3], np.array([0.2, -0.1, 0.3]), 1.0)
     assert fm.euler_characteristic(s["faces"]) == 2 and fm.signed_volume(s["vpos"], s["faces"]) > 0
     flipped = _stages(p, -n, depth)
     assert fm.signed_volume(flipped["vpos"], flipped["faces"]) < 0
-    p, n = _torus(200_000, rng)
+    p, n, _ = clouds.torus(200_000, rng)
     s = _stages(p, n, depth)
     _closed_checks(s["vpos"], s["faces"], s["frame"][3])
     assert fm.euler_characteristic(s["faces"]) == 0 and fm.components(s["faces"]) == 1
-    a, na = _sphere(100_000, rng, 0.6, (-1, 0, 0))
-    b, nb = _sphere(100_000, rng, 0.5, (1, 0.2, 0))
+    a, na = clouds.sphere(100_000, rng, 0.6, (-1, 0, 0))
+    b, nb = clouds.sphere(100_000, rng, 0.5, (1, 0.2, 0))
     s = _stages(np.r_[a, b], np.r_[na, nb], depth)
     _closed_checks(s["vpos"], s["faces"], s["frame"][3])
     assert fm.components(s["faces"]) == 2
     # the whole pipeline: every triangle after the trim indexes a kept vertex, the normals are unit or zero
     from g2pc import mesh
-    m = mesh.poisson_mesh(_t(p), _t(n), _t(rng.uniform(0, 255, p.shape).astype(np.float32)), depth=depth)
+    m = mesh.poisson_mesh(gpu(p), gpu(n), gpu(rng.uniform(0, 255, p.shape).astype(np.float32)), depth=depth)
     assert int(m.faces.max()) < m.vertices.shape[0] and m.colours.dtype == torch.uint8
     ln = torch.linalg.norm(m.normals.double(), dim=1)
     assert bool(((ln - 1).abs() < 1e-5).logical_or(ln == 0).all())
@@ -228,7 +207,7 @@ def test_end_to_end_shapes(lib):
 
 def _run_to_host(p, n, c):
     from g2pc import mesh
-    m, dbg = mesh.poisson_mesh(_t(p), _t(n), _t(c), depth=7, laplacian_iters=4, return_debug=True)
+    m, dbg = mesh.poisson_mesh(gpu(p), gpu(n), gpu(c), depth=7, laplacian_iters=4, return_debug=True)
     out = [t.cpu().numpy() for t in m]
     out += [dbg[k].cpu().numpy() for k in ("chi", "iso", "B", "keep", "threshold")] + [dbg["cycles"], dbg["ratio"]]
     return out
@@ -236,20 +215,15 @@ def _run_to_host(p, n, c):
 
 def test_determinism_on_poisoned_memory(lib):
     rng = np.random.default_rng(9)
-    p, n = _sphere(200_000, rng, noise=1e-3)
+    p, n = clouds.sphere(200_000, rng, noise=1e-3)
     c = rng.uniform(0, 255, p.shape).astype(np.float32)
-    runs = [_run_to_host(p, n, c) for _ in range(2)]
-    poison_allocator(0xFF, large_bytes=1 << 30, large_blocks=2)
-    runs.append(_run_to_host(p, n, c))
-    for r in runs[1:]:
-        for a, b in zip(runs[0], r):
-            assert (a == b) if not isinstance(a, np.ndarray) else _same(a, b)
+    assert_repeatable(lambda: _run_to_host(p, n, c), byte=0xFF, large_bytes=1 << 30, large_blocks=2)
 
 
 def test_refusals(lib):
     from g2pc import capi, mesh
-    p, n = _sphere(2_000, np.random.default_rng(1))
-    P, N = _t(p), _t(n)
+    p, n = clouds.sphere(2_000, np.random.default_rng(1))
+    P, N = gpu(p), gpu(n)
     for d in (1, 11):
         with pytest.raises(capi.G2pcError):
             mesh.poisson_mesh(P, N, depth=d)
@@ -277,8 +251,8 @@ def test_refusals(lib):
 def test_scale_10m_depth10(lib):
     from g2pc import mesh
     rng = np.random.default_rng(3)
-    p, n = _sphere(10_000_000, rng, noise=2e-3)
-    P, N = _t(p), _t(n)
+    p, n = clouds.sphere(10_000_000, rng, noise=2e-3)
+    P, N = gpu(p), gpu(n)
     del p, n
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()

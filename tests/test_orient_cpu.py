@@ -3,46 +3,22 @@ tree and shapes whose outward side is known; mesh_pc.py's --orient_normals flag.
 import numpy as np
 import pytest
 
+import clouds
 import f64ref_orient as fo
-
-
-def _sphere(n, rng, r=1.0, centre=(0.0, 0.0, 0.0), noise=1e-3):
-    d = rng.normal(size=(n, 3))
-    d /= np.linalg.norm(d, axis=1, keepdims=True)
-    return (np.asarray(centre) + r * d + noise * rng.normal(size=(n, 3))).astype(np.float32), d.astype(np.float32)
-
-
-def _torus(n, rng, R0=1.0, r0=0.35):
-    u, v = rng.uniform(0, 2 * np.pi, n), rng.uniform(0, 2 * np.pi, n)
-    c = np.stack([np.cos(u), np.sin(u), np.zeros(n)], 1)
-    nrm = np.cos(v)[:, None] * c + np.sin(v)[:, None] * np.array([0, 0, 1.0])
-    return (R0 * c + r0 * nrm).astype(np.float32), nrm.astype(np.float32), (R0 * c)
 
 
 def _negate_some(n, rng):
     return np.where(rng.random(n.shape[0]) < 0.5, -1.0, 1.0).astype(n.dtype)[:, None] * n
 
 
-def _lattice(m):
-    g = np.arange(m, dtype=np.float32)
-    return np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3)
-
-
-def _dup_runs(rng, k):
-    parts = [rng.random((200, 3))]
-    for r in (k - 1, k, k + 1, k + 2, 2 * k):
-        parts += [np.repeat(rng.random((1, 3)), r, 0), rng.random((3, 3))]
-    p = np.concatenate(parts).astype(np.float32)
-    return p[rng.permutation(p.shape[0])]
-
-
 @pytest.mark.parametrize("k", [1, 3, 10, 31])
 def test_knn_ids_against_brute_force(k):
     rng = np.random.default_rng(k)
-    clouds = [rng.random((n, 3)).astype(np.float32) for n in (0, 1, 2, k, k + 1, 300)]
-    clouds += [_lattice(5), _lattice(4) * np.float32(0.5), _dup_runs(rng, k), np.zeros((40, 3), np.float32),
-               np.repeat(np.float32([[1.0, 2.0, 3.0]]), k + 1, 0)]
-    for p in clouds:
+    cases = [rng.random((n, 3)).astype(np.float32) for n in (0, 1, 2, k, k + 1, 300)]
+    cases += [clouds.lattice(5), clouds.lattice(4) * np.float32(0.5),
+              clouds.dup_runs(200, rng, (k - 1, k, k + 1, k + 2, 2 * k), 3), np.zeros((40, 3), np.float32),
+              np.repeat(np.float32([[1.0, 2.0, 3.0]]), k + 1, 0)]
+    for p in cases:
         ids, d2 = fo.knn_ids(p, k)
         bi, bd = fo.knn_ids_brute(p, k)
         assert ids.shape == (p.shape[0], k) and np.array_equal(ids, bi) and np.array_equal(d2, bd), p.shape
@@ -52,7 +28,7 @@ def test_knn_ids_against_brute_force(k):
 
 
 def test_ties_go_to_the_smaller_index():
-    p = _lattice(3)  # the centre (13) has 6 neighbours at d2 = 1, 12 at 2, 8 at 3
+    p = clouds.lattice(3)  # the centre (13) has 6 neighbours at d2 = 1, 12 at 2, 8 at 3
     ids, d2 = fo.knn_ids(p, 10)
     c = ids[13]
     assert list(c[:6]) == [4, 10, 12, 14, 16, 22] and (d2[13, :6] == 1).all()
@@ -66,7 +42,7 @@ def test_mst_weight_matches_scipy():
     from scipy.sparse import coo_matrix
     from scipy.sparse.csgraph import minimum_spanning_tree
     rng = np.random.default_rng(2)
-    for p, n in (_sphere(2000, rng), _torus(3000, rng)[:2]):
+    for p, n in (clouds.sphere(2000, rng, noise=1e-3), clouds.torus(3000, rng)[:2]):
         n = _negate_some(n, rng)
         _, info = fo.orient(p, n, k=10)
         e, w, mst = info["edges"], info["weights"].astype(np.float64), info["mst"]
@@ -85,18 +61,18 @@ def _outward(out, p, centres):
 
 def test_sphere_and_torus_point_outward():
     rng = np.random.default_rng(4)
-    p, n = _sphere(3000, rng, 1.0, (0.3, -0.2, 0.1))
+    p, n = clouds.sphere(3000, rng, 1.0, (0.3, -0.2, 0.1), noise=1e-3)
     out, info = fo.orient(p, _negate_some(n, rng), k=10)
     assert info["components"] == 1 and (_outward(out, p, np.float64([0.3, -0.2, 0.1])) > 0).all()
-    p, n, ring = _torus(6000, rng)
+    p, n, ring = clouds.torus(6000, rng)
     out, info = fo.orient(p, _negate_some(n, rng), k=10)
     assert info["components"] == 1 and (_outward(out, p, ring) > 0).all()
 
 
 def test_two_far_spheres_are_two_components():
     rng = np.random.default_rng(6)
-    a, na = _sphere(1500, rng, 0.6, (-50, 0, 0))
-    b, nb = _sphere(1500, rng, 0.5, (50, 0.2, 0))
+    a, na = clouds.sphere(1500, rng, 0.6, (-50, 0, 0), noise=1e-3)
+    b, nb = clouds.sphere(1500, rng, 0.5, (50, 0.2, 0), noise=1e-3)
     p, n = np.r_[a, b], _negate_some(np.r_[na, nb], rng)
     out, info = fo.orient(p, n, k=10)
     assert info["components"] == 2
@@ -107,7 +83,7 @@ def test_two_far_spheres_are_two_components():
 
 def test_unusable_rows_and_magnitudes():
     rng = np.random.default_rng(8)
-    p, n = _sphere(500, rng)
+    p, n = clouds.sphere(500, rng, noise=1e-3)
     n = n.astype(np.float64) * rng.uniform(1e-3, 1e3, (500, 1))
     n[:5] = 0.0
     n[5:8, 1] = np.nan

@@ -11,9 +11,11 @@ import numpy as np
 import pytest
 import torch
 
+import clouds
 import f64ref_mesh as fm
 import f64ref_orient as fo
-from sanitizer_harness import check_target, poison_allocator
+from sanitizer_harness import assert_repeatable, check_target
+from util import gpu, same
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -22,40 +24,27 @@ TARGET = os.path.join(HERE, "orient_sanitizer_target.py")
 K_MAX = 31
 
 
-def _sphere(n, rng, r=1.0, centre=(0.0, 0.0, 0.0), noise=1e-3):
-    d = rng.normal(size=(n, 3))
-    d /= np.linalg.norm(d, axis=1, keepdims=True)
-    return (np.asarray(centre) + r * d + noise * rng.normal(size=(n, 3))).astype(np.float32), d.astype(np.float32)
-
-
 def _cloud(name, rng):
     """(points float32, normals float32 with random signs)"""
-    u = lambda n, lo=0.0, hi=1.0: rng.uniform(lo, hi, (n, 3)).astype(np.float32)
+    u = lambda n, lo=0.0, hi=1.0: clouds.uniform(n, rng, lo, hi)
     if name == "sphere_floaters":
-        p, n = _sphere(15_000, rng)
+        p, n = clouds.sphere(15_000, rng, noise=1e-3)
         p = np.r_[p, u(300, -3.0, 3.0)]
         n = np.r_[n, rng.normal(size=(300, 3)).astype(np.float32)]
     elif name == "plane":
-        p = u(12_000, -2.0, 2.0)
-        p[:, 2] = np.float32(0.5)
+        p = clouds.plane(12_000, rng, -2.0, 2.0, 0.5)
         n = np.tile(np.float32([0, 0, 1]), (p.shape[0], 1)) + u(p.shape[0], -0.1, 0.1)
     elif name == "lattice":  # ties at every slot
-        g = np.arange(20, dtype=np.float32)
-        p = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3)
+        p = clouds.lattice(20)
         n = rng.normal(size=p.shape).astype(np.float32)
     elif name == "clusters":  # 1e-4 clusters beside sparse points
-        p = np.concatenate([np.float32(0.3) + u(8_000, 0.0, 1e-4), np.float32(-0.4) + u(4_000, 0.0, 1e-4), u(2_000)])
+        p = np.concatenate([clouds.clusters(rng, [0.3, -0.4], [8_000, 4_000], 1e-4), u(2_000)])
         n = rng.normal(size=p.shape).astype(np.float32)
     elif name == "dup_runs":  # runs of exact copies around k
-        parts = [u(3_000)]
-        for r in (9, 10, 11, 12, 30, 31, 32, 33, 100):
-            parts += [np.repeat(u(1), r, 0), u(5)]
-        p = np.concatenate(parts)
-        p = p[rng.permutation(p.shape[0])]
+        p = clouds.dup_runs(3_000, rng, (9, 10, 11, 12, 30, 31, 32, 33, 100), 5)
         n = rng.normal(size=p.shape).astype(np.float32)
     elif name == "far":  # +-1e4 coordinates
-        p = np.concatenate([c + u(3_000, 0.0, 1.0) for c in np.float32([[1e4, 1e4, 1e4], [-1e4, 1e4, -1e4],
-                                                                          [1e4, -1e4, 0]])])
+        p = clouds.clusters(rng, clouds.FAR[:3], [3_000] * 3, 1.0)
         n = rng.normal(size=p.shape).astype(np.float32)
     elif name.startswith("small"):
         p = u(int(name[5:]))
@@ -70,35 +59,27 @@ CLOUDS = ["sphere_floaters", "plane", "lattice", "clusters", "dup_runs", "far", 
           "small11", "small31", "small32"]
 
 
-def _t(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(DEV)
-
-
-def _same(a, b):
-    return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
-
-
 @pytest.mark.parametrize("k", [1, 10, K_MAX])
 @pytest.mark.parametrize("name", CLOUDS)
 def test_knn_ids_bit_identical(lib, name, k):
     from g2pc import orient
     p, _ = _cloud(name, np.random.default_rng(zlib.crc32(name.encode())))
-    ids, d2, status = orient.knn_ids(_t(p), k)
+    ids, d2, status = orient.knn_ids(gpu(p), k)
     want_i, want_d = fo.knn_ids(p, k)
     got_i, got_d = ids.cpu().numpy(), d2.cpu().numpy()
     bad = np.nonzero((got_i != want_i).any(1))[0]
     if bad.size:
         print(f"[{name} k={k}] {bad.size} rows differ; first {bad[:3]}: got {got_i[bad[:3]]} want {want_i[bad[:3]]}")
-    assert int(status.item()) == 0 and np.array_equal(got_i, want_i) and _same(got_d, want_d)
+    assert int(status.item()) == 0 and np.array_equal(got_i, want_i) and same(got_d, want_d)
 
 
 def _check_against_restatement(p, n, k, tag):
     from g2pc import orient
-    out, st, dbg = orient.orient_normals(_t(p), _t(n), k=k, return_debug=True)
+    out, st, dbg = orient.orient_normals(gpu(p), gpu(n), k=k, return_debug=True)
     want, info = fo.orient(p, n, k=k)
     got = {key: v.cpu().numpy() for key, v in dbg.items()}
     assert np.array_equal(got["rows"], info["rows"]), tag
-    assert np.array_equal(got["ids"], info["ids"]) and _same(got["d2"], info["d2"]), tag
+    assert np.array_equal(got["ids"], info["ids"]) and same(got["d2"], info["d2"]), tag
     assert np.array_equal(got["edges"], info["edges"].reshape(-1, 2)), tag
     assert np.array_equal(got["mst"], info["mst"]), tag
     assert np.array_equal(got["seed"].astype(np.int64), info["seed"]), tag
@@ -106,7 +87,7 @@ def _check_against_restatement(p, n, k, tag):
     assert (st.components, st.flipped, st.skipped) == (info["components"], int(info["flip"].sum()), info["skipped"]), \
         (tag, st, info["components"], int(info["flip"].sum()), info["skipped"])
     o = out.cpu().numpy()
-    assert _same(o, want), tag
+    assert same(o, want), tag
     print(f"[{tag}] {p.shape[0]} points: {st.components} component(s), {st.flipped} flipped, {st.skipped} skipped, "
           f"{st.rounds} rounds")
     return o
@@ -127,7 +108,7 @@ def test_orientation_other_k(lib, k):
 
 def test_unusable_rows_and_float64(lib):
     rng = np.random.default_rng(21)
-    p, n = _sphere(8_000, rng)
+    p, n = clouds.sphere(8_000, rng, noise=1e-3)
     n = n.astype(np.float64) * rng.uniform(1e-3, 1e3, (n.shape[0], 1))
     n *= np.where(rng.random(n.shape[0]) < 0.5, -1.0, 1.0)[:, None]
     n[:40] = 0.0
@@ -135,7 +116,7 @@ def test_unusable_rows_and_float64(lib):
     n[50:60, 2] = -np.inf
     p[60, 0] = np.inf
     o = _check_against_restatement(p, n, 10, "unusable f64")
-    assert o.dtype == np.float64 and _same(o[:61], n[:61])  # untouched rows
+    assert o.dtype == np.float64 and same(o[:61], n[:61])  # untouched rows
     assert (np.abs(o) == np.abs(n))[61:].all()
     o32 = _check_against_restatement(p, n.astype(np.float32), 10, "unusable f32")
     assert o32.dtype == np.float32
@@ -143,26 +124,21 @@ def test_unusable_rows_and_float64(lib):
 
 def _run_to_host(p, n):
     from g2pc import orient
-    out, st, dbg = orient.orient_normals(_t(p), _t(n), return_debug=True)
+    out, st, dbg = orient.orient_normals(gpu(p), gpu(n), return_debug=True)
     return [out.cpu().numpy()] + [dbg[k].cpu().numpy() for k in sorted(dbg)] + [np.array(st)]
 
 
 def test_determinism_on_poisoned_memory(lib):
     rng = np.random.default_rng(9)
-    p, n = _sphere(200_000, rng, noise=1e-3)
+    p, n = clouds.sphere(200_000, rng, noise=1e-3)
     n *= np.where(rng.random(n.shape[0]) < 0.5, -1.0, 1.0).astype(np.float32)[:, None]
-    runs = [_run_to_host(p, n) for _ in range(2)]
-    poison_allocator(0xFF, large_bytes=1 << 30, large_blocks=2)
-    runs.append(_run_to_host(p, n))
-    for r in runs[1:]:
-        for a, b in zip(runs[0], r):
-            assert _same(a, b)
+    assert_repeatable(lambda: _run_to_host(p, n), byte=0xFF, large_bytes=1 << 30, large_blocks=2)
 
 
 def test_refusals(lib):
     from g2pc import capi, orient
-    p, n = _sphere(500, np.random.default_rng(1))
-    P, N = _t(p), _t(n)
+    p, n = clouds.sphere(500, np.random.default_rng(1), noise=1e-3)
+    P, N = gpu(p), gpu(n)
     with pytest.raises(capi.G2pcError):
         orient.orient_normals(P.cpu(), N.cpu())
     with pytest.raises(capi.G2pcError):
@@ -285,28 +261,12 @@ def test_mesh_pc_orient_end_to_end(lib, tmp_path, kind):
     assert closed and chi == (2 if kind == "sphere" else 0) and vol0 > 0
 
 
-def _sampled_cloud(n_gaussians, num_points, seed):
-    import gauss_to_pc as g2p
-    from g2pc import sampler, synth
-    sc = {k: v.to(DEV) for k, v in synth.make_scene(n_gaussians, seed=seed).items()}
-    st = g2p.GaussPointCloudSettings(
-        renderer_type="python", num_points=num_points, prioritise_visible_gaussians=True, mahalanobis_distance_std=2.0,
-        camera_skip_rate=0, render_colours=False, min_opacity=0.0, bounding_box_min=None, bounding_box_max=None,
-        calculate_normals=True, cull_large_percentage=0.0, remove_unrendered_gaussians=True, colour_resolution=None,
-        max_sh_degree=3, exact_num_points=False, visibility_threshold=0.05, surface_distance_std=None,
-        generate_mesh=False, quiet=True, device=DEV)
-    sampler.reset_call_counter(0)
-    pc, _ = g2p.convert_gaussians_to_pc(sc["xyz"], sc["scales"], sc["rots"], sc["colours"].clone() * 255,
-                                        sc["opacities"], sc["shs"], None, None, None, st)
-    return pc
-
-
 def test_scale_c3_cloud(lib):
     """A 10 M-point cloud sampled like C3, k = 10: the neighbour lists of a 20 k subset bit-identical to the restatement
     over all 10 M points; every spanning-forest edge joins two output normals with a non-negative dot product (the
     parity of the whole forest); time and peak memory printed."""
-    from g2pc import orient
-    pc = _sampled_cloud(3_000_000, 10_000_000, seed=1236)
+    from g2pc import orient, synth
+    pc = synth.sampled_cloud(3_000_000, 10_000_000, 1236, DEV)
     pts, nrm = pc.points, pc.normals
     del pc
     orient.orient_normals(pts[:1000].contiguous(), nrm[:1000].contiguous())  # warm-up
@@ -331,4 +291,4 @@ def test_scale_c3_cloud(lib):
     sub = np.random.default_rng(4).choice(m, 20_000, replace=False)
     want_i, want_d = fo.knn_ids(up, 10, query=sub)
     assert np.array_equal(dbg["ids"][torch.from_numpy(sub).to(DEV)].cpu().numpy(), want_i)
-    assert _same(dbg["d2"][torch.from_numpy(sub).to(DEV)].cpu().numpy(), want_d)
+    assert same(dbg["d2"][torch.from_numpy(sub).to(DEV)].cpu().numpy(), want_d)

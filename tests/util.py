@@ -7,6 +7,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
+def gpu(a, dtype=None):
+    """A numpy array (cast to dtype when given) as a contiguous tensor on cuda:0."""
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a if dtype is None else a.astype(dtype))).to("cuda:0")
+
+
+def same(a, b):
+    """Bit-for-bit equality of two arrays as a plain bool (keeps pytest from diffing megabytes of bytes on a failure)."""
+    return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
+
+
 def scene_to(sc, device):
     return {k: v.to(device) for k, v in sc.items()}
 
