@@ -9,6 +9,7 @@ residual once per cycle, the vertex / triangle counts before and after the trim.
 """
 import collections
 import math
+import warnings
 
 import numpy as np
 import torch
@@ -183,6 +184,9 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     with capi.phase(timings, "solve"):
         chi, cycles, ratio = solve(B, frame, depth)
         iso = iso_value(pts, cell, frame, depth, chi)
+    if ratio > TOLERANCE:
+        warnings.warn(f"the Poisson solve stopped after {cycles} V-cycles at |r| / |b| = {ratio:.2e}, above the "
+                      f"{TOLERANCE:g} target: the surface may be displaced", RuntimeWarning, stacklevel=2)
     debug = {}
     if return_debug:
         debug = {"B": B.clone(), "frame": frame, "cycles": cycles, "ratio": ratio, "skipped": skipped}

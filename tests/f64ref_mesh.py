@@ -54,8 +54,9 @@ def usable_normals(normals):
     return ok, nh
 
 
-def splat(points, normals, depth):
-    """(B (R^3,) int64, cell (n,) int64 dual-cell index or CELL_NONE, skipped count, frame)."""
+def _splat_terms(points, normals, depth):
+    """(cell (n,) int64 dual-cell index or CELL_NONE, skipped count, frame, [(nodes, q)]): every integer term the splat
+    adds to B, in (corner, axis, side) order."""
     fr = frame(points, depth)
     R = fr["R"]
     p = np.asarray(points, np.float32)
@@ -63,10 +64,10 @@ def splat(points, normals, depth):
     ok, nh = usable_normals(normals)
     skipped = int((finite & ~ok).sum())
     use = finite & ok & (fr["h"] > 0)
-    B = np.zeros(R ** 3, np.int64)
     cell = np.full(p.shape[0], CELL_NONE, np.int64)
+    terms = []
     if not use.any():
-        return B, cell, skipped, fr
+        return cell, skipped, fr, terms
     idx = np.nonzero(use)[0]
     i0, f = point_cells(p[idx], fr)
     cell[idx] = (i0[:, 2] * (R - 1) + i0[:, 1]) * (R - 1) + i0[:, 0]
@@ -78,9 +79,37 @@ def splat(points, normals, depth):
         for a in range(3):
             q = np.rint((w[:, o] * nh[idx, a]) * 4294967296.0).astype(np.int64)
             lo, hi = c[:, a] > 0, c[:, a] < R - 1
-            np.add.at(B, node[lo] - stride[a], q[lo])
-            np.add.at(B, node[hi] + stride[a], -q[hi])
+            terms.append((node[lo] - stride[a], q[lo]))
+            terms.append((node[hi] + stride[a], -q[hi]))
+    return cell, skipped, fr, terms
+
+
+def splat(points, normals, depth):
+    """(B (R^3,) int64, cell (n,) int64 dual-cell index or CELL_NONE, skipped count, frame)."""
+    cell, skipped, fr, terms = _splat_terms(points, normals, depth)
+    B = np.zeros(fr["R"] ** 3, np.int64)
+    for node, q in terms:
+        np.add.at(B, node, q)
     return B, cell, skipped, fr
+
+
+def splat_sparse(points, normals, depth):
+    """(nodes (k,) int64 ascending, values (k,) int64, cell, skipped, frame): the non-zero entries of splat's B without
+    the dense R^3 array.  B is an integer sum, so grouping its terms by node gives the same values in any order."""
+    cell, skipped, fr, terms = _splat_terms(points, normals, depth)
+    if not terms:
+        return np.zeros(0, np.int64), np.zeros(0, np.int64), cell, skipped, fr
+    node = np.concatenate([t[0] for t in terms])
+    q = np.concatenate([t[1] for t in terms])
+    del terms
+    order = np.argsort(node, kind="stable")
+    node, q = node[order], q[order]
+    del order
+    start = np.r_[0, np.nonzero(np.diff(node))[0] + 1]
+    vals = np.add.reduceat(q, start)
+    nodes = node[start]
+    nz = vals != 0
+    return nodes[nz], vals[nz], cell, skipped, fr
 
 
 # ---- solve and iso --------------------------------------------------------------------------------------------------
@@ -112,9 +141,62 @@ def solve_direct(b, R):
     return x - x.mean()
 
 
+def solve_dct(b, R):
+    """Exact mean-free chi of the Neumann system, computed in place in b's memory (b (R^3,) float64 is overwritten).
+    The orthonormal DCT-II along each axis diagonalises the 1-D operator with mirrored ghosts, eigenvalue
+    2 cos(pi k / R) - 2 for mode k, so the 3-D operator has the sum over the axes; the k = 0 mode (the null space, the
+    mean) is set to 0."""
+    import scipy.fft as sfft
+    x = b.reshape(R, R, R)
+    sfft.dctn(x, type=2, norm="ortho", overwrite_x=True, workers=-1)
+    lam = 2.0 * np.cos(np.pi * np.arange(R) / R) - 2.0
+    plane = lam[:, None] + lam[None, :]
+    for k in range(R):
+        x[k] /= plane + lam[k] if k else np.where(plane == 0.0, 1.0, plane)
+    x[0, 0, 0] = 0.0
+    sfft.idctn(x, type=2, norm="ortho", overwrite_x=True, workers=-1)
+    return b
+
+
 def residual_ratio(chi, b, R):
     r = b - neumann_laplacian(R) @ np.asarray(chi, np.float64)
     return float(np.linalg.norm(r) / np.linalg.norm(b))
+
+
+def residual_ratio_slabs(chi, b, R, slab=64):
+    """residual_ratio with a numpy stencil, `slab` z-layers at a time: no sparse matrix, and no temporary larger than
+    one slab."""
+    c = np.asarray(chi).reshape(R, R, R)
+    bb = np.asarray(b).reshape(R, R, R)
+    cnt_ij = np.full((R, R), 6.0)
+    cnt_ij[:, 0] -= 1
+    cnt_ij[:, -1] -= 1
+    cnt_ij[0, :] -= 1
+    cnt_ij[-1, :] -= 1
+    rr = bsq = 0.0
+    for k0 in range(0, R, slab):
+        k1 = min(k0 + slab, R)
+        x = c[k0:k1].astype(np.float64)
+        s = np.zeros_like(x)
+        s[:, :, 1:] += x[:, :, :-1]
+        s[:, :, :-1] += x[:, :, 1:]
+        s[:, 1:, :] += x[:, :-1, :]
+        s[:, :-1, :] += x[:, 1:, :]
+        s[1:] += x[:-1]
+        s[:-1] += x[1:]
+        cnt = np.repeat(cnt_ij[None], k1 - k0, 0)
+        if k0 > 0:
+            s[0] += c[k0 - 1]
+        else:
+            cnt[0] -= 1
+        if k1 < R:
+            s[-1] += c[k1]
+        else:
+            cnt[-1] -= 1
+        r = bb[k0:k1] - (s - cnt * x)
+        rr += float(np.vdot(r, r))
+        bsq += float(np.vdot(bb[k0:k1], bb[k0:k1]))
+    return float(np.sqrt(rr) / np.sqrt(bsq))
 
 
 def trilinear(points, fr, chi):
@@ -175,24 +257,49 @@ def tet_triangles(p, inside):
 _TABLE = [[tet_triangles(p, m) for m in range(256)] for p in range(6)]
 
 
-def marching_tetrahedra(chi, R, iso, origin=(0.0, 0.0, 0.0), h=1.0):
-    """(vkey (m,) int64 ascending, vt (m,), vpos (m,3), faces (t,3) int64) on the node lattice of chi (R^3, node
-    (k R + j) R + i); a node is inside iff chi < iso; node positions origin + (i + 1/2) h."""
-    c = np.asarray(chi).astype(np.float64).reshape(R, R, R)  # [k, j, i]
+def _slab(chi, R, k0, k1):
+    """(k0, k1, chi[k0 : k1 + 1] as float64 (z, y, x)): the layers the vertices of node layers [k0, k1) and the cubes
+    with lowest corner in [k0, k1) read."""
+    k0 = 0 if k0 is None else int(k0)
+    k1 = R if k1 is None else int(k1)
+    assert 0 <= k0 < k1 <= R
+    c = np.asarray(chi).reshape(R, R, R)[k0:min(k1 + 1, R)].astype(np.float64)
+    return k0, k1, c
+
+
+def crossed_edges(chi, R, iso, k0=None, k1=None):
+    """(vkey (m,) int64 ascending, vt (m,)) of the lattice edges crossed by the iso-surface whose first node lies in
+    z-layers [k0, k1) (default: all); a node is inside iff chi < iso."""
+    k0, k1, c = _slab(chi, R, k0, k1)
     inside = c < iso
+    nk = k1 - k0
     keys = []
     for d in range(1, 8):
         dx, dy, dz = d & 1, (d >> 1) & 1, d >> 2
-        crossed = inside[:R - dz, :R - dy, :R - dx] != inside[dz:, dy:, dx:]
+        top = min(nk, c.shape[0] - dz)
+        crossed = inside[:top, :R - dy, :R - dx] != inside[dz:top + dz, dy:, dx:]
         k, j, i = np.nonzero(crossed)
-        keys.append(((k * R + j) * R + i) * 8 + d)
+        keys.append((((k + k0) * R + j) * R + i) * 8 + d)
     vkey = np.sort(np.concatenate(keys)).astype(np.int64)
     node, d = vkey >> 3, vkey & 7
     flat = c.reshape(-1)
+    ii, jj, kk = node % R, (node // R) % R, node // (R * R) - k0
+    ib, jb, kb = ii + (d & 1), jj + ((d >> 1) & 1), kk + (d >> 2)
+    ca, cb = flat[(kk * R + jj) * R + ii], flat[(kb * R + jb) * R + ib]
+    return vkey, (iso - ca) / (cb - ca)
+
+
+def marching_tetrahedra(chi, R, iso, origin=(0.0, 0.0, 0.0), h=1.0, k0=None, k1=None):
+    """(vkey (m,) int64 ascending, vt (m,), vpos (m,3), faces (t,3) int64) on the node lattice of chi (R^3, node
+    (k R + j) R + i); a node is inside iff chi < iso; node positions origin + (i + 1/2) h.  With k0 / k1, one z-slab:
+    the vertices whose node lies in layers [k0, k1) and the triangles of the cubes whose lowest corner does, the faces
+    then as triples of vertex keys (global vertex indices need the whole grid)."""
+    slab = k0 is not None or k1 is not None
+    vkey, t = crossed_edges(chi, R, iso, k0, k1)
+    k0, k1, c = _slab(chi, R, k0, k1)
+    node, d = vkey >> 3, vkey & 7
     ii, jj, kk = node % R, (node // R) % R, node // (R * R)
     ib, jb, kb = ii + (d & 1), jj + ((d >> 1) & 1), kk + (d >> 2)
-    ca, cb = flat[node], flat[(kb * R + jb) * R + ib]
-    t = (iso - ca) / (cb - ca)
     origin = np.asarray(origin, np.float64)
     vpos = np.empty((vkey.size, 3))
     for a, (lo, hi) in enumerate(((ii, ib), (jj, jb), (kk, kb))):
@@ -200,13 +307,15 @@ def marching_tetrahedra(chi, R, iso, origin=(0.0, 0.0, 0.0), h=1.0):
         pb = origin[a] + (hi + 0.5) * h
         vpos[:, a] = pa + t * (pb - pa)
     # cubes: 8-bit inside mask per cube origin (k, j, i) <= R - 2
-    m = np.zeros((R - 1,) * 3, np.int64)
+    inside = c < iso
+    nc = min(k1, R - 1) - k0
+    m = np.zeros((max(nc, 0), R - 1, R - 1), np.uint8)
     for o in range(8):
         dx, dy, dz = o & 1, (o >> 1) & 1, o >> 2
-        m |= inside[dz:R - 1 + dz, dy:R - 1 + dy, dx:R - 1 + dx].astype(np.int64) << o
+        m |= inside[dz:nc + dz, dy:R - 1 + dy, dx:R - 1 + dx].astype(np.uint8) << o
     k, j, i = np.nonzero((m != 0) & (m != 255))
-    cube_node = (k * R + j) * R + i
     mask = m[k, j, i]
+    cube_node = ((k + k0) * R + j) * R + i
     rows = []  # (cube node, tetrahedron, triangle, 3 edge keys)
     for p in range(6):
         for case in np.unique(mask):
@@ -218,7 +327,10 @@ def marching_tetrahedra(chi, R, iso, origin=(0.0, 0.0, 0.0), h=1.0):
                     off = (lo & 1) + ((lo >> 1) & 1) * R + (lo >> 2) * R * R
                     ek.append((sel + off) * 8 + (hi ^ lo))
                 rows.append(np.stack([sel, np.full_like(sel, p), np.full_like(sel, ti)] + ek, 1))
-    if rows:
+    if rows and slab:
+        rows = np.concatenate(rows)
+        faces = rows[np.lexsort((rows[:, 2], rows[:, 1], rows[:, 0]))][:, 3:6]
+    elif rows:
         rows = np.concatenate(rows)
         rows = rows[np.lexsort((rows[:, 2], rows[:, 1], rows[:, 0]))]
         faces = np.searchsorted(vkey, rows[:, 3:6])
@@ -305,10 +417,13 @@ def trim(dens, vpos, vcol, faces):
 
 # ---- smoothing and normals ----------------------------------------------------------------------------------------
 def one_ring(faces, m):
+    """(u, v) of the distinct directed one-ring edges, sorted by (u, v): unique packed keys u << 32 | v (vertex indices
+    are below 2^31, so the key order is the pair order)."""
     f = np.asarray(faces, np.int64)
-    e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-    e = np.unique(np.concatenate([e, e[:, ::-1]]), axis=0)  # sorted by (u, v), distinct
-    return e[:, 0], e[:, 1]
+    a = np.concatenate([f[:, 0], f[:, 1], f[:, 2]])
+    b = np.concatenate([f[:, 1], f[:, 2], f[:, 0]])
+    e = np.unique(np.concatenate([a << 32 | b, b << 32 | a]))
+    return e >> 32, e & 0xFFFFFFFF
 
 
 def smooth(vpos, faces, iterations, lam=0.5):

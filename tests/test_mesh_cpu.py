@@ -7,6 +7,7 @@ import torch
 
 import clouds
 import f64ref_mesh as fm
+from util import same
 
 R = 32
 
@@ -174,3 +175,81 @@ def test_splat_restatement_conserves_and_skips():
     b = fm.rhs(B, fr)
     chi = fm.solve_direct(b, 16)
     assert fm.residual_ratio(chi, b, 16) < 1e-10 and abs(chi.mean()) < 1e-12 * np.abs(chi).max()
+
+
+@pytest.mark.parametrize("R", [4, 8, 16, 32, 64])
+def test_dct_solve_against_sparse_solve(R):
+    """The DCT solve against spsolve (R <= 32) and conjugate gradients to 1e-13 (R = 64), on a splatted sphere's b and
+    on white noise made mean-free."""
+    rng = np.random.default_rng(R)
+    p, n = clouds.sphere(4_000, rng, 0.8, (0.1, 0.0, -0.1))
+    B, _, _, fr = fm.splat(p, n, R.bit_length() - 1)
+    noise = rng.normal(size=R ** 3)
+    for b in (fm.rhs(B, fr), noise - noise.mean()):
+        x = fm.solve_direct(b, R)
+        y = fm.solve_dct(b.copy(), R)
+        assert np.abs(y - x).max() <= 1e-11 * (x.max() - x.min()), R
+        assert abs(y.mean()) <= 1e-13 * np.abs(y).max()
+        assert fm.residual_ratio(y, b, R) < 1e-12
+
+
+@pytest.mark.parametrize("name", ["sphere", "two_spheres", "plane", "node_planes", "cube_faces", "copies",
+                                  "bad_normals"])
+def test_sparse_splat_equals_dense(name):
+    from test_mesh_gpu import _cloud
+    rng = np.random.default_rng(len(name))
+    for depth in range(2, 7):
+        p, n = _cloud(name, rng, depth)
+        B, cell, skipped, fr = fm.splat(p, n, depth)
+        nodes, vals, cell_s, skipped_s, fr_s = fm.splat_sparse(p, n, depth)
+        nz = np.nonzero(B)[0]
+        assert np.array_equal(nodes, nz) and np.array_equal(vals, B[nz]), (name, depth)
+        assert np.array_equal(cell_s, cell) and skipped_s == skipped and fr_s["h"] == fr["h"], (name, depth)
+
+
+def _bumpy_field(R, rng):
+    """A sphere's signed distance plus smooth noise on an R^3 grid, float32, with nodes exactly at the iso 0."""
+    x, y, z = _cell_centres(R)
+    f = np.sqrt((x - R * 0.47) ** 2 + (y - R * 0.52) ** 2 + (z - R * 0.5) ** 2) - R * 0.37
+    f = f + 1.5 * np.sin(x * 0.41) * np.cos(y * 0.37 + z * 0.23)
+    f = f.astype(np.float32)
+    f[rng.choice(f.size, 200, replace=False)] = 0.0
+    return f
+
+
+def test_slab_extraction_matches_whole_grid():
+    """Slabs over partitions of k with edges at several offsets give, concatenated, the whole grid's vertices, and its
+    triangles as vertex-key triples."""
+    R = 64
+    rng = np.random.default_rng(6)
+    chi = _bumpy_field(R, rng)
+    origin, h = np.array([-1.0, 0.5, 2.0]), 0.03
+    vkey, vt, vpos, faces = fm.marching_tetrahedra(chi, R, 0.0, origin, h)
+    assert faces.shape[0] > 1000
+    for edges in ([0, 64], [0, 1, 2, 31, 32, 33, 63, 64], [0, 7, 20, 21, 50, 62, 64], list(range(0, 65, 16))):
+        parts = [fm.marching_tetrahedra(chi, R, 0.0, origin, h, k0, k1) for k0, k1 in zip(edges[:-1], edges[1:])]
+        assert np.array_equal(np.concatenate([q[0] for q in parts]), vkey), edges
+        assert same(np.concatenate([q[1] for q in parts]), vt) and same(np.concatenate([q[2] for q in parts]), vpos)
+        assert np.array_equal(np.concatenate([q[3] for q in parts]), vkey[faces]), edges
+        ek = [fm.crossed_edges(chi, R, 0.0, k0, k1) for k0, k1 in zip(edges[:-1], edges[1:])]
+        assert np.array_equal(np.concatenate([q[0] for q in ek]), vkey) and same(np.concatenate([q[1] for q in ek]), vt)
+
+
+def test_slab_residual_equals_sparse_residual():
+    rng = np.random.default_rng(8)
+    for R, slab in ((16, 3), (32, 32), (32, 7)):
+        b = rng.normal(size=R ** 3)
+        b -= b.mean()
+        chi = fm.solve_dct(b.copy(), R).astype(np.float32)
+        want = fm.residual_ratio(chi, b, R)
+        assert abs(fm.residual_ratio_slabs(chi, b, R, slab) - want) <= 1e-12 * want, (R, slab)
+
+
+def test_one_ring_packed_keys_sorted_and_distinct():
+    rng = np.random.default_rng(12)
+    f = rng.integers(0, 50, (300, 3))
+    f = np.r_[f, f[:20], f[:5, ::-1]]
+    u, v = fm.one_ring(f, 50)
+    e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
+    want = np.unique(np.concatenate([e, e[:, ::-1]]), axis=0)
+    assert np.array_equal(np.stack([u, v], 1), want)

@@ -24,28 +24,30 @@ TARGET = os.path.join(HERE, "mesh_sanitizer_target.py")
 CHI_TOL = 2e-5  # |chi_gpu - chi_direct| <= CHI_TOL * range(chi_direct), both mean-free: measured <= 3.4e-6 (DESIGN.md §2)
 
 
-def _cloud(name, rng, depth):
+def _cloud(name, rng, depth, n=20_000):
+    """Splat test cloud `name`; n is the size of the clouds that sample a surface (sphere, two spheres, plane, node
+    planes, box faces)."""
     if name == "sphere":
-        return clouds.sphere(20_000, rng)
+        return clouds.sphere(n, rng)
     if name == "two_spheres":
-        a, na = clouds.sphere(10_000, rng, 0.6, (-1, 0, 0))
-        b, nb = clouds.sphere(10_000, rng, 0.5, (1, 0.2, 0))
+        a, na = clouds.sphere(n // 2, rng, 0.6, (-1, 0, 0))
+        b, nb = clouds.sphere(n // 2, rng, 0.5, (1, 0.2, 0))
         return np.r_[a, b], np.r_[na, nb]
     if name == "plane":
-        p = clouds.plane(20_000, rng, -1.0, 1.0, 0.1)
+        p = clouds.plane(n, rng, -1.0, 1.0, 0.1)
         return p, np.tile(np.float32([0, 0, 1]), (p.shape[0], 1))
     if name == "node_planes":  # bbox [0, 1]^3: points on the (float32-rounded) node planes, f = 0 and f = 1
         R = 1 << depth
         h, o = 1.1 / R, 0.5 - 0.55
         g = o + (np.arange(R) + 0.5) * h
         g = g[(g >= 0) & (g <= 1)]
-        p = rng.uniform(0, 1, (20_000, 3))
+        p = rng.uniform(0, 1, (n, 3))
         for a in range(3):
             p[a::3, a] = rng.choice(g, p[a::3, a].shape)
         p = np.r_[p, [[0, 0, 0], [1, 1, 1]]].astype(np.float32)
         return p, rng.normal(size=p.shape).astype(np.float32)
     if name == "cube_faces":  # every point on a face of its bounding box, the largest extent along x
-        p = rng.uniform(-1, 1, (20_000, 3)) * np.array([2.0, 1.0, 0.5])
+        p = rng.uniform(-1, 1, (n, 3)) * np.array([2.0, 1.0, 0.5])
         ax = rng.integers(0, 3, p.shape[0])
         p[np.arange(p.shape[0]), ax] = np.sign(rng.normal(size=p.shape[0])) * np.array([2.0, 1.0, 0.5])[ax]
         return p.astype(np.float32), rng.normal(size=p.shape).astype(np.float32)
@@ -257,12 +259,14 @@ def test_scale_10m_depth10(lib):
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
     t0 = time.perf_counter()
-    m = mesh.poisson_mesh(P, N, depth=10)
+    m, dbg = mesh.poisson_mesh(P, N, depth=10, return_debug=True)
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
-    print(f"[10M, depth 10] {dt:.2f} s, peak {peak:.2f} GiB, {m.vertices.shape[0]} vertices, {m.faces.shape[0]} faces")
+    print(f"[10M, depth 10] {dt:.2f} s, peak {peak:.2f} GiB, {m.vertices.shape[0]} vertices, {m.faces.shape[0]} faces, "
+          f"{dbg['cycles']} cycles, ratio {dbg['ratio']:.2e}")
     assert dt < 60.0 and m.faces.shape[0] > 0 and int(m.faces.max()) < m.vertices.shape[0]
+    assert dbg["cycles"] < mesh.MAX_CYCLES and dbg["ratio"] <= mesh.TOLERANCE
 
 
 def test_mesh_pc_command(lib, tmp_path):
