@@ -470,3 +470,78 @@ extern "C" int g2pc_orient_finish(const float* uxyz, const double* unh, const in
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }
+
+// ---- normals turned toward the camera that saw each Gaussian best ----------------------------------------------
+// One grid-stride pass.  Row r reads f = cam_of[ids[r]]; a row whose id or camera index is out of range is invalid, a row
+// with f == INT32_MAX unseen; both are copied.  Otherwise dot = (nx*dx + ny*dy) + nz*dz with d = c_f - mu, in float64
+// from the stored values without FMA: dot < 0 negates the row, dot == 0 or NaN leaves it (undecided).  Each thread counts
+// its rows; at the end every warp folds its counts and one lane issues the four atomics.
+namespace {
+
+constexpr int FC_CTAS_MAX = 1024;
+
+template <typename NT>
+__global__ void __launch_bounds__(OB) face_cameras_kernel(const float* __restrict__ means, const NT* __restrict__ nrm,
+                                                          const int32_t* __restrict__ ids, int64_t m,
+                                                          const int32_t* __restrict__ cam_of, int64_t n,
+                                                          const float* __restrict__ cams, int64_t ncam,
+                                                          NT* __restrict__ out, unsigned long long* __restrict__ counts) {
+    unsigned c[4] = {0u, 0u, 0u, 0u};  // flipped, unseen, undecided, invalid
+    const int64_t stride = (int64_t)gridDim.x * OB;
+    for (int64_t r = (int64_t)blockIdx.x * OB + threadIdx.x; r < m; r += stride) {
+        const NT x = nrm[3 * r], y = nrm[3 * r + 1], z = nrm[3 * r + 2];
+        bool flip = false;
+        const int32_t g = ids[r];
+        if (g < 0 || g >= n) {
+            ++c[3];
+        } else {
+            const int32_t f = cam_of[g];
+            if (f == INT32_MAX) {
+                ++c[1];
+            } else if (f < 0 || f >= ncam) {
+                ++c[3];
+            } else {
+                const double dx = __dsub_rn((double)cams[3 * (int64_t)f], (double)means[3 * r]);
+                const double dy = __dsub_rn((double)cams[3 * (int64_t)f + 1], (double)means[3 * r + 1]);
+                const double dz = __dsub_rn((double)cams[3 * (int64_t)f + 2], (double)means[3 * r + 2]);
+                const double dot = __dadd_rn(__dadd_rn(__dmul_rn((double)x, dx), __dmul_rn((double)y, dy)),
+                                             __dmul_rn((double)z, dz));
+                flip = dot < 0.0;
+                if (flip) ++c[0];
+                else if (!(dot > 0.0)) ++c[2];
+            }
+        }
+        out[3 * r] = flip ? -x : x;
+        out[3 * r + 1] = flip ? -y : y;
+        out[3 * r + 2] = flip ? -z : z;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const unsigned s = __reduce_add_sync(0xffffffffu, c[k]);
+        if ((threadIdx.x & 31) == 0 && s) atomicAdd(counts + k, (unsigned long long)s);
+    }
+}
+
+}  // namespace
+
+extern "C" int g2pc_face_cameras(const float* means, const void* normals, int normal_dtype, const int32_t* ids,
+                                 int64_t m, const int32_t* cam_of, int64_t n, const float* cams, int64_t ncam,
+                                 void* out, int64_t* counts, void* stream) {
+    G2PC_CHECK_ARG(m >= 0 && n >= 0 && ncam >= 0, "m, n and ncam must be >= 0");
+    G2PC_CHECK_ARG(normal_dtype == G2PC_F32 || normal_dtype == G2PC_F64, "normals must be float32 or float64");
+    if (m == 0) return G2PC_OK;
+    G2PC_CHECK_ARG(means && normals && ids && out && counts && (n == 0 || cam_of) && (ncam == 0 || cams),
+                   "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    G2PC_CUDA(cudaMemsetAsync(counts, 0, 4 * sizeof(int64_t), st));
+    const unsigned grid = grid_of(m) < (unsigned)FC_CTAS_MAX ? grid_of(m) : (unsigned)FC_CTAS_MAX;
+    unsigned long long* cnt = (unsigned long long*)counts;
+    if (normal_dtype == G2PC_F32)
+        face_cameras_kernel<<<grid, OB, 0, st>>>(means, (const float*)normals, ids, m, cam_of, n, cams, ncam,
+                                                 (float*)out, cnt);
+    else
+        face_cameras_kernel<<<grid, OB, 0, st>>>(means, (const double*)normals, ids, m, cam_of, n, cams, ncam,
+                                                 (double*)out, cnt);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}

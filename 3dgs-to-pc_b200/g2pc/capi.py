@@ -81,6 +81,8 @@ SIGNATURES = {
     "g2pc_orient_finish_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_orient_finish": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, ctypes.c_int, _i64, _c_void_p, _c_void_p,
                             _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_face_cameras": ([_c_void_p, _c_void_p, ctypes.c_int, _c_void_p, _i64, _c_void_p, _i64, _c_void_p, _i64,
+                           _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_points_per_gaussian": ([_c_void_p, _c_void_p, _i64, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _i64,
                                   _c_void_p], ctypes.c_int),
     "g2pc_pack_geometry": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p], ctypes.c_int),

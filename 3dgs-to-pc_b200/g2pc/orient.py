@@ -6,6 +6,9 @@ Steps: g2pc_orient_prepare (usable points, unit normals) -> g2pc_knn_ids (k near
 (undirected k-NN edges, keys, flip bits) -> g2pc_orient_round until a round hooks nothing (Borůvka with sign parity) ->
 g2pc_orient_finish (seed per component, flips, output).  Host reads: the usable count after the prepare, the two round
 counts once per round, the stats at the end.
+
+face_cameras turns the normals of Gaussians toward the camera that saw each one best (g2pc_face_cameras, one pass, no
+neighbour graph); gauss_to_mesh.py orients its surface cloud that way.
 """
 import collections
 
@@ -17,6 +20,7 @@ K_MAX = 31  # G2PC_ORIENT_K_MAX in include/g2pc.h
 K_DEFAULT = 10
 
 OrientStats = collections.namedtuple("OrientStats", ["components", "flipped", "skipped", "rounds"])
+FaceCameraStats = collections.namedtuple("FaceCameraStats", ["flipped", "unseen", "undecided", "invalid"])
 
 
 def knn_ids(xyz, k):
@@ -109,3 +113,39 @@ def orient_normals(points, normals, k=K_DEFAULT, return_debug=False, timings=Non
              "edges": torch.stack([e >> 32, e & 0xFFFFFFFF], 1),
              "mst": torch.nonzero(mst[:E]).flatten(), "rel": srel[:m], "seed": seed[:m]}
     return out, info, debug
+
+
+def face_cameras(means, normals, ids, cam_of, cam_centres):
+    """Normals turned toward the camera that gave each Gaussian its maximum contribution (rules in DESIGN.md §2).
+
+    means (m,3) float32 and normals (m,3) float32 / float64 (not modified) of m Gaussians; ids (m,) int32: the original
+    row of each (Gaussians.ids); cam_of (N,) int32: the colour stage's first_frame over the original rows, INT32_MAX
+    where no camera raised a maximum; cam_centres (ncam,3) float32 in camera-index order; all CUDA tensors.  Returns
+    (normals: the input's dtype and values, with every row whose normal points away from its camera negated,
+    FaceCameraStats(flipped, unseen, undecided, invalid)).  Unseen rows (no camera) and undecided rows (normal
+    perpendicular to the view direction, or not finite) keep their sign.  Raises G2pcError when a row's id or camera index
+    is out of range."""
+    capi.check_cloud(means, normals, what="turning normals toward the cameras")
+    capi.require_cuda(ids, cam_of, cam_centres)
+    m, dev = means.shape[0], means.device
+    if ids is None or ids.dtype != torch.int32 or tuple(ids.shape) != (m,):
+        raise capi.G2pcError(f"ids must be ({m},) int32 like the means")
+    if cam_of is None or cam_of.dtype != torch.int32 or cam_of.dim() != 1:
+        raise capi.G2pcError("cam_of must be a 1-D int32 tensor")
+    if cam_centres is None or cam_centres.dtype != torch.float32 or cam_centres.dim() != 2 or cam_centres.shape[1] != 3:
+        raise capi.G2pcError("cam_centres must be (ncam, 3) float32")
+    if len({str(t.device) for t in (means, ids, cam_of, cam_centres)}) > 1:
+        raise capi.G2pcError("means, ids, cam_of and cam_centres are on different devices")
+    nrm = normals.contiguous()
+    out = torch.empty_like(nrm)
+    counts = torch.zeros((4,), dtype=torch.int64, device=dev)
+    if m:
+        capi.call("g2pc_face_cameras", capi.ptr(means.contiguous()), capi.ptr(nrm), capi.dtype_code(nrm),
+                  capi.ptr(ids.contiguous()), m, capi.ptr(cam_of.contiguous()), cam_of.shape[0],
+                  capi.ptr(cam_centres.contiguous()), cam_centres.shape[0], capi.ptr(out), capi.ptr(counts),
+                  capi.stream_ptr(dev))
+    stats = FaceCameraStats(*counts.tolist())
+    if stats.invalid:
+        raise capi.G2pcError(f"{stats.invalid} row(s) have a Gaussian id outside [0, {cam_of.shape[0]}) or a camera index "
+                             f"outside [0, {cam_centres.shape[0]})")
+    return out, stats

@@ -19,6 +19,9 @@ from g2pc.trace import nvtx
 
 LAST_SAMPLE_STATS = {}
 LAST_RENDER_STATS = {}
+# the surface stage of the last convert_gaussians_to_pc with generate_mesh: ids (original rows of the surface Gaussians),
+# first_frame (per original row, the camera that raised its maximum contribution), cam_centres, face_cameras (stats)
+LAST_SURFACE_STATS = {}
 COLOR_QUALITY_OPTIONS = {"tiny": 180, "low": 360, "medium": 720, "high": 1280, "ultra": 1920, "original": None}
 
 
@@ -264,13 +267,21 @@ def convert_3dgs_to_pc(input_path, transform_path, mask_path, pointcloud_setting
 
 
 def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transforms, intrinsics, mask_images,
-                            pointcloud_settings, render_shs=False):
+                            pointcloud_settings, render_shs=False, timings=None):
     """The device-resident part of convert_3dgs_to_pc (gauss_to_pc.py:414-601): everything between the loaders and the
     PLY writer.  transforms: {name: 4x4 c2w (nested list / tensor)} or None; intrinsics: {name: [w, h, fx, fy]}.
     render_shs=True evaluates the SH colour per camera inside the colour stage (the reference's CLI never passes the SH
-    coefficients to its renderer, gauss_to_pc.py:429-432; get_renderer accepts them)."""
+    coefficients to its renderer, gauss_to_pc.py:429-432; get_renderer accepts them).  `timings`: a dict that receives
+    CUDA event pairs per phase (colour, cull, sample, and with generate_mesh surface_select, face_cameras,
+    surface_sample).
+
+    With generate_mesh the surface cloud's normals are turned toward the camera that gave each surface Gaussian its
+    maximum contribution (g2pc.orient.face_cameras), so that they point from the solid toward free space."""
     s = pointcloud_settings
     say = (lambda *a: None) if s.quiet else print
+    if s.generate_mesh and s.render_colours and s.renderer_type != "cuda":
+        raise capi.G2pcError("meshing needs the surface distances of the cuda renderer (renderer_type='cuda'); the "
+                             "python renderer has none")
 
     with nvtx("g2pc: covariances + normals"):
         gaussians = Gaussians(xyz, scales, rots, colours, opacities, shs=shs)
@@ -297,32 +308,43 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
         if transforms is None:
             raise Exception("Transforms are required to render colours")
 
-        for img_name, transform in transforms.items():
-            # the 4x4 pose stays on the host: the camera matrices are kernel arguments, not device data
-            transform = torch.as_tensor(transform, dtype=torch.float32) if not torch.is_tensor(transform) else transform
-            mask = None
-            if mask_images is not None and img_name in mask_images.keys():
-                mask = mask_images[img_name].to(s.device)
-            camera = get_camera(s.renderer_type, transform, intrinsics[img_name], colour_resolution=s.colour_resolution,
-                                sh_degree=s.max_sh_degree, white_bkgd=True, mask=mask)
-            with nvtx(f"g2pc: camera {img_name}"):
-                render, _, _, depth_map = gaussian_renderer(camera)
+        first_frame, cam_centres = None, []
+        if s.generate_mesh:
+            # the accumulate kernels record, per Gaussian, the index of the camera that raised its maximum contribution
+            first_frame = torch.full((gaussians.xyz.shape[0],), torch.iinfo(torch.int32).max, dtype=torch.int32,
+                                     device=gaussians.xyz.device)
+            gaussian_renderer.first_frame = first_frame
 
-        say(f"\nNumber Initial Gaussians: {gaussians.xyz.shape[0]}")
+        with capi.phase(timings, "colour"):
+            for img_name, transform in transforms.items():
+                # the 4x4 pose stays on the host: the camera matrices are kernel arguments, not device data
+                transform = torch.as_tensor(transform, dtype=torch.float32) if not torch.is_tensor(transform) else transform
+                mask = None
+                if mask_images is not None and img_name in mask_images.keys():
+                    mask = mask_images[img_name].to(s.device)
+                camera = get_camera(s.renderer_type, transform, intrinsics[img_name], colour_resolution=s.colour_resolution,
+                                    sh_degree=s.max_sh_degree, white_bkgd=True, mask=mask)
+                if first_frame is not None:
+                    cam_centres.append(camera._campos_host)  # the centre the kernels use, in camera-index order
+                with nvtx(f"g2pc: camera {img_name}"):
+                    render, _, _, depth_map = gaussian_renderer(camera)
 
-        gaussians.colours = gaussian_renderer.get_gaussian_colours()
+            say(f"\nNumber Initial Gaussians: {gaussians.xyz.shape[0]}")
+
+            gaussians.colours = gaussian_renderer.get_gaussian_colours()
 
         # every cull of gauss_to_pc.py:483-496 in one fused mask + compaction (csrc/s8_cull.cu): surface distance,
         # visibility, min opacity, bounding box (+ the size-percentile cull, which needs a sort, through filter_indices)
-        surface_mask = None
-        if s.surface_distance_std is not None:
-            surface_mask = gaussian_renderer.get_gaussians_with_low_surface_distance()
-        gaussians.cull_large_gaussians(s.cull_large_percentage)
-        gaussian_renderer.flush() if hasattr(gaussian_renderer, "flush") else None
-        culled_indices = gaussians.fused_cull(
-            max_contribution=gaussian_renderer.gaussian_max_contribution if s.remove_unrendered_gaussians else None,
-            visibility_threshold=gaussian_renderer.visible_gaussian_threshold, min_opacity=s.min_opacity,
-            bounding_box_min=s.bounding_box_min, bounding_box_max=s.bounding_box_max, extra_mask=surface_mask)
+        with capi.phase(timings, "cull"):
+            surface_mask = None
+            if s.surface_distance_std is not None:
+                surface_mask = gaussian_renderer.get_gaussians_with_low_surface_distance()
+            gaussians.cull_large_gaussians(s.cull_large_percentage)
+            gaussian_renderer.flush() if hasattr(gaussian_renderer, "flush") else None
+            culled_indices = gaussians.fused_cull(
+                max_contribution=gaussian_renderer.gaussian_max_contribution if s.remove_unrendered_gaussians else None,
+                visibility_threshold=gaussian_renderer.visible_gaussian_threshold, min_opacity=s.min_opacity,
+                bounding_box_min=s.bounding_box_min, bounding_box_max=s.bounding_box_max, extra_mask=surface_mask)
 
         say(f"\nNumber Gaussians after Culling: {gaussians.xyz.shape[0]}")
 
@@ -330,8 +352,10 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
             raise Exception("Number of Gaussians after culling is 0, meaning a point cloud cannot be generated")
 
         if s.generate_mesh:
-            surface_gaussian_idxs = gaussian_renderer.get_predicted_surface_gaussians(predicted_surface_std=1.0)
-            surface_gaussian_idxs = surface_gaussian_idxs[culled_indices]
+            # a mask over the original rows, then over the kept rows of the cull (culled_indices is their ascending list)
+            with capi.phase(timings, "surface_select"):
+                surface_gaussian_idxs = gaussian_renderer.get_predicted_surface_gaussians(predicted_surface_std=1.0)
+                surface_gaussian_idxs = surface_gaussian_idxs[culled_indices]
 
         if s.prioritise_visible_gaussians:
             total_gaussian_contributions = gaussian_renderer.get_total_gaussian_contributions()[culled_indices]
@@ -356,7 +380,7 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
 
     say("\nStarting Point Cloud Generation for All Gaussians\n")
 
-    with nvtx("g2pc: point budget + sampling"):
+    with nvtx("g2pc: point budget + sampling"), capi.phase(timings, "sample"):
         points, colours, normals = generate_pointcloud(gaussians, s.num_points, exact_num_points=s.exact_num_points,
                                                        mahalanobis_distance_std=s.mahalanobis_distance_std,
                                                        calculate_normals=s.calculate_normals,
@@ -369,23 +393,45 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
 
     if s.generate_mesh and s.render_colours:
         say("Starting Point Cloud Generation for Surface Gaussians\n")
-        surface_gaussian_idxs = surface_gaussian_idxs[valid]
-        gaussians.add_gaussians_to_cull(surface_gaussian_idxs)
-        gaussians.filter_gaussians()
+        from g2pc import orient
+        with capi.phase(timings, "surface_select"):
+            # the validation's keep mask, then the surface filter: the mask now runs over the validated rows
+            surface_gaussian_idxs = surface_gaussian_idxs[valid]
+            n_surface = int(surface_gaussian_idxs.sum().item())
+            if n_surface == 0:
+                raise capi.G2pcError("no Gaussian lies on a predicted surface (surface distance below its mean): "
+                                     "there is nothing to mesh")
+            gaussians.add_gaussians_to_cull(surface_gaussian_idxs)
+            gaussians.filter_gaussians()
+        with capi.phase(timings, "face_cameras"):
+            cams = torch.tensor(cam_centres, dtype=torch.float32).reshape(-1, 3).to(gaussians.xyz.device)
+            gaussians.normals, face_stats = orient.face_cameras(gaussians.xyz, gaussians.normals, gaussians.ids,
+                                                                first_frame, cams)
+        global LAST_SURFACE_STATS
+        LAST_SURFACE_STATS = {"ids": gaussians.ids, "first_frame": first_frame, "cam_centres": cams,
+                              "face_cameras": face_stats}
         avg_points_per_gauss_for_mesh = 25
         total_mesh_points = min(s.num_points // 2, int(gaussians.xyz.shape[0] * avg_points_per_gauss_for_mesh))
-        points, colours, normals = generate_pointcloud(gaussians, total_mesh_points, exact_num_points=s.exact_num_points,
-                                                       num_sample_attempts=num_sample_attempts,
-                                                       contributions=total_gaussian_contributions[surface_gaussian_idxs],
-                                                       device=s.device, quiet=s.quiet)
+        # (the reference indexes the contributions unconditionally and raises a TypeError when they are None)
+        contributions = None if total_gaussian_contributions is None else \
+            total_gaussian_contributions[surface_gaussian_idxs]
+        with capi.phase(timings, "surface_sample"):
+            points, colours, normals = generate_pointcloud(gaussians, total_mesh_points,
+                                                           exact_num_points=s.exact_num_points,
+                                                           num_sample_attempts=num_sample_attempts,
+                                                           contributions=contributions, device=s.device, quiet=s.quiet)
         surface_point_cloud = PointCloudData(points=points, colours=colours, normals=normals)
 
     return total_point_cloud, surface_point_cloud
 
 
-def config_parser(argv=None):
+def config_parser(argv=None, mesh=False):
     """Same flags and validation as the reference (gauss_to_pc.py:603-710).  configargparse is optional in this
-    image; argparse accepts the same flag names."""
+    image; argparse accepts the same flag names.
+
+    mesh=True parses for gauss_to_mesh.py: --generate_mesh is implied and meshes with this project's GPU mesher
+    (g2pc/mesh.py) instead of Open3D, which needs renderer_type cuda, a depth in mesh.DEPTH_MIN..DEPTH_MAX and
+    laplacian_iterations >= 0."""
     try:
         import configargparse as ap
     except ImportError:
@@ -421,6 +467,15 @@ def config_parser(argv=None):
     parser.add_argument("--quiet", action="store_true", help="Suppress output")
 
     args = parser.parse_args(argv)
+    if mesh:
+        from g2pc import mesh as gmesh
+        args.generate_mesh = True
+        if args.renderer_type != "cuda":
+            raise AttributeError("Meshing needs the surface distances of the cuda renderer (--renderer_type cuda)")
+        if not gmesh.DEPTH_MIN <= args.poisson_depth <= gmesh.DEPTH_MAX:
+            raise AttributeError(f"Poisson depth must be between {gmesh.DEPTH_MIN} and {gmesh.DEPTH_MAX}")
+        if args.laplacian_iterations < 0:
+            raise AttributeError("Laplacian iterations must be 0 or more")
 
     if args.min_opacity < 0 or args.min_opacity > 1:
         raise AttributeError("Minumum opacity must be between 0 and 1")
@@ -460,19 +515,23 @@ def config_parser(argv=None):
         raise AttributeError("Cannot use masks when no transforms have been provided")
     if args.renderer_type != "cuda" and args.surface_distance_std is not None:
         raise AttributeError("Surface distance calculations only supported in CUDA renderer")
-    if args.generate_mesh:
+    if args.generate_mesh and not mesh:
         # Open3D meshing is outside this build (SURVEY.md §2 row 15): fail before any loading / rendering
         try:
             import open3d  # noqa: F401
         except ImportError:
-            raise AttributeError("--generate_mesh needs Open3D, which is not installed")
-        raise AttributeError("--generate_mesh (Open3D Poisson meshing) is not part of this build")
+            raise AttributeError("--generate_mesh needs Open3D, which is not installed; gauss_to_mesh.py meshes on "
+                                 "the GPU")
+        raise AttributeError("--generate_mesh (Open3D Poisson meshing) is not part of this build; gauss_to_mesh.py "
+                             "meshes on the GPU")
 
     return args
 
 
-def main(argv=None):
-    args = config_parser(argv)
+def main(argv=None, mesh=False):
+    """The command.  mesh=True is gauss_to_mesh.py: after the point cloud it writes the mesh of the surface cloud to
+    --mesh_output_path and returns (surface PointCloudData with normals facing the cameras, g2pc.mesh.Mesh)."""
+    args = config_parser(argv, mesh=mesh)
 
     if not torch.cuda.is_available():
         raise capi.G2pcError("a CUDA device is required (the g2pc kernels have no CPU fallback)")
@@ -519,7 +578,20 @@ def main(argv=None):
     save_xyz_to_ply(total_point_cloud.points, args.output_path, rgb_colors=total_point_cloud.colours,
                     normals_points=total_point_cloud.normals, chunk_size=10**6, quiet=args.quiet)
 
-    if pointcloud_settings.generate_mesh:
+    if mesh:
+        from g2pc import mesh as gmesh
+        st = LAST_SURFACE_STATS["face_cameras"]
+        if not args.quiet:
+            print(f"Turned the surface normals toward their cameras: {st.flipped} flipped, {st.unseen} unseen, "
+                  f"{st.undecided} undecided")
+            print(f"Meshing {surface_point_cloud.points.shape[0]} surface points at depth {args.poisson_depth}")
+        m = gmesh.poisson_mesh(surface_point_cloud.points, surface_point_cloud.normals, surface_point_cloud.colours,
+                               depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations, std_ratio=3.0)
+        gmesh.write_mesh_ply(args.mesh_output_path, m)
+        if not args.quiet:
+            print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")
+        return surface_point_cloud, m
+    elif pointcloud_settings.generate_mesh:
         from mesh_handler import generate_mesh
         generate_mesh(surface_point_cloud.points, surface_point_cloud.colours, surface_point_cloud.normals,
                       args.mesh_output_path, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations)

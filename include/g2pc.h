@@ -310,6 +310,18 @@ int g2pc_orient_finish(const float* uxyz, const double* unh, const int32_t* rows
                        int normal_dtype, int64_t n, const int32_t* comp, const uint8_t* rel, void* out, int32_t* seed,
                        uint8_t* seed_rel, int64_t* stats, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Normals turned toward the camera that saw each Gaussian (gauss_to_mesh.py; rules in DESIGN.md §2).  means (m,3
+ * float32), normals (m,3 float32 or float64, normal_dtype), ids (m int32): the original Gaussian row of each row;
+ * cam_of (n int32): the colour stage's first_frame, INT32_MAX = never raised a maximum; cams (ncam,3 float32): camera
+ * centres in camera-index order.  Row r with f = cam_of[ids[r]]: invalid when ids[r] is outside [0, n) or f is outside
+ * [0, ncam) and not INT32_MAX; unseen when f == INT32_MAX; otherwise dot = (nx*dx + ny*dy) + nz*dz, d = cams[f] - means[r],
+ * in float64 of the stored values without FMA.  out (m,3, the normals' dtype) = the row negated when dot < 0 (flipped),
+ * the row unchanged otherwise (dot == 0 or NaN: undecided).  counts (4 int64) = flipped, unseen, undecided, invalid.
+ * The normals are not modified.  m = 0 launches nothing and writes nothing. */
+int g2pc_face_cameras(const float* means, const void* normals, int normal_dtype, const int32_t* ids, int64_t m,
+                      const int32_t* cam_of, int64_t n, const float* cams, int64_t ncam, void* out, int64_t* counts,
+                      void* stream);
+
 /* ---- S3-S6: colour stage, renderer_type=python semantics (gauss_render.py:101-465) ------------------------------ */
 /* Replaces GaussPythonRenderer.__call__/render (gauss_render.py:266-465) and — as the native op boundary — the role
  * of _C.rasterize_gaussians (rasterize_points.cu:36-145) in the per-camera loop of gauss_to_pc.py:437-454.
