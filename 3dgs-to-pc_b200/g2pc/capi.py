@@ -88,6 +88,9 @@ SIGNATURES = {
     "g2pc_pack_geometry": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_preprocess": ([_c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i64, _c_void_p, _c_void_p, _c_void_p, _i32, _u32,
                          _u32, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
+    "g2pc_preprocess_cameras": ([_c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i64, _c_void_p, _i32, _c_void_p,
+                                 _c_void_p, _i32, _u32, _u32, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p],
+                                ctypes.c_int),
     "g2pc_depth_sort_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_depth_sort": ([_c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_build_tree": ([_c_void_p, _i32, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i64, _i64,
@@ -135,6 +138,7 @@ HDR_WORDS = 16
 WORK_COUNTERS = 4
 STAT_WARP_GAUSSIANS, STAT_WORDS = 0, 4
 LEAF_WORDS = 8  # g2pc_leaf_t = 8 x int32
+PREPROCESS_MAX_CAMERAS = 8  # G2PC_PREPROCESS_MAX_CAMERAS
 
 _lib = None
 

@@ -34,6 +34,11 @@ BLEND_T_STOP = 1e-6
 # second CUDA stream (g2pc/frames.py); 1 = strictly serial.
 FRAME_SLOTS = 2
 
+# python back-end, async mode: consecutive cameras of one resolution projected by one preprocess launch, which reads the
+# scene once per batch instead of once per camera (g2pc/frames.py, csrc/s3_preprocess.cu).  1..8; 1 = one launch per
+# camera.  Each further camera costs two more sets of per-camera outputs (N x 60 bytes each: 180 MB at 3 M Gaussians).
+PREPROCESS_CAMERAS = 4
+
 # NVTX ranges around the stages of the pipeline (covariances / colour stage / culls / validate / sampling) and around
 # every camera: visible in nsys / ncu timelines, ~1 us each when no tool is attached.
 NVTX = True

@@ -193,7 +193,8 @@ class GaussianRasterizer(FrameQueue):
         # (kept per slot: the tensor must outlive the frame's kernels, the slot is reused only after they have run)
         self._slots[slot]["mask"] = self._mask_of(rs, int(rs.image_width), int(rs.image_height))
 
-    def _enqueue_front(self, rs, frame, slot):
+    def _enqueue_front(self, rs, frame, slot, pre=None):
+        # (this back-end projects each camera here, into the slot's own buffers: `pre` is not used)
         st = capi.stream_ptr(self.device)
         W, H = int(rs.image_width), int(rs.image_height)
         n = self._n

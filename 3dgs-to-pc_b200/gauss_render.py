@@ -88,7 +88,10 @@ class GaussPythonRenderer(FrameQueue):
         self._geom = torch.empty((max(n, 1), 12), dtype=torch.float32, device=dev)
         capi.call("g2pc_pack_geometry", capi.ptr(self.means3D), capi.ptr(self.cov3d), capi.ptr(self.opacity), n,
                   capi.ptr(self._geom), st)
-        self._init_frames()
+        k = int(config.PREPROCESS_CAMERAS)
+        if not 1 <= k <= capi.PREPROCESS_MAX_CAMERAS:
+            raise capi.G2pcError(f"config.PREPROCESS_CAMERAS must be 1..{capi.PREPROCESS_MAX_CAMERAS}, got {k}")
+        self._init_frames(preprocess_cameras=k)
         self._leaf_colour = None
 
     # ---- getters (gauss_render.py:237-264; get_gaussian_colours in FrameQueue) -------------------------------------
@@ -135,6 +138,9 @@ class GaussPythonRenderer(FrameQueue):
                      image=torch.ones((H, W, 3), dtype=torch.float32, device=dev),
                      leaf_cap=0, pix_cap=int(1.25 * W * H) + 4096,
                      max_leaf=(int(min(self.max_tile_size, W)), int(min(self.max_tile_size, H))))
+            # tile counters of every camera of a batch set (the preprocess fills them, g2pc_build_tree clears them)
+            t["pre_cnt"] = [[ts["node_cnt"]] + [torch.zeros((qt.nodes_2d,), dtype=torch.int32, device=dev)
+                                                for _ in range(self.preprocess_cameras - 1)] for ts in t["slots"]]
             self._set_leaf_cap(t, min(qt.nodes_2d, 2 * (4 ** base)))
             self._tables[key] = t
         return t
@@ -180,26 +186,45 @@ class GaussPythonRenderer(FrameQueue):
         if self._leaf_colour is None or self._leaf_colour.numel() < 3 * t["pix_cap"]:
             self._leaf_colour = torch.empty((3 * t["pix_cap"],), dtype=torch.float32, device=self.device)
 
-    def _enqueue_front(self, camera, frame, slot):
-        """Projection, depth sort, tile table and per-tile lists of one camera, asynchronously on the current stream."""
+    def _enqueue_preprocess(self, cameras, bset):
+        """Projection, SH colour and tile counts of a batch of cameras of one resolution into batch set bset, in one pass
+        over the scene (one camera: g2pc_preprocess), asynchronously on the current stream."""
+        st = capi.stream_ptr(self.device)
+        k = len(cameras)
+        t = self._get_tables(int(cameras[0].image_width), int(cameras[0].image_height))
+        qt = t["qt"]
+        sets, cnts = self._pre_sets[bset][:k], t["pre_cnt"][bset][:k]
+        scene = (capi.ptr(self._geom), capi.ptr(self._colour_f32) if self.shs is None else None, capi.ptr(self.shs),
+                 int(self.shs.shape[-1]) if self.shs is not None else 0, self.sh_degree, self._n)
+        if k == 1:
+            cam = self._camera_struct(cameras[0])
+            capi.call("g2pc_preprocess", *scene, ctypes.byref(cam), capi.ptr(t["tables"]), capi.ptr(t["luts"]),
+                      qt.num_levels, t["level_mask"], t["clean_mask"], capi.ptr(sets[0]["proj"]), capi.ptr(cnts[0]),
+                      capi.ptr(sets[0]["depth_key"]), capi.ptr(sets[0]["val"]), st)
+            return
+        cams = (capi.Camera * k)(*[self._camera_struct(c) for c in cameras])
+        ptrs = lambda ts: (ctypes.c_void_p * k)(*[capi.ptr(x) for x in ts])
+        capi.call("g2pc_preprocess_cameras", *scene, cams, k, capi.ptr(t["tables"]), capi.ptr(t["luts"]), qt.num_levels,
+                  t["level_mask"], t["clean_mask"], ptrs([x["proj"] for x in sets]), ptrs(cnts),
+                  ptrs([x["depth_key"] for x in sets]), ptrs([x["val"] for x in sets]), st)
+
+    def _enqueue_front(self, camera, frame, slot, pre):
+        """Depth sort, tile table and per-tile lists of one camera whose projection _enqueue_preprocess wrote into
+        pre = (batch set, camera of the batch), asynchronously on the current stream."""
         st = capi.stream_ptr(self.device)
         W, H = int(camera.image_width), int(camera.image_height)
-        cam = self._camera_struct(camera)
         n = self._n
         t = self._get_tables(W, H)
         qt = t["qt"]
+        ps, node_cnt = self._pre_sets[pre[0]][pre[1]], t["pre_cnt"][pre[0]][pre[1]]
         sl, ts = self._slots[slot], t["slots"][slot]
-        capi.call("g2pc_preprocess", capi.ptr(self._geom), capi.ptr(self._colour_f32) if self.shs is None else None,
-                  capi.ptr(self.shs), int(self.shs.shape[-1]) if self.shs is not None else 0, self.sh_degree, n,
-                  ctypes.byref(cam), capi.ptr(t["tables"]), capi.ptr(t["luts"]), qt.num_levels, t["level_mask"],
-                  t["clean_mask"], capi.ptr(sl["proj"]),
-                  capi.ptr(ts["node_cnt"]), capi.ptr(sl["depth_key"]), capi.ptr(sl["val"]), st)
-        self._depth_sort(sl, st)
+        sl["pre"] = ps  # the records the back half blends
+        self._depth_sort(sl, st, ps)
         capi.call("g2pc_build_tree", capi.ptr(t["tables"]), qt.num_levels, qt.max_gaussians_per_tile,
-                  capi.ptr(ts["node_cnt"]), capi.ptr(ts["node_state"]), capi.ptr(ts["node_leaf"]), capi.ptr(ts["leaves"]),
+                  capi.ptr(node_cnt), capi.ptr(ts["node_state"]), capi.ptr(ts["node_leaf"]), capi.ptr(ts["leaves"]),
                   capi.ptr(ts["leaf_order"]), t["leaf_cap"], self._inst_cap, t["pix_cap"], sl["matrix"].numel(),
                   t["chunks"], frame, capi.ptr(sl["hdr"]), capi.ptr(self._fail), capi.ptr(sl["work"]), st)
-        capi.call("g2pc_multisplit", capi.ptr(sl["val_sorted"]), n, capi.ptr(sl["proj"]), W, H, capi.ptr(t["tables"]),
+        capi.call("g2pc_multisplit", capi.ptr(sl["val_sorted"]), n, capi.ptr(ps["proj"]), W, H, capi.ptr(t["tables"]),
                   qt.num_levels, t["level_mask"], t["clean_mask"], capi.ptr(ts["node_leaf"]), capi.ptr(ts["leaves"]),
                   capi.ptr(sl["hdr"]),
                   capi.ptr(self._fail), frame, t["leaf_cap"], capi.ptr(sl["matrix"]), capi.ptr(sl["inst_gid"]), st)
@@ -215,7 +240,7 @@ class GaussPythonRenderer(FrameQueue):
         sl, ts = self._slots[slot], t["slots"][slot]
         bg = 1.0 if self.white_bkgd else 0.0
         capi.call("g2pc_blend", capi.ptr(ts["leaves"]), capi.ptr(ts["leaf_order"]), capi.ptr(sl["hdr"]),
-                  capi.ptr(self._fail), frame, *t["max_leaf"], capi.ptr(sl["inst_gid"]), capi.ptr(sl["proj"]),
+                  capi.ptr(self._fail), frame, *t["max_leaf"], capi.ptr(sl["inst_gid"]), capi.ptr(sl["pre"]["proj"]),
                   capi.ptr(self._cam_best), capi.ptr(self.gaussian_max_contribution), capi.ptr(self._leaf_colour),
                   capi.ptr(t["owner"]), W, H, bg, float(self.t_stop), capi.ptr(sl["work"]), capi.ptr(self._stats), st)
         capi.call("g2pc_accumulate", capi.ptr(self._cam_best), capi.ptr(self._leaf_colour), n,
@@ -233,10 +258,11 @@ class GaussPythonRenderer(FrameQueue):
         self._submit(camera, camera_index)
         if not self.compose_image:
             return None, None, None, None
-        t = self._last_tables  # (a replay may have switched to a deeper table set)
         # confirmed frames get their own tensor, like the reference; in async mode the shared buffer is handed out (it is
-        # final once flush() has run and is overwritten by the next camera)
-        return (t["image"] if self.async_mode else t["image"].clone()), None, None, None
+        # final once flush() has run and is overwritten by the next camera; the camera itself may still be deferred)
+        if self.async_mode:
+            return self._get_tables(int(camera.image_width), int(camera.image_height))["image"], None, None, None
+        return self._last_tables["image"].clone(), None, None, None  # (a replay may have switched to a deeper table set)
 
     # ---- FrameQueue hooks ---------------------------------------------------------------------------------------------
     def _confirm(self, h):
@@ -279,7 +305,7 @@ class GaussPythonRenderer(FrameQueue):
         out = []
         for (r0, c0, w, h, beg, cnt, pix, node) in leaves:
             out.append((int(r0), int(c0), int(w), int(h), gids[beg:beg + cnt]))
-        return sl["proj"].cpu().numpy(), out
+        return sl["pre"]["proj"].cpu().numpy(), out
 
 
 def get_renderer(renderer_type: str, xyz, opacities, colours, covariances, shs=None, visible_gaussian_threshold=0.0,

@@ -393,6 +393,18 @@ int g2pc_preprocess(const void* geom, const float* colours, const float* shs, in
                     int32_t num_levels, uint32_t level_mask, uint32_t clean_mask, void* proj, uint32_t* node_cnt,
                     uint32_t* depth_key, uint64_t* val, void* stream);
 
+/* S3 for a batch of cameras: the same outputs as num_cameras calls of g2pc_preprocess, bit for bit, with the scene read
+ * once per batch instead of once per camera.  cams_host: num_cameras (1..G2PC_PREPROCESS_MAX_CAMERAS) cameras of one
+ * resolution, which share tables / luts / masks.  proj, node_cnt, depth_key, val: host arrays of num_cameras device
+ * pointers, camera c's outputs as g2pc_preprocess describes them.  The cameras whose node histograms do not fit the
+ * shared memory together go to further launches (one camera per launch when even one histogram does not fit). */
+#define G2PC_PREPROCESS_MAX_CAMERAS 8
+int g2pc_preprocess_cameras(const void* geom, const float* colours, const float* shs, int32_t sh_stride,
+                            int32_t sh_degree, int64_t n, const g2pc_camera_t* cams_host, int32_t num_cameras,
+                            const int32_t* tables, const uint16_t* luts, int32_t num_levels, uint32_t level_mask,
+                            uint32_t clean_mask, void* const* proj, uint32_t* const* node_cnt,
+                            uint32_t* const* depth_key, uint64_t* const* val, void* stream);
+
 /* S4a.  val_sorted[k] = val of the k-th nearest Gaussian (stable radix sort of depth_key: ties keep index order, the
  * reference's torch.sort is unstable there, gauss_render.py:340-344).  cub::DeviceRadixSort (library call). */
 int64_t g2pc_depth_sort_workspace_bytes(int64_t n);
