@@ -27,7 +27,35 @@
 // Short-cuts: (i) a warp stops once ALL its pixels have T below t_stop (checked every 32 Gaussians): every contribution
 // it skips is < t_stop and so is their sum per pixel; t_stop = FLT_MIN in strict-parity runs; (ii) the arg-max
 // bookkeeping of a Gaussian is skipped by a warp when none of its contributions exceeds the maximum the Gaussian already
-// holds from earlier cameras (the update rule is a strict >, so such contributions can never be recorded).
+// holds from earlier cameras (the update rule is a strict >, so such contributions can never be recorded); (iii) the
+// footprint cull below.
+//
+// Footprint cull (only when t_stop > FLT_MIN and g2pc_blend_set_cull is on, the default; the strict-parity setting
+// t_stop = FLT_MIN runs the kernel instantiated without it).  Every Gaussian of a list reaches every pixel of the leaf,
+// but a splat that touches one corner of a leaf is negligible over most of the warps' pixel rectangles.  Per leaf
+//     eps = min(2^-26, t_stop / cnt)                                       (cnt: the leaf's list length)
+// and at the start of each 32-entry sub-step lane l tests entry j0 + l against the warp's rectangle R (the bounding box
+// of its active pixels).  With the record's conic pre-scaled by K = -log2(e)/2, (a, b, c) = (q0.z, q0.w, q1.x), and
+// L = log2(opacity) (q1.y), the kernel's exponent is e = L - q(d), q(d) = -(a dx^2 + b dx dy + c dy^2), d = pixel -
+// mean, and alpha <= exp2(e).  So alpha < eps on all of R when  min_R q > kappa = L - log2(eps).  For a < 0, c < 0 the
+// restriction of q to a line of constant x or y is a convex parabola, and q has no critical point but d = 0, so when
+// the mean lies outside R the minimum over R is the least of the four edge minima, each found by clamping the
+// parabola's vertex to the edge: the test is exact (not a bounding-box test) and needs no det > 0.  The lane votes
+// "skip" only when all of: a < 0, c < 0, 4ac > b^2, the mean is outside R (closed), every term is finite, and
+//     min_R q > kappa + 2^-16 S + 2^-12,    S = |L| + |a| Dx^2 + |b| Dx Dy + |c| Dy^2,
+// Dx, Dy the largest |dx|, |dy| over R.  The margin: each product of the kernel's e (dx, dy, dy^2, b dy, the two FMAs)
+// is rounded at most 5 times, so |e_f32 - e| <= 5 u S (u = 2^-24); the test's own f32 edge minima and S are off by a
+// few u S more (the clamped vertex is off by a rounding, which raises q by a second-order amount); together below
+// 16 u S = 2^-20 S, taken with 16x headroom.  The absolute 2^-12 covers ex2.approx (relative error < 2^-21, i.e.
+// < 2^-20 in log2 units) and the rounding of log2(eps) and kappa (|log2 eps| < 64: a few ulp of 64 = 2^-17).  NaN or
+// infinite terms make S or kappa + margin non-finite, and every comparison then keeps the entry.  The warp walks the
+// kept entries of the ballot in ascending order, so depth order is unchanged; `iters` counts only those.  Two
+// properties follow:
+//   * T is bit-identical: a skipped alpha is < 2^-26, so c = T alpha < half an ulp of T and T - c rounds to T.  Every
+//     kept contribution is computed bit for bit as without the cull, and so are the per-Gaussian maxima and arg-max
+//     pixels of every Gaussian whose maximum is >= 2^-26 (>= eps of every leaf).
+//   * bounded colour change: the skipped contributions of a pixel sum to < cnt eps <= t_stop, the same bound as the
+//     transmittance stop, so default vs strict still moves a colour by < 2 t_stop x max |colour|.
 #include "colour_common.cuh"
 
 namespace {
@@ -73,6 +101,32 @@ __device__ __forceinline__ void cp_async4(void* dst, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 
+// q(d) = -(a dx^2 + b dx dy + c dy^2)
+__device__ __forceinline__ float cull_q(float a, float b, float c, float dx, float dy) {
+    return -fmaf(dx, fmaf(a, dx, b * dy), c * dy * dy);
+}
+
+// footprint cull (header comment): true when alpha < 2^log2eps at every point of the rectangle [x0, x1] x [y0, y1]
+__device__ __forceinline__ bool cull_negligible(float4 q0, float4 q1, float x0, float x1, float y0, float y1,
+                                                float log2eps) {
+    const float a = q0.z, b = q0.w, c = q1.x, L = q1.y;
+    const float dx0 = x0 - q0.x, dx1 = x1 - q0.x, dy0 = y0 - q0.y, dy1 = y1 - q0.y;
+    const bool inside = dx0 <= 0.0f && dx1 >= 0.0f && dy0 <= 0.0f && dy1 >= 0.0f;
+    const float Dx = fmaxf(fabsf(dx0), fabsf(dx1)), Dy = fmaxf(fabsf(dy0), fabsf(dy1));
+    const float S = fabsf(L) + fabsf(a) * Dx * Dx + fabsf(b) * Dx * Dy + fabsf(c) * Dy * Dy;
+    // edge minima: the parabola along x = const has its vertex at dy = -b dx / (2c), along y = const at dx = -b dy / (2a)
+    const float ry = -0.5f * b / c, rx = -0.5f * b / a;
+    const float qmin = fminf(fminf(cull_q(a, b, c, dx0, fminf(fmaxf(ry * dx0, dy0), dy1)),
+                                   cull_q(a, b, c, dx1, fminf(fmaxf(ry * dx1, dy0), dy1))),
+                             fminf(cull_q(a, b, c, fminf(fmaxf(rx * dy0, dx0), dx1), dy0),
+                                   cull_q(a, b, c, fminf(fmaxf(rx * dy1, dx0), dx1), dy1)));
+    const float kappa = L - log2eps;
+    // a finite S bounds every term; finite vertex slopes keep the clamps from meeting inf x 0
+    return S + fabsf(rx) + fabsf(ry) < INFINITY && a < 0.0f && c < 0.0f && 4.0f * a * c > b * b && !inside &&
+           qmin > kappa + fmaf(S, 0x1p-16f, 0x1p-12f);
+}
+
+template <bool CULL>
 __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
     __shared__ __align__(16) float4 s_q0[2][CH];
     __shared__ __align__(16) float4 s_q1[2][CH];
@@ -145,6 +199,16 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
     const int pix_row = row * lf.w + x0;
 
     const int cnt = lf.inst_count;
+    // footprint cull: the warp's rectangle (bounding box of its active pixels; a warp without one has T = 0 everywhere,
+    // so whatever it skips changes nothing) and log2 eps = min(-26, log2(t_stop / cnt))
+    float rx0 = 0.f, rx1 = 0.f, ry0 = 0.f, ry1 = 0.f, log2eps = 0.f;
+    if constexpr (CULL) {
+        rx0 = (float)(lf.c0 + (int)__reduce_min_sync(FULLM, active ? (unsigned)x0 : 1u << 30));
+        rx1 = (float)(lf.c0 + (int)__reduce_max_sync(FULLM, active ? (unsigned)min(x0 + 3, lf.w - 1) : 0u));
+        ry0 = (float)(lf.r0 + (int)__reduce_min_sync(FULLM, active ? (unsigned)row : 1u << 30));
+        ry1 = (float)(lf.r0 + (int)__reduce_max_sync(FULLM, active ? (unsigned)row : 0u));
+        log2eps = fminf(-26.0f, log2f(t_stop) - log2f((float)cnt));
+    }
     const int nchunks = (cnt + CH - 1) / CH;
     const uint32_t* list = p.inst_gid + (int64_t)lf.inst_begin;  // 16-byte aligned (tree kernel)
 
@@ -189,7 +253,7 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
         if (!warp_done) {
             for (int j0 = 0; j0 < nload; j0 += SUB) {
                 const int j1 = min(nload, j0 + SUB);
-                for (int j = j0; j < j1; ++j) {
+                auto blend_one = [&](const int j) {
                     const float4 q0 = q0s[j];
                     const float4 q1 = q1s[j];
                     const float2 bt = bs[j];
@@ -225,8 +289,21 @@ __global__ void __launch_bounds__(BT, 8) blend_kernel(const BlendParams p) {
                         const uint32_t wp = __reduce_max_sync(FULLM, pk);
                         if (lane == 0) s_best[warp][j] = ((unsigned long long)wm << 32) | (unsigned long long)wp;
                     }
+                };
+                if constexpr (CULL) {
+                    // lane l votes for entry j0 + l; the kept entries are walked in ascending (depth) order
+                    const bool mine = lane < j1 - j0;
+                    unsigned keep = __ballot_sync(FULLM, mine && !cull_negligible(q0s[j0 + lane], q1s[j0 + lane],
+                                                                                  rx0, rx1, ry0, ry1, log2eps));
+                    iters += (unsigned long long)__popc(keep);
+                    while (keep) {
+                        blend_one(j0 + __ffs(keep) - 1);
+                        keep &= keep - 1u;
+                    }
+                } else {
+                    for (int j = j0; j < j1; ++j) blend_one(j);
+                    iters += (unsigned long long)(j1 - j0);
                 }
-                iters += (unsigned long long)(j1 - j0);
                 const float tmax = fmaxf(fmaxf(T01.x, T01.y), fmaxf(T23.x, T23.y));
                 warp_done = __all_sync(FULLM, tmax < t_stop);
                 if (warp_done) break;
@@ -316,6 +393,10 @@ static int g_blend_compact = 1;
 /* experiment switch (bench / tests): 1 = compact warp footprints (default), 0 = row strips */
 extern "C" void g2pc_blend_set_compact(int on) { g_blend_compact = on ? 1 : 0; }
 
+static int g_blend_cull = 1;
+/* experiment switch (bench / tests): 1 = footprint cull when t_stop > FLT_MIN (default), 0 = never */
+extern "C" void g2pc_blend_set_cull(int on) { g_blend_cull = on ? 1 : 0; }
+
 extern "C" int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header,
                           const uint32_t* fail, int32_t frame, int32_t max_leaf_width, int32_t max_leaf_height,
                           const uint32_t* inst_gid, const void* proj,
@@ -349,7 +430,10 @@ extern "C" int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, 
     p.slabs = (int32_t)slabs;
     p.work_counter = work_counters;
     p.stats = (unsigned long long*)stats;
-    blend_kernel<<<(unsigned)g2pc_resident_ctas(blend_kernel, BT, 0, 8), BT, 0, (cudaStream_t)stream>>>(p);
+    if (g_blend_cull && p.t_stop > 1.17549435e-38f)
+        blend_kernel<true><<<(unsigned)g2pc_resident_ctas(blend_kernel<true>, BT, 0, 8), BT, 0, (cudaStream_t)stream>>>(p);
+    else
+        blend_kernel<false><<<(unsigned)g2pc_resident_ctas(blend_kernel<false>, BT, 0, 8), BT, 0, (cudaStream_t)stream>>>(p);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
 }

@@ -103,6 +103,7 @@ SIGNATURES = {
                     _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _f32, _f32, _c_void_p, _c_void_p, _c_void_p],
                    ctypes.c_int),
     "g2pc_blend_set_compact": ([ctypes.c_int], None),
+    "g2pc_blend_set_cull": ([ctypes.c_int], None),
     "g2pc_accumulate": ([_c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i32, _c_void_p], ctypes.c_int),
     "g2pc_tiles_preprocess": ([_c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i32, _i64, _c_void_p, _c_void_p, _c_void_p,
                                _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
@@ -179,7 +180,7 @@ _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sor
                 "g2pc_orient_round": 5, "g2pc_orient_finish": 3}
 # host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",
-                "g2pc_multisplit_rows", "g2pc_blend_set_compact"}
+                "g2pc_multisplit_rows", "g2pc_blend_set_compact", "g2pc_blend_set_cull"}
 
 
 def call(name, *args):

@@ -11,8 +11,8 @@
  *   - every pointer is a DEVICE pointer unless the name ends in `_host`; the caller owns all memory,
  *     including scratch (sizes come from the *_bytes query functions or are stated in the comment);
  *   - every call is asynchronous on `stream` (a cudaStream_t passed as void*); no allocation, no host
- *     synchronisation and no global mutable state inside the library, except the blend footprint switch
- *     set by g2pc_blend_set_compact;
+ *     synchronisation and no global mutable state inside the library, except the blend switches
+ *     set by g2pc_blend_set_compact and g2pc_blend_set_cull;
  *   - return value: 0 = G2PC_OK, otherwise an error code; g2pc_last_error() gives a thread-local message;
  *   - no C++ exception crosses the ABI.
  */
@@ -456,6 +456,11 @@ int g2pc_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32
 /* Pixel-to-thread mapping of g2pc_blend: 1 (default) = a warp owns a compact block of <= 32 quads (e.g. 20 x 6 pixels),
  * 0 = a warp owns a strip of full rows.  Results do not depend on it up to the t_stop tolerance. */
 void g2pc_blend_set_compact(int on);
+
+/* Footprint cull of g2pc_blend: 1 (default) = when t_stop > FLT_MIN, a warp skips the Gaussians whose alpha is below
+ * eps = min(2^-26, t_stop / list length) over its whole pixel rectangle (transmittance bit-identical, each pixel's colour
+ * moves by < t_stop x max |colour|); 0 = never.  t_stop = 0 (FLT_MIN) never culls. */
+void g2pc_blend_set_cull(int on);
 
 /* S6.  Fold one camera into the per-Gaussian accumulators (gauss_render.py:387-395; the role of
  * GaussianRasterizer.update_max_contributions, gaussian_pointcloud_rasterization/__init__.py:142-152):
