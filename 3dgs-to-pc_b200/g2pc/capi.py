@@ -69,6 +69,31 @@ SIGNATURES = {
     "g2pc_mesh_normals_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
     "g2pc_mesh_normals": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
                           ctypes.c_int),
+    "g2pc_mesh_band_bricks_workspace_bytes": ([_i32], ctypes.c_int64),
+    "g2pc_mesh_band_bricks": ([_c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                               _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_list": ([_c_void_p, _i32, _c_void_p, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_splat": ([_c_void_p, _c_void_p, ctypes.c_int, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _i64,
+                              _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_ghosts": ([_c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
+                               _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_cg_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_mesh_band_cg_start": ([_c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64,
+                                 _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_cg_step": ([_c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p,
+                                _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_iso_workspace_bytes": ([], ctypes.c_int64),
+    "g2pc_mesh_band_iso": ([_c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                            _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_extract_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_mesh_band_extract_count": ([_c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
+                                      _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_band_extract_emit": ([_c_void_p, _i32, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64,
+                                     _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p],
+                                    ctypes.c_int),
+    "g2pc_mesh_band_gather_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_mesh_band_gather": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p, _i64,
+                               _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_orient_prepare_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_orient_prepare": ([_c_void_p, _c_void_p, ctypes.c_int, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                              _c_void_p, _i64, _c_void_p], ctypes.c_int),
@@ -176,7 +201,10 @@ TIMING = None     # None, or a dict filled as {entry point name: [(start_event, 
 _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
                 "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_knn_ids": 6, "g2pc_sor_mask": 5, "g2pc_mesh_splat": 5,
                 "g2pc_mesh_iso": 7, "g2pc_mesh_extract_count": 2, "g2pc_mesh_extract_emit": 2, "g2pc_mesh_gather": 3,
-                "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
+                "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3, "g2pc_mesh_band_bricks": 4, "g2pc_mesh_band_cg_start": 4,
+                "g2pc_mesh_band_cg_step": 6,
+                "g2pc_mesh_band_iso": 4, "g2pc_mesh_band_extract_count": 2, "g2pc_mesh_band_extract_emit": 2,
+                "g2pc_mesh_band_gather": 2, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
                 "g2pc_orient_round": 5, "g2pc_orient_finish": 3}
 # host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",

@@ -6,6 +6,11 @@ Steps: statistical outlier removal (g2pc/outliers.py) -> g2pc_mesh_splat -> g2pc
 cycles -> g2pc_mesh_iso -> g2pc_mesh_extract_count / _emit (marching tetrahedra) -> g2pc_mesh_gather (density, colour)
 -> g2pc_mesh_trim -> g2pc_mesh_smooth -> g2pc_mesh_normals.  Host reads: the frame and skip counts after the splat, the
 residual once per cycle, the vertex / triangle counts before and after the trim.
+
+With band_depth (N6b, s12_mesh_band.cu): after the dense solve and iso, per level depth + 1 .. band_depth
+g2pc_mesh_band_bricks (host reads the brick count) -> _list -> memory check -> _splat -> _ghosts -> _cg until
+|r| <= 1e-6 |b| (one host read per iteration); then g2pc_mesh_band_iso / _extract_count / _extract_emit / _gather at
+band_depth and the same trim, smoothing and normals.
 """
 import collections
 import math
@@ -17,6 +22,18 @@ import torch
 from . import capi, outliers
 
 DEPTH_MIN, DEPTH_MAX = 2, 10  # G2PC_MESH_DEPTH_MAX in include/g2pc.h
+BAND_DEPTH_MAX = 12  # G2PC_MESH_BAND_DEPTH_MAX
+BRICK = 8  # G2PC_MESH_BRICK: nodes per brick edge
+BAND_MARGIN = 1  # G2PC_MESH_BAND_MARGIN: bricks of band around the seed bricks
+CG_WORDS = 5  # G2PC_MESH_CG_WORDS
+MAX_CG_ITERATIONS = 2000
+# The band solve stops 10x below the dense target: conjugate gradients leave their error in smooth modes, where
+# |r| / |b| = 1e-5 still lets chi move by up to 2.4e-4 of its range (DESIGN.md §2, N6b).
+BAND_TOLERANCE = 1e-6
+# new device bytes per band node: B, chi, rhs while the ghosts are formed, then chi, rhs and the CG vectors r, p, q;
+# with return_debug B, the ghost sums and a copy of the initial chi stay alive as well
+BAND_BYTES_PER_NODE = max(8 + 4 + 4, 4 + 4 + 12)
+BAND_DEBUG_BYTES_PER_NODE = 8 + 8 + 4 + 4 + 4 + 12
 FRAME_WORDS = 8
 MAX_CYCLES = 40
 TOLERANCE = 1e-5
@@ -148,18 +165,162 @@ def vertex_normals(vpos, faces):
     return v, nrm
 
 
+def band_bricks(pts, cell, frame, depth, parent_map):
+    """Level `depth` of the band: band frame (8,) float64, brick map (NB^3,) int32, brick list (k,) int32, and the
+    count of seed bricks the nesting rule dropped.  Reads the counts once."""
+    dev, n, NB = pts.device, pts.shape[0], 1 << (depth - 3)
+    bframe = torch.empty((FRAME_WORDS,), dtype=torch.float64, device=dev)
+    bmap = torch.empty((NB ** 3,), dtype=torch.int32, device=dev)
+    counts = torch.empty((2,), dtype=torch.int64, device=dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_band_bricks_workspace_bytes(depth), dev)
+    st = capi.stream_ptr(dev)
+    capi.call("g2pc_mesh_band_bricks", capi.ptr(pts), capi.ptr(cell), n, capi.ptr(frame), depth, capi.ptr(parent_map),
+              capi.ptr(bframe), capi.ptr(bmap), capi.ptr(counts), capi.ptr(ws), ws.numel(), st)
+    del ws
+    k, lost = counts.tolist()
+    blist = torch.empty((k,), dtype=torch.int32, device=dev)
+    if k:
+        capi.call("g2pc_mesh_band_list", capi.ptr(bmap), depth, capi.ptr(blist), st)
+    return bframe, bmap, blist, lost
+
+
+def band_splat(pts, nrm, cell, bframe, depth, bmap, nbricks):
+    """B (nbricks * 512,) int64 on band storage, and the count of terms that fell outside the band (0 when nested)."""
+    dev = pts.device
+    B = torch.empty((nbricks * BRICK ** 3,), dtype=torch.int64, device=dev)
+    status = torch.empty((1,), dtype=torch.int32, device=dev)
+    capi.call("g2pc_mesh_band_splat", capi.ptr(pts), capi.ptr(nrm), capi.dtype_code(nrm), capi.ptr(cell),
+              pts.shape[0], capi.ptr(bframe), depth, capi.ptr(bmap), nbricks, capi.ptr(B), capi.ptr(status),
+              capi.stream_ptr(dev))
+    return B, status
+
+
+def band_ghosts(parent_chi, parent_map, depth, bmap, blist, B, bframe, with_ghosts=False):
+    """(ghost sums (float64, None unless with_ghosts), initial chi (float32), right-hand side (float32)) per band node."""
+    dev, nodes = B.device, B.shape[0]
+    ghost = torch.empty((nodes,), dtype=torch.float64, device=dev) if with_ghosts else None
+    chi = torch.empty((nodes,), dtype=torch.float32, device=dev)
+    rhs = torch.empty((nodes,), dtype=torch.float32, device=dev)
+    capi.call("g2pc_mesh_band_ghosts", capi.ptr(parent_chi), capi.ptr(parent_map), depth, capi.ptr(bmap),
+              capi.ptr(blist), blist.shape[0], capi.ptr(B), capi.ptr(bframe), capi.ptr(ghost), capi.ptr(chi),
+              capi.ptr(rhs), capi.stream_ptr(dev))
+    return ghost, chi, rhs
+
+
+def band_solve(rhs, chi, depth, bmap, blist, max_iterations=MAX_CG_ITERATIONS, tol=BAND_TOLERANCE):
+    """Jacobi-preconditioned CG on chi (in place): (iterations, |r| / |rhs|).  One host read per iteration.  When the
+    recurrence says the target is met, the residual is recomputed from chi (a restart) and the solve continues if the
+    recomputed one is above it."""
+    dev = rhs.device
+    sc = torch.zeros((CG_WORDS,), dtype=torch.float64, device=dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_band_cg_workspace_bytes(blist.shape[0]), dev)
+    st = capi.stream_ptr(dev)
+    args = (capi.ptr(rhs), depth, capi.ptr(bmap), capi.ptr(blist), blist.shape[0], capi.ptr(chi))
+    tail = (capi.ptr(sc), capi.ptr(ws), ws.numel(), st)
+    total, it, ratio, cc = 0, 0, 0.0, None
+    while True:
+        if it == 0:
+            capi.call("g2pc_mesh_band_cg_start", *args, *tail)
+        else:
+            capi.call("g2pc_mesh_band_cg_step", *args, it, *tail)
+        c2, _, rr = sc[:3].tolist()
+        cc = c2 if cc is None else cc
+        if cc == 0.0:
+            return total, 0.0
+        ratio = math.sqrt(rr / cc)
+        if ratio <= tol and it > 0:
+            it = 0  # confirm with a fresh residual
+            continue
+        if ratio <= tol or total >= max_iterations:
+            return total, ratio
+        it += 1
+        total += 1
+
+
+def band_iso(pts, cell, bframe, depth, bmap, chi):
+    dev = pts.device
+    iso = torch.empty((3,), dtype=torch.float64, device=dev)
+    ws = capi.workspace(capi.load().g2pc_mesh_band_iso_workspace_bytes(), dev)
+    capi.call("g2pc_mesh_band_iso", capi.ptr(pts), capi.ptr(cell), pts.shape[0], capi.ptr(bframe), depth,
+              capi.ptr(bmap), capi.ptr(chi), capi.ptr(iso), capi.ptr(ws), ws.numel(), capi.stream_ptr(dev))
+    return iso
+
+
+def band_extract(chi, depth, bmap, blist, bframe, iso, smoothing=False):
+    """Marching tetrahedra over the covered cubes of the band: vkey, vt, vpos, faces as extract().  smoothing: the
+    mesh goes on to g2pc_mesh_smooth, whose one-ring lists hold 6 entries per triangle in int32."""
+    dev, k = chi.device, blist.shape[0]
+    ws = capi.workspace(capi.load().g2pc_mesh_band_extract_workspace_bytes(k), dev)
+    counts = torch.empty((2,), dtype=torch.int64, device=dev)
+    st = capi.stream_ptr(dev)
+    capi.call("g2pc_mesh_band_extract_count", capi.ptr(chi), depth, capi.ptr(bmap), capi.ptr(blist), k, capi.ptr(iso),
+              capi.ptr(counts), capi.ptr(ws), ws.numel(), st)
+    m, t = counts.tolist()
+    if m >= 2 ** 31 - 1 or 3 * t >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the surface at band_depth {depth} has {m} vertices and {t} triangles: more than int32 "
+                             f"indices can address; use a smaller band_depth")
+    if smoothing and 6 * t >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the surface at band_depth {depth} has {t} triangles: the Laplacian smoothing's one-ring "
+                             f"lists (6 per triangle) exceed int32; use a smaller band_depth or laplacian_iters=0")
+    # extraction scratch and mesh, then the larger of the trim's and the smoothing's buffers
+    check_memory(5 * chi.shape[0] + 40 * m + 12 * t + max(52 * m + 20 * t, 96 * t + 24 * m), dev,
+                 f"the band surface at depth {depth} ({m} vertices, {t} triangles)")
+    vkey = torch.empty((m,), dtype=torch.int64, device=dev)
+    vt = torch.empty((m,), dtype=torch.float64, device=dev)
+    vpos = torch.empty((m, 3), dtype=torch.float64, device=dev)
+    faces = torch.empty((t, 3), dtype=torch.int32, device=dev)
+    if m:
+        scratch = torch.empty((5 * chi.shape[0],), dtype=torch.uint8, device=dev)
+        capi.call("g2pc_mesh_band_extract_emit", capi.ptr(chi), depth, capi.ptr(bmap), capi.ptr(blist), k,
+                  capi.ptr(bframe), capi.ptr(iso), capi.ptr(scratch), scratch.numel(), capi.ptr(ws), ws.numel(),
+                  capi.ptr(vkey), capi.ptr(vt), capi.ptr(vpos), capi.ptr(faces), st)
+    return vkey, vt, vpos, faces
+
+
+def band_gather(points, colours, cell, bframe, depth, vkey, vt):
+    """gather() at a band level (int64 dual cells)."""
+    dev, n, m = points.device, points.shape[0], vkey.shape[0]
+    dens = torch.empty((m,), dtype=torch.float64, device=dev)
+    vcol = torch.empty((m, 3), dtype=torch.uint8, device=dev) if colours is not None else None
+    ws = capi.workspace(capi.load().g2pc_mesh_band_gather_workspace_bytes(n), dev)
+    capi.call("g2pc_mesh_band_gather", capi.ptr(points), capi.ptr(colours), capi.ptr(cell), n, capi.ptr(bframe), depth,
+              capi.ptr(vkey), capi.ptr(vt), m, capi.ptr(dens), capi.ptr(vcol), capi.ptr(ws), ws.numel(),
+              capi.stream_ptr(dev))
+    return dens, vcol
+
+
+def check_memory(need, dev, what):
+    """Raises G2pcError when `what` needs more than the device's free bytes (after emptying PyTorch's cache)."""
+    torch.cuda.empty_cache()
+    free, _ = torch.cuda.mem_get_info(dev)
+    if need > free:
+        raise capi.G2pcError(f"{what} needs {need} bytes, but only {free} bytes of device memory are free: use a "
+                             f"smaller band_depth")
+
+
 def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, std_ratio=3.0, return_debug=False,
-                 timings=None):
+                 timings=None, band_depth=None, band_stats=None):
     """Mesh of an oriented point cloud.  points (n,3) float32 CUDA; normals (n,3) float32 / float64 (outward for an
     outward-facing mesh); colours (n,3) in 0..255 or None.  Returns Mesh(vertices (m,3) float32, faces (t,3) int32,
     colours (m,3) uint8 or None, normals (m,3) float32, densities (m,) float64).  With return_debug also a dict: chi
     (R^3 float32, mean-free), iso, B (R^3 int64), frame, cycles, ratio (final |r| / |b|), skipped (points whose normal is
     zero or not finite), keep (vertex trim mask), threshold.  `timings`: a dict that receives CUDA event pairs per phase
-    (clean, splat, solve, extract, gather_trim, smooth, normals)."""
+    (clean, splat, solve, extract, gather_trim, smooth, normals).
+
+    band_depth: None meshes the dense level `depth`.  An integer in depth + 1 .. 12 adds the narrow-band levels
+    depth + 1 .. band_depth (DESIGN.md §2, N6b: bricks of 8^3 nodes around the points, boundary values from the level
+    below) and extracts the mesh at band_depth; depth 10 with band_depth 12 is the reference's Poisson depth 12.  Its
+    debug dict adds "levels": one dict per band level (depth, frame, map, bricks, B, ghost, chi0, rhs, chi, iterations,
+    ratio), and chi / iso are those of band_depth ("dense_chi", "dense_iso" the dense level's); its timings add
+    band<D>_bricks, band<D>_splat, band<D>_solve per level.  band_stats: a list that receives one dict per band level
+    (depth, bricks, nodes, iterations, ratio: host values), with or without return_debug."""
     capi.check_cloud(points, normals, colours, what="Poisson meshing")
     if int(depth) != depth or not DEPTH_MIN <= depth <= DEPTH_MAX:
         raise capi.G2pcError(f"depth must be an integer in {DEPTH_MIN}..{DEPTH_MAX} (the dense int64 right-hand side "
                              f"alone is 69 GB at depth 11), got {depth}")
+    if band_depth is not None and (int(band_depth) != band_depth or not depth < band_depth <= BAND_DEPTH_MAX):
+        raise capi.G2pcError(f"band_depth must be None or an integer in {int(depth) + 1}..{BAND_DEPTH_MAX}, got "
+                             f"{band_depth}")
     if int(laplacian_iters) != laplacian_iters or laplacian_iters < 0:
         raise capi.G2pcError(f"laplacian_iters must be an integer >= 0, got {laplacian_iters}")
     if points.shape[0] == 0:
@@ -190,6 +351,12 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     debug = {}
     if return_debug:
         debug = {"B": B.clone(), "frame": frame, "cycles": cycles, "ratio": ratio, "skipped": skipped}
+    if band_depth is not None:
+        del B
+        dense = {"chi": chi}  # handed over, so that the band levels can free it
+        del chi
+        return _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, int(band_depth), laplacian_iters, debug,
+                          return_debug, timings, band_stats)
     with capi.phase(timings, "extract"):
         # B is dead after the solve: its memory holds the node lists of the extraction and the cell lists of the gather
         vkey, vt, vpos, faces = extract(chi, depth, frame, iso, B)
@@ -205,6 +372,73 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     out = Mesh(v, faces, vcol, vn, dens)
     if return_debug:
         debug.update(chi=chi, iso=iso, keep=keep, threshold=thr, vkey=vkey, vpos_smoothed=vpos)
+        return out, debug
+    return out
+
+
+def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, laplacian_iters, debug, return_debug,
+               timings, band_stats):
+    """The band levels depth + 1 .. band_depth after the dense solve, then the mesh at band_depth.  dense: {"chi": the
+    dense level's chi}, emptied here."""
+    dev = pts.device
+    parent_chi, parent_map = dense.pop("chi"), None
+    if return_debug:
+        debug.update(dense_chi=parent_chi, dense_iso=iso, levels=[])
+    for D in range(depth + 1, band_depth + 1):
+        with capi.phase(timings, f"band{D}_bricks"):
+            bframe, bmap, blist, lost = band_bricks(pts, cell, frame, D, parent_map)
+        k = blist.shape[0]
+        if lost:
+            raise capi.G2pcError(f"{lost} seed brick(s) at depth {D} are not nested in the level below")
+        if k == (1 << (D - 3)) ** 3:
+            raise capi.G2pcError(f"the band at depth {D} covers the whole grid (no boundary): mesh at a dense depth "
+                                 f"of at least {D} instead")
+        check_memory(k * BRICK ** 3 * (BAND_DEBUG_BYTES_PER_NODE if return_debug else BAND_BYTES_PER_NODE), dev,
+                     f"the band at depth {D} ({k} bricks, {k * BRICK ** 3} nodes)")
+        with capi.phase(timings, f"band{D}_splat"):
+            B, status = band_splat(pts, nrm, cell, bframe, D, bmap, k)
+            ghost, bchi, rhs = band_ghosts(parent_chi, parent_map, D, bmap, blist, B, bframe, with_ghosts=return_debug)
+        outside = int(status.item())
+        if outside:
+            raise capi.G2pcError(f"{outside} splat term(s) at depth {D} fall outside the band")
+        parent_chi = parent_map = None  # the level below is dead once the ghosts are known
+        level = {"depth": D, "frame": bframe, "map": bmap, "bricks": blist}
+        if return_debug:
+            level.update(B=B, ghost=ghost, chi0=bchi.clone(), rhs=rhs)
+        del B, ghost
+        with capi.phase(timings, f"band{D}_solve"):
+            its, ratio = band_solve(rhs, bchi, D, bmap, blist)
+        del rhs
+        if ratio > BAND_TOLERANCE:
+            warnings.warn(f"the band solve at depth {D} stopped after {its} iterations at |r| / |b| = {ratio:.2e}, "
+                          f"above the {BAND_TOLERANCE:g} target: the surface may be displaced", RuntimeWarning,
+                          stacklevel=3)
+        level.update(chi=bchi, iterations=its, ratio=ratio, nodes=k * BRICK ** 3)
+        if band_stats is not None:
+            band_stats.append({"depth": D, "bricks": k, "nodes": k * BRICK ** 3, "iterations": its, "ratio": ratio})
+        if return_debug:
+            debug["levels"].append(level)
+        parent_chi, parent_map = bchi, bmap
+    with capi.phase(timings, "extract"):
+        biso = band_iso(pts, cell, bframe, band_depth, bmap, bchi)
+        vkey, vt, vpos, faces = band_extract(bchi, band_depth, bmap, blist, bframe, biso,
+                                             smoothing=laplacian_iters > 0)
+    if vkey.shape[0] == 0:
+        raise capi.G2pcError("no surface: the indicator function does not cross its iso-value in the band")
+    if not return_debug:
+        del bchi, bmap, blist, parent_chi, parent_map
+    with capi.phase(timings, "gather_trim"):
+        dens, vcol = band_gather(pts, cols.to(torch.int32) if cols is not None else None, cell, bframe, band_depth,
+                                 vkey, vt)
+        dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
+    with capi.phase(timings, "smooth"):
+        smooth(vpos, faces, laplacian_iters)
+    with capi.phase(timings, "normals"):
+        v, vn = vertex_normals(vpos, faces)
+    out = Mesh(v, faces, vcol, vn, dens)
+    if return_debug:
+        debug.update(chi=bchi, iso=biso, keep=keep, threshold=thr, vkey=vkey, vpos_smoothed=vpos, cell=cell,
+                     points=pts, normals=nrm, colours=cols)
         return out, debug
     return out
 

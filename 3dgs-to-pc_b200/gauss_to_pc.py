@@ -431,7 +431,8 @@ def config_parser(argv=None, mesh=False):
 
     mesh=True parses for gauss_to_mesh.py: --generate_mesh is implied and meshes with this project's GPU mesher
     (g2pc/mesh.py) instead of Open3D, which needs renderer_type cuda, a depth in mesh.DEPTH_MIN..DEPTH_MAX and
-    laplacian_iterations >= 0."""
+    laplacian_iterations >= 0.  It also adds --band_depth (narrow-band levels above --poisson_depth, up to
+    mesh.BAND_DEPTH_MAX; --poisson_depth 10 --band_depth 12 is the reference's depth 12)."""
     try:
         import configargparse as ap
     except ImportError:
@@ -465,6 +466,11 @@ def config_parser(argv=None, mesh=False):
     parser.add_argument("--cull_gaussian_sizes", type=float, default=0.0, help="Percentage of gaussians to remove from largest to smallest")
     parser.add_argument("--max_sh_degree", type=int, default=3, help="Spherical-harmonics degree of the loaded point cloud")
     parser.add_argument("--quiet", action="store_true", help="Suppress output")
+    if mesh:
+        parser.add_argument("--band_depth", default=None, type=int,
+                            help="Mesh at this depth (poisson_depth + 1 .. 12), solving the levels above poisson_depth "
+                                 "only in a narrow band around the points; --poisson_depth 10 --band_depth 12 is the "
+                                 "reference's depth 12")
 
     args = parser.parse_args(argv)
     if mesh:
@@ -476,6 +482,8 @@ def config_parser(argv=None, mesh=False):
             raise AttributeError(f"Poisson depth must be between {gmesh.DEPTH_MIN} and {gmesh.DEPTH_MAX}")
         if args.laplacian_iterations < 0:
             raise AttributeError("Laplacian iterations must be 0 or more")
+        if args.band_depth is not None and not args.poisson_depth < args.band_depth <= gmesh.BAND_DEPTH_MAX:
+            raise AttributeError(f"Band depth must be between {args.poisson_depth + 1} and {gmesh.BAND_DEPTH_MAX}")
 
     if args.min_opacity < 0 or args.min_opacity > 1:
         raise AttributeError("Minumum opacity must be between 0 and 1")
@@ -584,9 +592,11 @@ def main(argv=None, mesh=False):
         if not args.quiet:
             print(f"Turned the surface normals toward their cameras: {st.flipped} flipped, {st.unseen} unseen, "
                   f"{st.undecided} undecided")
-            print(f"Meshing {surface_point_cloud.points.shape[0]} surface points at depth {args.poisson_depth}")
+            band = f" with a band to depth {args.band_depth}" if args.band_depth is not None else ""
+            print(f"Meshing {surface_point_cloud.points.shape[0]} surface points at depth {args.poisson_depth}{band}")
         m = gmesh.poisson_mesh(surface_point_cloud.points, surface_point_cloud.normals, surface_point_cloud.colours,
-                               depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations, std_ratio=3.0)
+                               depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations, std_ratio=3.0,
+                               band_depth=args.band_depth)
         gmesh.write_mesh_ply(args.mesh_output_path, m)
         if not args.quiet:
             print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")

@@ -1,13 +1,14 @@
 """Mesh an existing point cloud on the GPU: Poisson reconstruction with a multigrid solve, marching tetrahedra, density
 trim and Laplacian smoothing (g2pc/mesh.py).
 
-    python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10]
+    python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10] [--band_depth 12]
                       [--laplacian_iterations 10] [--orient_normals] [--quiet]
 
 The cloud must carry normals (nx ny nz), as gauss_to_pc.py writes them by default; its colours (red green blue) are
 carried over to the mesh's vertices.  A mesh faces the way its normals point.  By default the normals are used as they
 are; --orient_normals first gives them a consistent sign (g2pc/orient.py, k = 10), which the normals of a cloud sampled
-from Gaussians lack: each takes its sign from its Gaussian's rotation."""
+from Gaussians lack: each takes its sign from its Gaussian's rotation.  --band_depth adds finer levels stored only in a narrow band around the points:
+--poisson_depth 10 --band_depth 12 is the reference's Poisson depth 12."""
 import argparse
 import time
 
@@ -38,11 +39,18 @@ def config_parser(argv=None):
     p.add_argument("--mesh_output_path", default="mesh.ply", help="output mesh PLY")
     p.add_argument("--poisson_depth", type=_depth, default=10,
                    help=f"grid of 2^depth nodes per axis, {mesh.DEPTH_MIN}..{mesh.DEPTH_MAX}")
+    p.add_argument("--band_depth", type=int, default=None,
+                   help=f"mesh at this depth, poisson_depth + 1 .. {mesh.BAND_DEPTH_MAX}, solving the levels above "
+                        f"poisson_depth only in a narrow band around the points (--poisson_depth 10 --band_depth 12 is "
+                        f"the reference's depth 12); default: mesh at poisson_depth")
     p.add_argument("--laplacian_iterations", type=_iterations, default=10, help="Laplacian smoothing steps (0: none)")
     p.add_argument("--orient_normals", action="store_true",
                    help=f"orient the normals consistently (k = {orient.K_DEFAULT} nearest neighbours) before meshing")
     p.add_argument("--quiet", action="store_true", help="print nothing")
-    return p.parse_args(argv)
+    args = p.parse_args(argv)
+    if args.band_depth is not None and not args.poisson_depth < args.band_depth <= mesh.BAND_DEPTH_MAX:
+        p.error(f"--band_depth must be in {args.poisson_depth + 1}..{mesh.BAND_DEPTH_MAX}")
+    return args
 
 
 def load_cloud(path, device="cuda:0"):
@@ -62,12 +70,14 @@ def main(argv=None):
     t0 = time.perf_counter()
     points, normals, colours = load_cloud(args.input_path)
     if not args.quiet:
-        print(f"Meshing {points.shape[0]} points at depth {args.poisson_depth}")
+        band = f" with a band to depth {args.band_depth}" if args.band_depth is not None else ""
+        print(f"Meshing {points.shape[0]} points at depth {args.poisson_depth}{band}")
     if args.orient_normals:
         normals, st = orient.orient_normals(points, normals, k=orient.K_DEFAULT)
         if not args.quiet:
             print(f"Oriented the normals: {st.flipped} flipped, {st.components} component(s), {st.skipped} skipped")
-    m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations)
+    m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations,
+                          band_depth=args.band_depth)
     mesh.write_mesh_ply(args.mesh_output_path, m)
     if not args.quiet:
         print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path} "

@@ -267,6 +267,72 @@ int64_t g2pc_mesh_normals_workspace_bytes(int64_t m, int64_t t);
 int g2pc_mesh_normals(const double* vpos, int64_t m, const int32_t* faces, int64_t t, float* vertices, float* normals,
                       void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- N6b: narrow-band levels of the Poisson mesh (s12_mesh_band.cu, g2pc/mesh.py band_depth) ------------------- */
+/* One or two levels D = depth + 1 .. G2PC_MESH_BAND_DEPTH_MAX above the dense solve, stored only in bricks of
+ * G2PC_MESH_BRICK^3 nodes within G2PC_MESH_BAND_MARGIN bricks of the points (rules in DESIGN.md §2, N6b).  Level D:
+ * R = 2^D, NB = R / 8 bricks per axis, brick map (NB^3 int32: slot or -1; slots in ascending linear brick index), brick
+ * list (slot -> brick), node storage slot * 512 + (lz * 8 + ly) * 8 + lx.  parent_map / parent_chi: the level below
+ * (parent_map NULL: the dense level, chi mean-free after g2pc_mesh_iso).  Order of calls per level: bricks (host reads
+ * counts) -> list -> splat -> ghosts -> cg_start, then cg_step 1, 2, ... (one host read of scalars per call); at the
+ * finest level: iso -> extract_count -> extract_emit -> gather, then g2pc_mesh_trim / _smooth / _normals. */
+#define G2PC_MESH_BAND_DEPTH_MAX 12
+#define G2PC_MESH_BRICK 8
+#define G2PC_MESH_BAND_MARGIN 1
+#define G2PC_MESH_CG_WORDS 5 /* float64: |c|^2, p.q, |r|^2, r.z (two slots) */
+
+/* band_frame (G2PC_MESH_FRAME_WORDS): the dense frame with h = L / R and R of level D.  map: NB^3 int32.  counts
+ * (2 int64): active bricks, seed bricks lost to the nesting rule (must be 0).  cell: the dense splat's cell (its
+ * CELL_NONE marks the points that are not splatted).  workspace: g2pc_mesh_band_bricks_workspace_bytes(depth). */
+int64_t g2pc_mesh_band_bricks_workspace_bytes(int32_t depth);
+int g2pc_mesh_band_bricks(const float* xyz, const uint32_t* cell, int64_t n, const double* frame, int32_t depth,
+                          const int32_t* parent_map, double* band_frame, int32_t* map, int64_t* counts, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+/* list: counts[0] int32, slot -> linear brick index. */
+int g2pc_mesh_band_list(const int32_t* map, int32_t depth, int32_t* list, void* stream);
+/* B (nbricks * 512 int64, zeroed here): the dense splat's terms at level D on band storage.  status (1 int32): terms
+ * whose node is not in the band (0 when the nesting rule held). */
+int g2pc_mesh_band_splat(const float* xyz, const void* normals, int normal_dtype, const uint32_t* cell, int64_t n,
+                         const double* band_frame, int32_t depth, const int32_t* map, int64_t nbricks, int64_t* B,
+                         int32_t* status, void* stream);
+/* Per band node: ghost (float64, may be NULL) = sum of s P(parent chi) over the in-grid neighbours outside the band,
+ * chi = s P(parent chi) (the initial guess), rhs = (float)(ghost - B h 2^-33), s = 1/8. */
+int g2pc_mesh_band_ghosts(const float* parent_chi, const int32_t* parent_map, int32_t depth, const int32_t* map,
+                          const int32_t* list, int64_t nbricks, const int64_t* B, const double* band_frame,
+                          double* ghost, float* chi, float* rhs, void* stream);
+/* Jacobi-preconditioned conjugate gradients on (count x chi - sum of the active in-grid neighbours) = rhs.  cg_start
+ * (re)starts from chi (residual from chi, direction = preconditioned residual); cg_step with iteration t = 1, 2, ...
+ * (counted from the last start) does one step.  scalars (G2PC_MESH_CG_WORDS float64): [0] |rhs|^2, [2] |r|^2 after
+ * either call.  workspace: g2pc_mesh_band_cg_workspace_bytes(nbricks), kept between the calls. */
+int64_t g2pc_mesh_band_cg_workspace_bytes(int64_t nbricks);
+int g2pc_mesh_band_cg_start(const float* rhs, int32_t depth, const int32_t* map, const int32_t* list, int64_t nbricks,
+                            float* chi, double* scalars, void* workspace, int64_t workspace_bytes, void* stream);
+int g2pc_mesh_band_cg_step(const float* rhs, int32_t depth, const int32_t* map, const int32_t* list, int64_t nbricks,
+                           float* chi, int32_t iteration, double* scalars, void* workspace, int64_t workspace_bytes,
+                           void* stream);
+/* iso (3 float64): 0, mean of trilinear chi over the splatted points, their count.  workspace:
+ * g2pc_mesh_band_iso_workspace_bytes(). */
+int64_t g2pc_mesh_band_iso_workspace_bytes(void);
+int g2pc_mesh_band_iso(const float* xyz, const uint32_t* cell, int64_t n, const double* band_frame, int32_t depth,
+                       const int32_t* map, const float* chi, double* iso, void* workspace, int64_t workspace_bytes,
+                       void* stream);
+/* Marching tetrahedra over the cubes whose 8 corners are in the band; keys node * 8 + d (global node, int64); vertices
+ * in ascending (storage index, d), triangles in ascending (storage index of the cube, tetrahedron, triangle).
+ * node_scratch: 5 bytes per band node.  workspace: g2pc_mesh_band_extract_workspace_bytes(nbricks). */
+int64_t g2pc_mesh_band_extract_workspace_bytes(int64_t nbricks);
+int g2pc_mesh_band_extract_count(const float* chi, int32_t depth, const int32_t* map, const int32_t* list,
+                                 int64_t nbricks, const double* iso, int64_t* counts, void* workspace,
+                                 int64_t workspace_bytes, void* stream);
+int g2pc_mesh_band_extract_emit(const float* chi, int32_t depth, const int32_t* map, const int32_t* list,
+                                int64_t nbricks, const double* band_frame, const double* iso, void* node_scratch,
+                                int64_t node_scratch_bytes, const void* workspace, int64_t workspace_bytes,
+                                int64_t* vkey, double* vt, double* vpos, int32_t* faces, void* stream);
+/* g2pc_mesh_gather at level D with int64 dual cells (no dense cell table).  workspace:
+ * g2pc_mesh_band_gather_workspace_bytes(n). */
+int64_t g2pc_mesh_band_gather_workspace_bytes(int64_t n);
+int g2pc_mesh_band_gather(const float* xyz, const int32_t* colours, const uint32_t* cell, int64_t n,
+                          const double* band_frame, int32_t depth, const int64_t* vkey, const double* vt, int64_t m,
+                          double* density, uint8_t* vcolours, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- N7: consistent orientation of point-cloud normals (s11_orient.cu, g2pc/orient.py) -------------------------- */
 /* Hoppe et al. 1992 (the rule behind Open3D's orient_normals_consistent_tangent_plane) with this project's own rules
  * (DESIGN.md §2): k-NN graph, edge weight 1 - |n_i . n_j|, minimum spanning forest, sign propagated from one seed per
