@@ -1,6 +1,7 @@
-// mesh_common.cuh — device code the dense Poisson mesher (s10_mesh.cu) and its narrow-band levels
-// (s12_mesh_band.cu) share: the frame words, a point's dual cell and trilinear weights, the fixed-order float64
-// finish step, and the marching-tetrahedra tables.  Every kernel stays in an anonymous namespace.
+// mesh_common.cuh — device code the dense Poisson mesher (s10_mesh.cu), its narrow-band levels (s12_mesh_band.cu) and
+// the decimation (s13_decimate.cu) share: the frame words, a point's dual cell and trilinear weights, the fixed-order
+// float64 finish step, the marching-tetrahedra tables and the one-ring / incidence list builders.  Every kernel stays
+// in an anonymous namespace.
 #pragma once
 #include "cloud_common.cuh"
 
@@ -161,6 +162,41 @@ __device__ __forceinline__ int tet_triangles(int p, uint32_t inside, int (&tri)[
         }
     }
     return nt;
+}
+
+// ---- one-ring / incidence lists of a triangle mesh (smoothing and normals in s10_mesh.cu, s13_decimate.cu) --------
+// directed one-ring edges (u << 32 | v), both directions of every triangle edge
+__global__ void __launch_bounds__(MB) ring_keys_kernel(const int32_t* __restrict__ faces, int64_t t,
+                                                       unsigned long long* __restrict__ keys) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t) return;
+    for (int s = 0; s < 3; ++s) {
+        const unsigned long long a = (uint32_t)faces[3 * f + s], b = (uint32_t)faces[3 * f + (s + 1) % 3];
+        keys[6 * f + 2 * s] = a << 32 | b;
+        keys[6 * f + 2 * s + 1] = b << 32 | a;
+    }
+}
+
+// incident triangles (v << 32 | triangle)
+__global__ void __launch_bounds__(MB) incidence_keys_kernel(const int32_t* __restrict__ faces, int64_t t,
+                                                            unsigned long long* __restrict__ keys) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t) return;
+    for (int s = 0; s < 3; ++s) keys[3 * f + s] = (unsigned long long)(uint32_t)faces[3 * f + s] << 32 | (uint64_t)f;
+}
+
+// row[v] = first sorted key with high word >= v, for v = 0..m
+__global__ void __launch_bounds__(MB) row_kernel(const unsigned long long* __restrict__ keys, int64_t e, int64_t m,
+                                                 int32_t* __restrict__ row) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v > m) return;
+    const unsigned long long K = (unsigned long long)v << 32;
+    int64_t lo = 0, hi = e;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (keys[mid] < K) lo = mid + 1; else hi = mid;
+    }
+    row[v] = (int32_t)lo;
 }
 
 }  // namespace

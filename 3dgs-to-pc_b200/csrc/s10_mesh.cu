@@ -530,41 +530,7 @@ __global__ void trim_counts_kernel(const int32_t* __restrict__ flag, const int32
     counts[1] = t ? (long long)tmap[t - 1] + tflag[t - 1] : 0;
 }
 
-// ---- one-ring / incidence lists, smoothing, normals ----------------------------------------------------------------
-// directed one-ring edges (u << 32 | v), both directions of every triangle edge
-__global__ void __launch_bounds__(MB) ring_keys_kernel(const int32_t* __restrict__ faces, int64_t t,
-                                                       unsigned long long* __restrict__ keys) {
-    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (f >= t) return;
-    for (int s = 0; s < 3; ++s) {
-        const unsigned long long a = (uint32_t)faces[3 * f + s], b = (uint32_t)faces[3 * f + (s + 1) % 3];
-        keys[6 * f + 2 * s] = a << 32 | b;
-        keys[6 * f + 2 * s + 1] = b << 32 | a;
-    }
-}
-
-// incident triangles (v << 32 | triangle)
-__global__ void __launch_bounds__(MB) incidence_keys_kernel(const int32_t* __restrict__ faces, int64_t t,
-                                                            unsigned long long* __restrict__ keys) {
-    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (f >= t) return;
-    for (int s = 0; s < 3; ++s) keys[3 * f + s] = (unsigned long long)(uint32_t)faces[3 * f + s] << 32 | (uint64_t)f;
-}
-
-// row[v] = first sorted key with high word >= v, for v = 0..m
-__global__ void __launch_bounds__(MB) row_kernel(const unsigned long long* __restrict__ keys, int64_t e, int64_t m,
-                                                 int32_t* __restrict__ row) {
-    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (v > m) return;
-    const unsigned long long K = (unsigned long long)v << 32;
-    int64_t lo = 0, hi = e;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (keys[mid] < K) lo = mid + 1; else hi = mid;
-    }
-    row[v] = (int32_t)lo;
-}
-
+// ---- smoothing, normals (their one-ring / incidence lists: mesh_common.cuh) ----------------------------------------
 // one Jacobi step, lambda = 1/2: v + (sum w_j v_j / sum w_j - v) / 2, w_j = 1 / (|v - v_j| + 1e-12), distinct
 // neighbours in ascending index
 __global__ void __launch_bounds__(MB) smooth_kernel(const double* __restrict__ p, int64_t m,

@@ -94,6 +94,19 @@ SIGNATURES = {
     "g2pc_mesh_band_gather_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_mesh_band_gather": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i32, _c_void_p, _c_void_p, _i64,
                                _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_decimate_prepare_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_mesh_decimate_prepare": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
+                                   ctypes.c_int),
+    "g2pc_mesh_decimate_round_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_mesh_decimate_select": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64,
+                                   _c_void_p], ctypes.c_int),
+    "g2pc_mesh_decimate_apply": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                  _c_void_p, _i64, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64,
+                                  _c_void_p], ctypes.c_int),
+    "g2pc_mesh_decimate_finish_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_mesh_decimate_finish": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                   _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
+                                  ctypes.c_int),
     "g2pc_orient_prepare_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_orient_prepare": ([_c_void_p, _c_void_p, ctypes.c_int, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                              _c_void_p, _i64, _c_void_p], ctypes.c_int),
@@ -204,7 +217,8 @@ _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sor
                 "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3, "g2pc_mesh_band_bricks": 4, "g2pc_mesh_band_cg_start": 4,
                 "g2pc_mesh_band_cg_step": 6,
                 "g2pc_mesh_band_iso": 4, "g2pc_mesh_band_extract_count": 2, "g2pc_mesh_band_extract_emit": 2,
-                "g2pc_mesh_band_gather": 2, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
+                "g2pc_mesh_band_gather": 2, "g2pc_mesh_decimate_prepare": 4, "g2pc_mesh_decimate_select": 8,
+                "g2pc_mesh_decimate_apply": 5, "g2pc_mesh_decimate_finish": 4, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
                 "g2pc_orient_round": 5, "g2pc_orient_finish": 3}
 # host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",

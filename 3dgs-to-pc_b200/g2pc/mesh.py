@@ -11,6 +11,9 @@ With band_depth (N6b, s12_mesh_band.cu): after the dense solve and iso, per leve
 g2pc_mesh_band_bricks (host reads the brick count) -> _list -> memory check -> _splat -> _ghosts -> _cg until
 |r| <= 1e-6 |b| (one host read per iteration); then g2pc_mesh_band_iso / _extract_count / _extract_emit / _gather at
 band_depth and the same trim, smoothing and normals.
+
+With target_triangles (N9, s13_decimate.cu): between the smoothing and the normals, decimate(): g2pc_mesh_decimate_prepare,
+then per round _select (host reads the counts) -> _apply until the target is met or nothing is selected, then _finish.
 """
 import collections
 import math
@@ -289,17 +292,151 @@ def band_gather(points, colours, cell, bframe, depth, vkey, vt):
     return dens, vcol
 
 
-def check_memory(need, dev, what):
+def check_memory(need, dev, what, remedy="use a smaller band_depth"):
     """Raises G2pcError when `what` needs more than the device's free bytes (after emptying PyTorch's cache)."""
     torch.cuda.empty_cache()
     free, _ = torch.cuda.mem_get_info(dev)
     if need > free:
-        raise capi.G2pcError(f"{what} needs {need} bytes, but only {free} bytes of device memory are free: use a "
-                             f"smaller band_depth")
+        raise capi.G2pcError(f"{what} needs {need} bytes, but only {free} bytes of device memory are free: {remedy}")
+
+
+def check_target(target_triangles):
+    """Refuses a triangle target that is not an integer >= 1 (bool included)."""
+    if isinstance(target_triangles, bool) or not isinstance(target_triangles, (int, np.integer)) or target_triangles < 1:
+        raise capi.G2pcError(f"target_triangles must be an integer >= 1, got {target_triangles!r}")
+
+
+def decimate(vpos, faces, target_triangles, colours=None, densities=None, return_debug=False, stats=None):
+    """Decimation by parallel quadric edge collapse (DESIGN.md §2, N9) to target_triangles or target_triangles - 1
+    triangles.  vpos (m,3) float64, faces (t,3) int32 (no face uses a vertex twice), colours (m,3) uint8 or None,
+    densities (m,) float64 or None, all CUDA.  Returns (vpos, faces, colours, densities) of the decimated mesh: the
+    surviving vertices in their order, a merged vertex with the rounded mean colour and the mean density of the original
+    vertices merged into it.  Boundary, non-manifold and unused vertices never move and are never removed.  When no edge
+    can collapse before the target is met, returns what was reached with a RuntimeWarning.  target_triangles >= t returns
+    the input tensors themselves and runs no kernel.
+
+    stats: a dict that receives rounds, collapses (per round) and reached (the target was met).  return_debug: also a
+    dict with quadrics and free (after the preparation) and rounds: per round a dict of edges, candidates, selected
+    (counts), keys (the applied keys, ascending) and ab (their survivor / removed vertex pairs), then vpos, quadrics,
+    colour_sums, merged, density_sums and faces after the round."""
+    check_target(target_triangles)
+    for name, x in (("vpos", vpos), ("faces", faces), ("colours", colours), ("densities", densities)):
+        if x is not None and not (torch.is_tensor(x) and x.is_cuda):
+            raise capi.G2pcError(f"{name} must be a CUDA tensor (the decimation has no CPU path)")
+    if vpos.dim() != 2 or vpos.shape[1] != 3 or vpos.dtype != torch.float64:
+        raise capi.G2pcError(f"vpos must be (m, 3) float64, got {tuple(vpos.shape)} {vpos.dtype}")
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype != torch.int32:
+        raise capi.G2pcError(f"faces must be (t, 3) int32, got {tuple(faces.shape)} {faces.dtype}")
+    m, t, dev = vpos.shape[0], faces.shape[0], vpos.device
+    if colours is not None and (colours.shape != (m, 3) or colours.dtype != torch.uint8):
+        raise capi.G2pcError(f"colours must be (m, 3) uint8, got {tuple(colours.shape)} {colours.dtype}")
+    if densities is not None and (densities.shape != (m,) or densities.dtype != torch.float64):
+        raise capi.G2pcError(f"densities must be (m,) float64, got {tuple(densities.shape)} {densities.dtype}")
+    if any(x is not None and x.device != dev for x in (faces, colours, densities)):
+        raise capi.G2pcError("vpos, faces, colours and densities must be on one device")
+    if m >= 2 ** 31 - 1 or 3 * t >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the mesh has {m} vertices and {t} triangles: more than the decimation's int32 lists "
+                             f"(3 entries per triangle) can hold")
+    if m and not bool(torch.isfinite(vpos).all()):
+        raise capi.G2pcError("a vertex position is not finite")
+    if t:
+        f = faces.long()
+        lo, hi, rep = torch.stack([f.min(), f.max(), ((f[:, 0] == f[:, 1]) | (f[:, 1] == f[:, 2]) |
+                                                       (f[:, 0] == f[:, 2])).sum()]).tolist()
+        del f
+        if lo < 0 or hi >= m:
+            raise capi.G2pcError(f"face indices must be in 0..{m - 1}, got {lo}..{hi}")
+        if rep:
+            raise capi.G2pcError(f"{rep} face(s) use a vertex twice")
+    target = int(target_triangles)
+    if target >= t:
+        if stats is not None:
+            stats.update(rounds=0, collapses=[], reached=True)
+        out = (vpos, faces, colours, densities)
+        return (out, {"rounds": []}) if return_debug else out
+    lib = capi.load()
+    round_bytes = lib.g2pc_mesh_decimate_round_workspace_bytes(m, t)
+    # positions, Q (80 B), flags, alive, merge counts, colour and density sums per vertex; two face buffers; the round
+    # workspace (sorted incidence and edge keys)
+    check_memory(m * (24 + 80 + 1 + 1 + 4 + 24 + 8) + 2 * 12 * t + round_bytes, dev,
+                 f"decimating {m} vertices and {t} triangles", remedy="decimate a smaller mesh")
+    st = capi.stream_ptr(dev)
+    p = vpos.clone()
+    Q = torch.empty((m, 10), dtype=torch.float64, device=dev)
+    free = torch.empty((m,), dtype=torch.uint8, device=dev)
+    ws = capi.workspace(lib.g2pc_mesh_decimate_prepare_workspace_bytes(m, t), dev)
+    capi.call("g2pc_mesh_decimate_prepare", capi.ptr(p), m, capi.ptr(faces), t, capi.ptr(Q), capi.ptr(free),
+              capi.ptr(ws), ws.numel(), st)
+    del ws
+    alive = torch.ones((m,), dtype=torch.uint8, device=dev)
+    merged = torch.ones((m,), dtype=torch.int32, device=dev)
+    csum = colours.to(torch.int64).contiguous() if colours is not None else None
+    dsum = densities.clone() if densities is not None else None
+    debug = {"quadrics": Q.clone(), "free": free.clone(), "rounds": []} if return_debug else None
+    ws = capi.workspace(round_bytes, dev)
+    counts = torch.zeros((4,), dtype=torch.int64, device=dev)  # edges, candidates, selected; faces kept by apply
+    bufs = [torch.empty_like(faces), torch.empty((max(t - 2, 1), 3), dtype=torch.int32, device=dev)]
+    cur, collapses = faces, []
+    while t > target:
+        capi.call("g2pc_mesh_decimate_select", capi.ptr(p), m, capi.ptr(cur), t, capi.ptr(Q), capi.ptr(free),
+                  capi.ptr(counts), capi.ptr(ws), ws.numel(), st)
+        E, C, S, kept = counts.tolist()
+        if collapses and kept != t:
+            raise capi.G2pcError(f"round {len(collapses)} kept {kept} triangles, expected {t}")
+        if S == 0:
+            warnings.warn(f"the decimation stopped at {t} triangles, above the target of {target}: no edge can "
+                          f"collapse (boundary, non-manifold or locked by the link and fold-over checks)",
+                          RuntimeWarning, stacklevel=2)
+            break
+        k = min(S, (t - target + 1) // 2)
+        nxt = bufs[len(collapses) % 2][:t - 2 * k]
+        keys = torch.empty((k,), dtype=torch.int64, device=dev) if return_debug else None
+        ab = torch.empty((k, 2), dtype=torch.int32, device=dev) if return_debug else None
+        capi.call("g2pc_mesh_decimate_apply", capi.ptr(p), m, capi.ptr(cur), t, capi.ptr(Q), capi.ptr(csum),
+                  capi.ptr(merged), capi.ptr(dsum), capi.ptr(alive), S, k, capi.ptr(nxt), capi.ptr(counts[3:]),
+                  capi.ptr(keys), capi.ptr(ab), capi.ptr(ws), ws.numel(), st)
+        t -= 2 * k
+        cur = nxt
+        collapses.append(k)
+        if return_debug:
+            debug["rounds"].append({"edges": E, "candidates": C, "selected": S, "keys": keys, "ab": ab,
+                                    "vpos": p.clone(), "quadrics": Q.clone(), "merged": merged.clone(),
+                                    "colour_sums": csum.clone() if csum is not None else None,
+                                    "density_sums": dsum.clone() if dsum is not None else None,
+                                    "faces": nxt.clone()})
+    del ws
+    if stats is not None:
+        stats.update(rounds=len(collapses), collapses=collapses, reached=t <= target)
+    vout = torch.empty((m, 3), dtype=torch.float64, device=dev)
+    cout = torch.empty((m, 3), dtype=torch.uint8, device=dev) if colours is not None else None
+    dout = torch.empty((m,), dtype=torch.float64, device=dev) if densities is not None else None
+    fout = torch.empty((t, 3), dtype=torch.int32, device=dev)
+    fin = torch.empty((1,), dtype=torch.int64, device=dev)
+    ws = capi.workspace(lib.g2pc_mesh_decimate_finish_workspace_bytes(m), dev)
+    capi.call("g2pc_mesh_decimate_finish", capi.ptr(p), m, capi.ptr(cur), t, capi.ptr(alive), capi.ptr(csum),
+              capi.ptr(merged), capi.ptr(dsum), capi.ptr(vout), capi.ptr(cout), capi.ptr(dout), capi.ptr(fout),
+              capi.ptr(fin), capi.ptr(ws), ws.numel(), st)
+    mk = int(fin.item())
+    out = (vout[:mk], fout, cout[:mk] if cout is not None else None, dout[:mk] if dout is not None else None)
+    return (out, debug) if return_debug else out
+
+
+def decimate_mesh(mesh, target_triangles, stats=None):
+    """decimate() of a Mesh (its float32 vertices taken as float64), with the normals recomputed by vertex_normals.
+    A target of at least the mesh's triangle count returns the mesh itself."""
+    check_target(target_triangles)
+    if target_triangles >= mesh.faces.shape[0]:
+        if stats is not None:
+            stats.update(rounds=0, collapses=[], reached=True)
+        return mesh
+    vpos, faces, vcol, dens = decimate(mesh.vertices.to(torch.float64), mesh.faces.contiguous(), target_triangles,
+                                       mesh.colours, mesh.densities, stats=stats)
+    v, vn = vertex_normals(vpos, faces)
+    return Mesh(v, faces, vcol, vn, dens)
 
 
 def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, std_ratio=3.0, return_debug=False,
-                 timings=None, band_depth=None, band_stats=None):
+                 timings=None, band_depth=None, band_stats=None, target_triangles=None):
     """Mesh of an oriented point cloud.  points (n,3) float32 CUDA; normals (n,3) float32 / float64 (outward for an
     outward-facing mesh); colours (n,3) in 0..255 or None.  Returns Mesh(vertices (m,3) float32, faces (t,3) int32,
     colours (m,3) uint8 or None, normals (m,3) float32, densities (m,) float64).  With return_debug also a dict: chi
@@ -313,8 +450,14 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     debug dict adds "levels": one dict per band level (depth, frame, map, bricks, B, ghost, chi0, rhs, chi, iterations,
     ratio), and chi / iso are those of band_depth ("dense_chi", "dense_iso" the dense level's); its timings add
     band<D>_bricks, band<D>_splat, band<D>_solve per level.  band_stats: a list that receives one dict per band level
-    (depth, bricks, nodes, iterations, ratio: host values), with or without return_debug."""
+    (depth, bricks, nodes, iterations, ratio: host values), with or without return_debug.
+
+    target_triangles: None keeps every triangle.  An integer >= 1 decimates the smoothed mesh to target_triangles or
+    target_triangles - 1 triangles (decimate(), DESIGN.md §2, N9) before the normals are computed; timings add
+    "decimate"."""
     capi.check_cloud(points, normals, colours, what="Poisson meshing")
+    if target_triangles is not None:
+        check_target(target_triangles)
     if int(depth) != depth or not DEPTH_MIN <= depth <= DEPTH_MAX:
         raise capi.G2pcError(f"depth must be an integer in {DEPTH_MIN}..{DEPTH_MAX} (the dense int64 right-hand side "
                              f"alone is 69 GB at depth 11), got {depth}")
@@ -356,7 +499,7 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
         dense = {"chi": chi}  # handed over, so that the band levels can free it
         del chi
         return _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, int(band_depth), laplacian_iters, debug,
-                          return_debug, timings, band_stats)
+                          return_debug, timings, band_stats, target_triangles)
     with capi.phase(timings, "extract"):
         # B is dead after the solve: its memory holds the node lists of the extraction and the cell lists of the gather
         vkey, vt, vpos, faces = extract(chi, depth, frame, iso, B)
@@ -367,17 +510,21 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
         dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
     with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
+    smoothed = vpos
+    if target_triangles is not None:
+        with capi.phase(timings, "decimate"):
+            vpos, faces, vcol, dens = decimate(vpos, faces, target_triangles, vcol, dens)
     with capi.phase(timings, "normals"):
         v, vn = vertex_normals(vpos, faces)
     out = Mesh(v, faces, vcol, vn, dens)
     if return_debug:
-        debug.update(chi=chi, iso=iso, keep=keep, threshold=thr, vkey=vkey, vpos_smoothed=vpos)
+        debug.update(chi=chi, iso=iso, keep=keep, threshold=thr, vkey=vkey, vpos_smoothed=smoothed)
         return out, debug
     return out
 
 
 def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, laplacian_iters, debug, return_debug,
-               timings, band_stats):
+               timings, band_stats, target_triangles):
     """The band levels depth + 1 .. band_depth after the dense solve, then the mesh at band_depth.  dense: {"chi": the
     dense level's chi}, emptied here."""
     dev = pts.device
@@ -433,11 +580,15 @@ def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, lapla
         dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
     with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
+    smoothed = vpos
+    if target_triangles is not None:
+        with capi.phase(timings, "decimate"):
+            vpos, faces, vcol, dens = decimate(vpos, faces, target_triangles, vcol, dens)
     with capi.phase(timings, "normals"):
         v, vn = vertex_normals(vpos, faces)
     out = Mesh(v, faces, vcol, vn, dens)
     if return_debug:
-        debug.update(chi=bchi, iso=biso, keep=keep, threshold=thr, vkey=vkey, vpos_smoothed=vpos, cell=cell,
+        debug.update(chi=bchi, iso=biso, keep=keep, threshold=thr, vkey=vkey, vpos_smoothed=smoothed, cell=cell,
                      points=pts, normals=nrm, colours=cols)
         return out, debug
     return out

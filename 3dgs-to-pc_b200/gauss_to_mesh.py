@@ -2,12 +2,14 @@
 
     python gauss_to_mesh.py --input_path scene.ply --transform_path transforms.json [gauss_to_pc.py's flags]
                             [--mesh_output_path 3dgs_mesh.ply] [--poisson_depth 10] [--laplacian_iterations 10]
+                            [--band_depth D] [--target_triangles N]
 
 Same flags and validation as gauss_to_pc.py; it writes the same point cloud to --output_path.  Then, as the reference's
 mesh recipe does: the Gaussians on a predicted surface (surface distance below its mean) are sampled into a second cloud
 of min(num_points // 2, 25 * n_surface) points, whose normals are first turned toward the camera that saw each Gaussian
 best (g2pc.orient.face_cameras), and that cloud is meshed by g2pc/mesh.py (outlier removal k = 20, std_ratio 3, Poisson,
-10 % density trim, Laplacian smoothing) and written to --mesh_output_path.  Needs --renderer_type cuda and a depth in
+10 % density trim, Laplacian smoothing, and with --target_triangles a decimation to that many triangles) and written
+to --mesh_output_path.  Needs --renderer_type cuda and a depth in
 2..10 (DESIGN.md §2)."""
 import gauss_to_pc
 

@@ -432,7 +432,8 @@ def config_parser(argv=None, mesh=False):
     mesh=True parses for gauss_to_mesh.py: --generate_mesh is implied and meshes with this project's GPU mesher
     (g2pc/mesh.py) instead of Open3D, which needs renderer_type cuda, a depth in mesh.DEPTH_MIN..DEPTH_MAX and
     laplacian_iterations >= 0.  It also adds --band_depth (narrow-band levels above --poisson_depth, up to
-    mesh.BAND_DEPTH_MAX; --poisson_depth 10 --band_depth 12 is the reference's depth 12)."""
+    mesh.BAND_DEPTH_MAX; --poisson_depth 10 --band_depth 12 is the reference's depth 12) and --target_triangles (>= 1:
+    decimate the mesh to that many triangles)."""
     try:
         import configargparse as ap
     except ImportError:
@@ -471,6 +472,9 @@ def config_parser(argv=None, mesh=False):
                             help="Mesh at this depth (poisson_depth + 1 .. 12), solving the levels above poisson_depth "
                                  "only in a narrow band around the points; --poisson_depth 10 --band_depth 12 is the "
                                  "reference's depth 12")
+        parser.add_argument("--target_triangles", default=None, type=int,
+                            help="Decimate the mesh to this many triangles (or one fewer) by quadric edge collapse on "
+                                 "the GPU; default: keep every triangle")
 
     args = parser.parse_args(argv)
     if mesh:
@@ -484,6 +488,8 @@ def config_parser(argv=None, mesh=False):
             raise AttributeError("Laplacian iterations must be 0 or more")
         if args.band_depth is not None and not args.poisson_depth < args.band_depth <= gmesh.BAND_DEPTH_MAX:
             raise AttributeError(f"Band depth must be between {args.poisson_depth + 1} and {gmesh.BAND_DEPTH_MAX}")
+        if args.target_triangles is not None and args.target_triangles < 1:
+            raise AttributeError("Target triangles must be 1 or more")
 
     if args.min_opacity < 0 or args.min_opacity > 1:
         raise AttributeError("Minumum opacity must be between 0 and 1")
@@ -596,7 +602,7 @@ def main(argv=None, mesh=False):
             print(f"Meshing {surface_point_cloud.points.shape[0]} surface points at depth {args.poisson_depth}{band}")
         m = gmesh.poisson_mesh(surface_point_cloud.points, surface_point_cloud.normals, surface_point_cloud.colours,
                                depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations, std_ratio=3.0,
-                               band_depth=args.band_depth)
+                               band_depth=args.band_depth, target_triangles=args.target_triangles)
         gmesh.write_mesh_ply(args.mesh_output_path, m)
         if not args.quiet:
             print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")

@@ -2,13 +2,14 @@
 trim and Laplacian smoothing (g2pc/mesh.py).
 
     python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10] [--band_depth 12]
-                      [--laplacian_iterations 10] [--orient_normals] [--quiet]
+                      [--laplacian_iterations 10] [--orient_normals] [--target_triangles N] [--quiet]
 
 The cloud must carry normals (nx ny nz), as gauss_to_pc.py writes them by default; its colours (red green blue) are
 carried over to the mesh's vertices.  A mesh faces the way its normals point.  By default the normals are used as they
 are; --orient_normals first gives them a consistent sign (g2pc/orient.py, k = 10), which the normals of a cloud sampled
 from Gaussians lack: each takes its sign from its Gaussian's rotation.  --band_depth adds finer levels stored only in a narrow band around the points:
---poisson_depth 10 --band_depth 12 is the reference's Poisson depth 12."""
+--poisson_depth 10 --band_depth 12 is the reference's Poisson depth 12.  --target_triangles decimates the smoothed mesh
+to N or N - 1 triangles on the GPU (quadric edge collapse, g2pc.mesh.decimate) before its normals are computed."""
 import argparse
 import time
 
@@ -33,6 +34,13 @@ def _iterations(s):
     return i
 
 
+def target(s):
+    n = int(s)
+    if n < 1:
+        raise argparse.ArgumentTypeError("must be >= 1")
+    return n
+
+
 def config_parser(argv=None):
     p = argparse.ArgumentParser(description="Mesh a point cloud with oriented normals (Poisson reconstruction)")
     p.add_argument("--input_path", required=True, help="point-cloud PLY with x y z and nx ny nz (red green blue optional)")
@@ -46,6 +54,8 @@ def config_parser(argv=None):
     p.add_argument("--laplacian_iterations", type=_iterations, default=10, help="Laplacian smoothing steps (0: none)")
     p.add_argument("--orient_normals", action="store_true",
                    help=f"orient the normals consistently (k = {orient.K_DEFAULT} nearest neighbours) before meshing")
+    p.add_argument("--target_triangles", type=target, default=None,
+                   help="decimate the mesh to this many triangles (or one fewer); default: keep every triangle")
     p.add_argument("--quiet", action="store_true", help="print nothing")
     args = p.parse_args(argv)
     if args.band_depth is not None and not args.poisson_depth < args.band_depth <= mesh.BAND_DEPTH_MAX:
@@ -77,7 +87,7 @@ def main(argv=None):
         if not args.quiet:
             print(f"Oriented the normals: {st.flipped} flipped, {st.components} component(s), {st.skipped} skipped")
     m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations,
-                          band_depth=args.band_depth)
+                          band_depth=args.band_depth, target_triangles=args.target_triangles)
     mesh.write_mesh_ply(args.mesh_output_path, m)
     if not args.quiet:
         print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path} "

@@ -333,6 +333,40 @@ int g2pc_mesh_band_gather(const float* xyz, const int32_t* colours, const uint32
                           const double* band_frame, int32_t depth, const int64_t* vkey, const double* vt, int64_t m,
                           double* density, uint8_t* vcolours, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- N9: decimation by parallel quadric edge collapse (s13_decimate.cu, g2pc/mesh.py decimate) ----------------- */
+/* Rules in DESIGN.md §2, N9.  vpos (m,3 float64), faces (t,3 int32, no face uses a vertex twice).  Order of calls:
+ * prepare once, then per round select (host reads counts) -> apply into a second face buffer, until the target is
+ * reached or no edge is selected; then finish.  quadrics: m x 10 float64 (A00 A01 A02 A11 A12 A22 b0 b1 b2 c). */
+/* quadrics: the area-weighted plane quadrics summed over each vertex's faces in ascending id; free_flags (m uint8): 1 iff
+ * the vertex has 1..128 faces, every edge at it is used by exactly two of them and they form one closed fan.
+ * workspace: g2pc_mesh_decimate_prepare_workspace_bytes(m, t). */
+int64_t g2pc_mesh_decimate_prepare_workspace_bytes(int64_t m, int64_t t);
+int g2pc_mesh_decimate_prepare(const double* vpos, int64_t m, const int32_t* faces, int64_t t, double* quadrics,
+                               uint8_t* free_flags, void* workspace, int64_t workspace_bytes, void* stream);
+/* Candidate edges and the 2-ring minimum selection.  counts (3 int64): unique edges, candidates, selected edges.  The
+ * workspace (g2pc_mesh_decimate_round_workspace_bytes(m, t)) carries the selection to the apply call of the same round
+ * with the same m and t. */
+int64_t g2pc_mesh_decimate_round_workspace_bytes(int64_t m, int64_t t);
+int g2pc_mesh_decimate_select(const double* vpos, int64_t m, const int32_t* faces, int64_t t, const double* quadrics,
+                              const uint8_t* free_flags, int64_t* counts, void* workspace, int64_t workspace_bytes,
+                              void* stream);
+/* Collapses the k (<= selected = counts[2] of the select call) selected edges with the smallest keys: vpos, quadrics,
+ * colour_sums (m,3 int64, may be NULL), merged (m int32), density_sums (m float64, may be NULL) and alive (m uint8) in
+ * place; faces_out (t - 2k, 3) = the surviving faces remapped, in their order; kept (1 int64) = their count.  applied
+ * (k uint64 keys, ascending) and applied_ab (k x 2 int32: survivor a, removed b) may be NULL. */
+int g2pc_mesh_decimate_apply(double* vpos, int64_t m, const int32_t* faces, int64_t t, double* quadrics,
+                             int64_t* colour_sums, int32_t* merged, double* density_sums, uint8_t* alive,
+                             int64_t selected, int64_t k, int32_t* faces_out, int64_t* kept, uint64_t* applied,
+                             int32_t* applied_ab, void* workspace, int64_t workspace_bytes, void* stream);
+/* The alive vertices in their order: vpos_out, colours_out = floor(sum / merged + 1/2) (NULL with colour_sums),
+ * densities_out = sum / merged (NULL with density_sums); faces_out = faces renumbered; counts (1 int64) = alive vertices.
+ * workspace: g2pc_mesh_decimate_finish_workspace_bytes(m). */
+int64_t g2pc_mesh_decimate_finish_workspace_bytes(int64_t m);
+int g2pc_mesh_decimate_finish(const double* vpos, int64_t m, const int32_t* faces, int64_t t, const uint8_t* alive,
+                              const int64_t* colour_sums, const int32_t* merged, const double* density_sums,
+                              double* vpos_out, uint8_t* colours_out, double* densities_out, int32_t* faces_out,
+                              int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- N7: consistent orientation of point-cloud normals (s11_orient.cu, g2pc/orient.py) -------------------------- */
 /* Hoppe et al. 1992 (the rule behind Open3D's orient_normals_consistent_tangent_plane) with this project's own rules
  * (DESIGN.md §2): k-NN graph, edge weight 1 - |n_i . n_j|, minimum spanning forest, sign propagated from one seed per
