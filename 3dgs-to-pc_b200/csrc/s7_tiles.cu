@@ -257,6 +257,8 @@ struct TileBlendParams {
     float bg[3];
     int32_t* work_counter;
     unsigned long long* stats;
+    float* out_T;              // (H,W) final transmittance (fusion variant only)
+    float* out_zmed;           // (H,W) median depth (fusion variant only)
 };
 
 __device__ __forceinline__ void pair_sync(int tile) {  // the two warps of one tile (static ids: a register id makes
@@ -268,8 +270,12 @@ __device__ __forceinline__ void pair_sync(int tile) {  // the two warps of one t
     }
 }
 
-template <bool SURF>
-__global__ void __launch_bounds__(TBT, SURF ? 3 : 4) blend_tiles_kernel(const TileBlendParams p) {
+// FUSION (never with SURF): also the final transmittance T and the median depth z_med of every pixel, the view depth of
+// the first blended Gaussian after which T < 0.5 (0 when T never drops below 0.5), for TSDF fusion (s14_tsdf.cu).  The
+// crossing is always seen when the final T < 0.5: alpha <= 0.99 keeps T >= 0.005 after a step from T >= 0.5, so the
+// stop at T < 1e-4 cannot come first.
+template <bool SURF, bool FUSION = false>
+__global__ void __launch_bounds__(TBT, (SURF || FUSION) ? 3 : 4) blend_tiles_kernel(const TileBlendParams p) {
     __shared__ __align__(16) float4 s_q0[2][TCH];
     __shared__ __align__(16) float4 s_q1[2][TCH];
     __shared__ __align__(16) float4 s_q2[2][TCH];  // (blue, depth, radius, packed tile rect)
@@ -305,6 +311,7 @@ __global__ void __launch_bounds__(TBT, SURF ? 3 : 4) blend_tiles_kernel(const Ti
     const bool row_in = row < th;
     // per pixel: inside the image and not masked out -> live; `live` drops to 0 when the pixel stops (T would fall below 1e-4)
     float live[4], T[4], Cr[4], Cg[4], Cb[4], D[4], ID[4], px[4];
+    float Z[FUSION ? 4 : 1];
     bool valid[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -314,6 +321,7 @@ __global__ void __launch_bounds__(TBT, SURF ? 3 : 4) blend_tiles_kernel(const Ti
         valid[i] = m;
         live[i] = m ? 1.0f : 0.0f;
         T[i] = 1.0f; Cr[i] = Cg[i] = Cb[i] = D[i] = ID[i] = 0.0f;
+        if (FUSION) Z[FUSION ? i : 0] = 0.0f;
         px[i] = (float)(tc0 + x0 + i);
     }
     const float py = (float)gy_;
@@ -440,6 +448,7 @@ __global__ void __launch_bounds__(TBT, SURF ? 3 : 4) blend_tiles_kernel(const Ti
                         if (keep && testT < 0.0001f) live[i] = 0.0f;
                         const float cc = (keep ? cand : 0.0f) * live[i];
                         const bool take = keep && (live[i] != 0.0f);
+                        if (FUSION && take && testT < 0.5f && T[i] >= 0.5f) Z[FUSION ? i : 0] = depth;
                         T[i] = take ? testT : T[i];
                         Cr[i] = fmaf(cc, q1.z, Cr[i]);
                         Cg[i] = fmaf(cc, q1.w, Cg[i]);
@@ -493,6 +502,11 @@ __global__ void __launch_bounds__(TBT, SURF ? 3 : 4) blend_tiles_kernel(const Ti
             p.out_color[2 * hw + pix] = fmaf(T[i], p.bg[2], Cb[i]);
             p.out_depth[pix] = D[i];
             p.out_invdepth[pix] = ID[i];
+        }
+        if (FUSION && row_in && x0 + i < tw) {  // masked pixels get 0
+            const int64_t pix = (int64_t)pix_base + i;
+            p.out_T[pix] = valid[i] ? T[i] : 0.0f;
+            p.out_zmed[pix] = valid[i] ? Z[FUSION ? i : 0] : 0.0f;
         }
     }
   }
@@ -599,11 +613,13 @@ extern "C" int g2pc_tiles_build(uint32_t* node_cnt, int32_t width, int32_t heigh
     return G2PC_OK;
 }
 
-extern "C" int g2pc_tiles_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header,
-                                const uint32_t* fail, int32_t frame, const uint32_t* inst_gid, const void* proj, uint64_t* cam_best, uint32_t* cam_dist,
-                                const int32_t* mask, float* out_color, float* out_depth, float* out_invdepth,
-                                int32_t width, int32_t height, const float* background3_host, int32_t* work_counters,
-                                uint64_t* stats, void* stream) {
+namespace {
+// g2pc_tiles_blend and, with out_T / out_zmed, g2pc_tiles_blend_fusion
+int tiles_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header, const uint32_t* fail,
+                int32_t frame, const uint32_t* inst_gid, const void* proj, uint64_t* cam_best, uint32_t* cam_dist,
+                const int32_t* mask, float* out_color, float* out_depth, float* out_invdepth, int32_t width,
+                int32_t height, const float* background3_host, int32_t* work_counters, uint64_t* stats, float* out_T,
+                float* out_zmed, void* stream) {
     G2PC_CHECK_ARG(leaves && leaf_order && header && fail && inst_gid && proj && cam_best && out_color && out_depth &&
                        out_invdepth && background3_host && work_counters, "null pointer");
     G2PC_CHECK_ARG(((uintptr_t)inst_gid & 15) == 0, "inst_gid must be 16-byte aligned (TMA bulk copies)");
@@ -615,13 +631,41 @@ extern "C" int g2pc_tiles_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_o
     p.W = width; p.H = height;
     for (int i = 0; i < 3; ++i) p.bg[i] = background3_host[i];
     p.work_counter = work_counters; p.stats = (unsigned long long*)stats;
+    p.out_T = out_T; p.out_zmed = out_zmed;
     cudaStream_t st = (cudaStream_t)stream;
-    if (cam_dist)
+    if (out_T)
+        blend_tiles_kernel<false, true><<<(unsigned)g2pc_resident_ctas(blend_tiles_kernel<false, true>, TBT, 0, 3), TBT,
+                                          0, st>>>(p);
+    else if (cam_dist)
         blend_tiles_kernel<true><<<(unsigned)g2pc_resident_ctas(blend_tiles_kernel<true>, TBT, 0, 3), TBT, 0, st>>>(p);
     else
         blend_tiles_kernel<false><<<(unsigned)g2pc_resident_ctas(blend_tiles_kernel<false>, TBT, 0, 4), TBT, 0, st>>>(p);
     G2PC_CHECK_LAUNCH();
     return G2PC_OK;
+}
+}  // namespace
+
+extern "C" int g2pc_tiles_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header,
+                                const uint32_t* fail, int32_t frame, const uint32_t* inst_gid, const void* proj, uint64_t* cam_best, uint32_t* cam_dist,
+                                const int32_t* mask, float* out_color, float* out_depth, float* out_invdepth,
+                                int32_t width, int32_t height, const float* background3_host, int32_t* work_counters,
+                                uint64_t* stats, void* stream) {
+    return tiles_blend(leaves, leaf_order, header, fail, frame, inst_gid, proj, cam_best, cam_dist, mask, out_color,
+                       out_depth, out_invdepth, width, height, background3_host, work_counters, stats, nullptr, nullptr,
+                       stream);
+}
+
+extern "C" int g2pc_tiles_blend_fusion(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header,
+                                       const uint32_t* fail, int32_t frame, const uint32_t* inst_gid, const void* proj,
+                                       uint64_t* cam_best, uint32_t* cam_dist, const int32_t* mask, float* out_color,
+                                       float* out_depth, float* out_invdepth, int32_t width, int32_t height,
+                                       const float* background3_host, int32_t* work_counters, uint64_t* stats,
+                                       float* out_T, float* out_zmed, void* stream) {
+    G2PC_CHECK_ARG(out_T && out_zmed, "null pointer");
+    G2PC_CHECK_ARG(!cam_dist, "the fusion blend computes no surface distances (cam_dist must be null)");
+    return tiles_blend(leaves, leaf_order, header, fail, frame, inst_gid, proj, cam_best, cam_dist, mask, out_color,
+                       out_depth, out_invdepth, width, height, background3_host, work_counters, stats, out_T, out_zmed,
+                       stream);
 }
 
 extern "C" int g2pc_tiles_accumulate(uint64_t* cam_best, uint32_t* cam_dist, const float* out_color, int32_t width,

@@ -107,6 +107,15 @@ SIGNATURES = {
     "g2pc_mesh_decimate_finish": ([_c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                    _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
                                   ctypes.c_int),
+    "g2pc_tsdf_frame_workspace_bytes": ([_i64], ctypes.c_int64),
+    "g2pc_tsdf_frame": ([_c_void_p, _i64, _i32, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_tsdf_integrate": ([_c_void_p, _i32, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32,
+                             _c_void_p, _c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p],
+                            ctypes.c_int),
+    "g2pc_tsdf_compact_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_tsdf_gather_compact": ([_c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i64,
+                                  _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                  _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_orient_prepare_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_orient_prepare": ([_c_void_p, _c_void_p, ctypes.c_int, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                              _c_void_p, _i64, _c_void_p], ctypes.c_int),
@@ -152,6 +161,9 @@ SIGNATURES = {
     "g2pc_tiles_blend": ([_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                           _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _c_void_p, _c_void_p,
                           _c_void_p], ctypes.c_int),
+    "g2pc_tiles_blend_fusion": ([_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p,
+                                 _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _c_void_p,
+                                 _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_tiles_accumulate": ([_c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i64, _c_void_p, _c_void_p, _c_void_p,
                                _c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_fill_u32": ([_c_void_p, _u32, _i64, _c_void_p], ctypes.c_int),
@@ -219,7 +231,7 @@ _OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sor
                 "g2pc_mesh_band_iso": 4, "g2pc_mesh_band_extract_count": 2, "g2pc_mesh_band_extract_emit": 2,
                 "g2pc_mesh_band_gather": 2, "g2pc_mesh_decimate_prepare": 4, "g2pc_mesh_decimate_select": 8,
                 "g2pc_mesh_decimate_apply": 5, "g2pc_mesh_decimate_finish": 4, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
-                "g2pc_orient_round": 5, "g2pc_orient_finish": 3}
+                "g2pc_orient_round": 5, "g2pc_orient_finish": 3, "g2pc_tsdf_frame": 2, "g2pc_tsdf_gather_compact": 4}
 # host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",
                 "g2pc_multisplit_rows", "g2pc_blend_set_compact", "g2pc_blend_set_cull"}

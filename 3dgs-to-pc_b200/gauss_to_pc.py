@@ -236,11 +236,12 @@ def sample_points_per_gaussian(xyz, covariances, colours, normals, points_per_ga
     return pts, cols, nrm, total, status, dbg
 
 
-def convert_3dgs_to_pc(input_path, transform_path, mask_path, pointcloud_settings):
+def convert_3dgs_to_pc(input_path, transform_path, mask_path, pointcloud_settings, mesh_method="poisson"):
     """
     Generates a pointcloud from a 3DGS file  (reference: gauss_to_pc.py:373-601; same stages in the same order)
 
-    Returns (total_point_cloud, surface_point_cloud) as PointCloudData tuples.
+    Returns (total_point_cloud, surface_point_cloud) as PointCloudData tuples (mesh_method: see
+    convert_gaussians_to_pc).
     """
     from transform_dataloader import load_transform_data
     from mask_dataloader import load_image_masks
@@ -263,11 +264,12 @@ def convert_3dgs_to_pc(input_path, transform_path, mask_path, pointcloud_setting
 
     say("Loading Gaussians from File\n")
     xyz, scales, rots, colours, opacities, shs = load_gaussians(input_path, max_sh_degree=s.max_sh_degree)
-    return convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transforms, intrinsics, mask_images, s)
+    return convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transforms, intrinsics, mask_images, s,
+                                   mesh_method=mesh_method)
 
 
 def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transforms, intrinsics, mask_images,
-                            pointcloud_settings, render_shs=False, timings=None):
+                            pointcloud_settings, render_shs=False, timings=None, mesh_method="poisson"):
     """The device-resident part of convert_3dgs_to_pc (gauss_to_pc.py:414-601): everything between the loaders and the
     PLY writer.  transforms: {name: 4x4 c2w (nested list / tensor)} or None; intrinsics: {name: [w, h, fx, fy]}.
     render_shs=True evaluates the SH colour per camera inside the colour stage (the reference's CLI never passes the SH
@@ -276,9 +278,19 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
     surface_sample).
 
     With generate_mesh the surface cloud's normals are turned toward the camera that gave each surface Gaussian its
-    maximum contribution (g2pc.orient.face_cameras), so that they point from the solid toward free space."""
+    maximum contribution (g2pc.orient.face_cameras), so that they point from the solid toward free space.
+
+    mesh_method="tsdf" (with generate_mesh) samples no surface cloud: the second result is a g2pc.tsdf.Scene instead,
+    the Gaussians the main cloud is sampled from (the rows kept by the culls and the covariance validation) with the
+    colour inputs the colour stage rendered (the loader's colours, or the SH with render_shs) and the same cameras, for
+    g2pc.tsdf.fuse_mesh.  The main cloud is the same either way."""
     s = pointcloud_settings
     say = (lambda *a: None) if s.quiet else print
+    if mesh_method not in ("poisson", "tsdf"):
+        raise capi.G2pcError(f"mesh_method must be 'poisson' or 'tsdf', got {mesh_method!r}")
+    fusion = s.generate_mesh and mesh_method == "tsdf"
+    if fusion and not s.render_colours:
+        raise capi.G2pcError("TSDF fusion renders the cameras: it needs render_colours")
     if s.generate_mesh and s.render_colours and s.renderer_type != "cuda":
         raise capi.G2pcError("meshing needs the surface distances of the cuda renderer (renderer_type='cuda'); the "
                              "python renderer has none")
@@ -290,11 +302,13 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
             gaussians.calculate_normals()
 
     total_gaussian_contributions = None
+    # TSDF fusion renders the kept rows again with the inputs of the colour stage, which overwrites gaussians.colours
+    fusion_colours, fusion_shs, fusion_cameras = gaussians.colours, (gaussians.shs if render_shs else None), []
 
     if s.render_colours:
         say("Rendering Gaussian Colours")
 
-        want_surface = True if (s.surface_distance_std is not None or s.generate_mesh) else False
+        want_surface = True if (s.surface_distance_std is not None or (s.generate_mesh and not fusion)) else False
         gaussian_renderer = get_renderer(s.renderer_type, gaussians.xyz, torch.unsqueeze(torch.clone(gaussians.opacities), 1),
                                          gaussians.colours, gaussians.covariances,
                                          shs=gaussians.shs if render_shs else None,
@@ -309,7 +323,7 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
             raise Exception("Transforms are required to render colours")
 
         first_frame, cam_centres = None, []
-        if s.generate_mesh:
+        if s.generate_mesh and not fusion:
             # the accumulate kernels record, per Gaussian, the index of the camera that raised its maximum contribution
             first_frame = torch.full((gaussians.xyz.shape[0],), torch.iinfo(torch.int32).max, dtype=torch.int32,
                                      device=gaussians.xyz.device)
@@ -326,6 +340,8 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
                                     sh_degree=s.max_sh_degree, white_bkgd=True, mask=mask)
                 if first_frame is not None:
                     cam_centres.append(camera._campos_host)  # the centre the kernels use, in camera-index order
+                if fusion:
+                    fusion_cameras.append(camera)
                 with nvtx(f"g2pc: camera {img_name}"):
                     render, _, _, depth_map = gaussian_renderer(camera)
 
@@ -351,7 +367,7 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
         if gaussians.xyz.shape[0] < 1:
             raise Exception("Number of Gaussians after culling is 0, meaning a point cloud cannot be generated")
 
-        if s.generate_mesh:
+        if s.generate_mesh and not fusion:
             # a mask over the original rows, then over the kept rows of the cull (culled_indices is their ascending list)
             with capi.phase(timings, "surface_select"):
                 surface_gaussian_idxs = gaussian_renderer.get_predicted_surface_gaussians(predicted_surface_std=1.0)
@@ -391,7 +407,14 @@ def convert_gaussians_to_pc(xyz, scales, rots, colours, opacities, shs, transfor
     total_point_cloud = PointCloudData(points=points, colours=colours, normals=normals)
     surface_point_cloud = None
 
-    if s.generate_mesh and s.render_colours:
+    if fusion:
+        from g2pc import tsdf
+        rows = gaussians.ids.to(torch.int64)
+        surface_point_cloud = tsdf.Scene(
+            xyz=gaussians.xyz, opacities=gaussians.opacities, covariances=gaussians.covariances,
+            colours=fusion_colours[rows] if fusion_shs is None else None,
+            shs=fusion_shs[rows] if fusion_shs is not None else None, cameras=fusion_cameras)
+    elif s.generate_mesh and s.render_colours:
         say("Starting Point Cloud Generation for Surface Gaussians\n")
         from g2pc import orient
         with capi.phase(timings, "surface_select"):
@@ -453,7 +476,8 @@ def config_parser(argv=None, mesh=False):
     parser.add_argument("--surface_distance_std", type=float, default=None, help="Cull Gaussians further than X standard deviations from the scene surfaces")
     parser.add_argument("--clean_pointcloud", action="store_true", help="Remove outliers after generation (statistical outlier removal, 20 nearest neighbours, on the GPU)")
     parser.add_argument("--generate_mesh", action="store_true", help="Also generate a mesh (requires Open3D)")
-    parser.add_argument("--poisson_depth", default=10, type=int, help="Depth of the poisson surface reconstruction")
+    parser.add_argument("--poisson_depth", default=10, type=int, help="Depth of the poisson surface reconstruction" +
+                        (" (unused with --mesh_method tsdf)" if mesh else ""))
     parser.add_argument("--laplacian_iterations", default=10, type=int, help="Iterations of laplacian mesh smoothing")
     parser.add_argument("--mesh_output_path", type=str, default="3dgs_mesh.ply", help="Path to mesh output file (must be ply file)")
     parser.add_argument("--camera_skip_rate", type=int, default=0, help="Number of cameras to skip for each rendered camera")
@@ -475,6 +499,13 @@ def config_parser(argv=None, mesh=False):
         parser.add_argument("--target_triangles", default=None, type=int,
                             help="Decimate the mesh to this many triangles (or one fewer) by quadric edge collapse on "
                                  "the GPU; default: keep every triangle")
+        parser.add_argument("--mesh_method", default="poisson", choices=("poisson", "tsdf"),
+                            help="poisson: mesh a surface cloud sampled from the surface Gaussians; tsdf: fuse the "
+                                 "rendered median depth of every camera into a voxel grid and mesh its zero crossing")
+        parser.add_argument("--tsdf_depth", default=9, type=int,
+                            help="With --mesh_method tsdf: 2^depth voxels per axis (2..10)")
+        parser.add_argument("--tsdf_trunc", default=4.0, type=float,
+                            help="With --mesh_method tsdf: truncation distance in voxels (> 0)")
 
     args = parser.parse_args(argv)
     if mesh:
@@ -482,14 +513,24 @@ def config_parser(argv=None, mesh=False):
         args.generate_mesh = True
         if args.renderer_type != "cuda":
             raise AttributeError("Meshing needs the surface distances of the cuda renderer (--renderer_type cuda)")
-        if not gmesh.DEPTH_MIN <= args.poisson_depth <= gmesh.DEPTH_MAX:
+        if args.mesh_method == "poisson" and not gmesh.DEPTH_MIN <= args.poisson_depth <= gmesh.DEPTH_MAX:
             raise AttributeError(f"Poisson depth must be between {gmesh.DEPTH_MIN} and {gmesh.DEPTH_MAX}")
         if args.laplacian_iterations < 0:
             raise AttributeError("Laplacian iterations must be 0 or more")
-        if args.band_depth is not None and not args.poisson_depth < args.band_depth <= gmesh.BAND_DEPTH_MAX:
+        if args.mesh_method == "poisson" and args.band_depth is not None and \
+                not args.poisson_depth < args.band_depth <= gmesh.BAND_DEPTH_MAX:
             raise AttributeError(f"Band depth must be between {args.poisson_depth + 1} and {gmesh.BAND_DEPTH_MAX}")
         if args.target_triangles is not None and args.target_triangles < 1:
             raise AttributeError("Target triangles must be 1 or more")
+        if args.mesh_method == "tsdf":
+            from g2pc import tsdf
+            if args.band_depth is not None:
+                raise AttributeError("--band_depth belongs to the Poisson mesher: it cannot be used with "
+                                     "--mesh_method tsdf")
+            if not tsdf.DEPTH_MIN <= args.tsdf_depth <= tsdf.DEPTH_MAX:
+                raise AttributeError(f"TSDF depth must be between {tsdf.DEPTH_MIN} and {tsdf.DEPTH_MAX}")
+            if not args.tsdf_trunc > 0:
+                raise AttributeError("TSDF truncation must be greater than 0 voxels")
 
     if args.min_opacity < 0 or args.min_opacity > 1:
         raise AttributeError("Minumum opacity must be between 0 and 1")
@@ -544,7 +585,8 @@ def config_parser(argv=None, mesh=False):
 
 def main(argv=None, mesh=False):
     """The command.  mesh=True is gauss_to_mesh.py: after the point cloud it writes the mesh of the surface cloud to
-    --mesh_output_path and returns (surface PointCloudData with normals facing the cameras, g2pc.mesh.Mesh)."""
+    --mesh_output_path and returns (surface PointCloudData with normals facing the cameras, g2pc.mesh.Mesh); with
+    --mesh_method tsdf it writes the TSDF fusion mesh instead and returns (None, g2pc.mesh.Mesh)."""
     args = config_parser(argv, mesh=mesh)
 
     if not torch.cuda.is_available():
@@ -573,8 +615,9 @@ def main(argv=None, mesh=False):
         device="cuda:0",
     )
 
-    total_point_cloud, surface_point_cloud = convert_3dgs_to_pc(args.input_path, args.transform_path, args.mask_path,
-                                                                pointcloud_settings)
+    total_point_cloud, surface_point_cloud = convert_3dgs_to_pc(
+        args.input_path, args.transform_path, args.mask_path, pointcloud_settings,
+        mesh_method=args.mesh_method if mesh else "poisson")
 
     if args.clean_pointcloud:
         if not args.quiet:
@@ -592,6 +635,18 @@ def main(argv=None, mesh=False):
     save_xyz_to_ply(total_point_cloud.points, args.output_path, rgb_colors=total_point_cloud.colours,
                     normals_points=total_point_cloud.normals, chunk_size=10**6, quiet=args.quiet)
 
+    if mesh and args.mesh_method == "tsdf":
+        from g2pc import mesh as gmesh, tsdf
+        scene = surface_point_cloud
+        if not args.quiet:
+            print(f"Fusing the median depth of {len(scene.cameras)} cameras into a 2^{args.tsdf_depth} voxel grid")
+        m = tsdf.fuse_mesh(scene.xyz, scene.opacities, scene.covariances, scene.cameras, colours=scene.colours,
+                           shs=scene.shs, depth=args.tsdf_depth, trunc=args.tsdf_trunc,
+                           laplacian_iters=args.laplacian_iterations, target_triangles=args.target_triangles)
+        gmesh.write_mesh_ply(args.mesh_output_path, m)
+        if not args.quiet:
+            print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")
+        return None, m
     if mesh:
         from g2pc import mesh as gmesh
         st = LAST_SURFACE_STATS["face_cameras"]

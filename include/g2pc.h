@@ -622,6 +622,16 @@ int g2pc_tiles_blend(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const
                      int32_t height, const float* background3_host, int32_t* work_counters, uint64_t* stats,
                      void* stream);
 
+/* g2pc_tiles_blend (cam_dist must be NULL) that also writes, for every pixel inside the image, out_T (H,W) f32 = the final
+ * transmittance and out_zmed (H,W) f32 = the view depth of the first blended Gaussian after which T < 0.5, 0 when T never
+ * drops below 0.5; both 0 where the mask is 0. */
+int g2pc_tiles_blend_fusion(const g2pc_leaf_t* leaves, const int32_t* leaf_order, const int32_t* header,
+                            const uint32_t* fail, int32_t frame, const uint32_t* inst_gid, const void* proj,
+                            uint64_t* cam_best, uint32_t* cam_dist, const int32_t* mask, float* out_color,
+                            float* out_depth, float* out_invdepth, int32_t width, int32_t height,
+                            const float* background3_host, int32_t* work_counters, uint64_t* stats, float* out_T,
+                            float* out_zmed, void* stream);
+
 /* Accumulator update of one camera (__init__.py:128-158): where the camera's contribution beats max_contrib (strict >)
  * store it and the FINAL colour of its arg-max pixel; total_contrib += contribution; min_dist = min(min_dist, cam_dist).
  * Clears cam_best / re-arms cam_dist.  Optional per-camera outputs of the op (n each): cam_contrib f32, cam_pixel i32,
@@ -632,6 +642,38 @@ int g2pc_tiles_accumulate(uint64_t* cam_best, uint32_t* cam_dist, const float* o
                           float* cam_surface, void* stream);
 
 int g2pc_fill_u32(uint32_t* v, uint32_t value, int64_t n, void* stream);
+
+/* ---- N10: TSDF fusion of rendered depth (s14_tsdf.cu, g2pc/tsdf.py, gauss_to_mesh.py --mesh_method tsdf) --------- */
+/* Frame words (8 doubles, the layout g2pc_mesh_splat writes) of a 2^depth grid over the finite points xyz (n,3) f32:
+ * L = 1.1 x the largest extent, centred on the bounding box, h = L / R.  workspace: g2pc_tsdf_frame_workspace_bytes(n),
+ * 4-byte aligned. */
+int64_t g2pc_tsdf_frame_workspace_bytes(int64_t n);
+int g2pc_tsdf_frame(const float* xyz, int64_t n, int32_t depth, double* frame, void* workspace, int64_t workspace_bytes,
+                    void* stream);
+
+/* Integrate one camera into the grid (R^3 voxels, node index (k*R + j)*R + i): tsdf f32, weight f32, colour (3, R^3)
+ * f32.  zmed / transmittance (H,W) f32 and image (3,H,W) f32 are g2pc_tiles_blend_fusion's outputs for the camera
+ * rs_host, mask (H*W) int32 or NULL, background3_host its background.  One thread per voxel: skipped when the view
+ * depth z <= 0.2, the nearest pixel is outside the image or masked, z_med = 0 there, or z_med - z < -mu with
+ * mu = float(trunc_voxels * h); otherwise tsdf, colour += (min(1, sdf / mu), un-blended pixel colour) as running means
+ * and weight += 1 (DESIGN.md §2, N10).  Does nothing when frame_index is skipped by the failure word fail. */
+int g2pc_tsdf_integrate(const double* frame, int32_t depth, double trunc_voxels, const float* zmed,
+                        const float* transmittance, const float* image, const int32_t* mask, int32_t width,
+                        int32_t height, const g2pc_raster_t* rs_host, const float* background3_host,
+                        const uint32_t* fail, int32_t frame_index, float* tsdf, float* weight, float* colour,
+                        void* stream);
+
+/* After g2pc_mesh_extract_emit on the tsdf grid (iso 0): keep[v] (m u8) = both ends of vertex v's edge have weight > 0,
+ * density[v] = (1-t) w_a + t w_b (f64), vcolours[v] (m,3 u8, NULL with colour NULL) = floor(255 ((1-t) c_a + t c_b) +
+ * 1/2) clamped; a triangle is kept iff its three vertices are; then the kept vertices (density, vpos, colours) and
+ * triangles (re-indexed) are compacted in order into the *_out arrays, counts (2 int64) = kept vertices, triangles.
+ * workspace: g2pc_tsdf_compact_workspace_bytes(m, t), 256-byte aligned. */
+int64_t g2pc_tsdf_compact_workspace_bytes(int64_t m, int64_t t);
+int g2pc_tsdf_gather_compact(const float* weight, const float* colour, int32_t depth, const int64_t* vkey,
+                             const double* vt, const double* vpos, int64_t m, const int32_t* faces, int64_t t,
+                             uint8_t* keep, double* density, uint8_t* vcolours, int64_t* counts, double* density_out,
+                             double* vpos_out, uint8_t* vcolours_out, int32_t* faces_out, void* workspace,
+                             int64_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
