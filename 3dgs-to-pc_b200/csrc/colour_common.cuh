@@ -51,6 +51,7 @@ __device__ __forceinline__ void g2pc_write_frame_header(int32_t* header, uint32_
     header[G2PC_HDR_LEAF_OVERFLOW] = leaf_over;
     header[G2PC_HDR_CAP_OVERFLOW] = cap_over;
     header[G2PC_HDR_FRAME] = frame;
+    header[G2PC_HDR_ROW_INST] = 0;  // (the multisplit fills it in)
     if (need_deeper | leaf_over | cap_over) atomicMin(fail, (uint32_t)(frame + 1));
     const uint32_t f = *(volatile uint32_t*)fail;
     header[G2PC_HDR_POISON] = f == 0xFFFFFFFFu ? 0 : (int32_t)f;

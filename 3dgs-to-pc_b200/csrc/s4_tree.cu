@@ -16,16 +16,22 @@
 //                           the frame header.  A frame that does not fit the caller's buffers (or needs a deeper table)
 //                           sets the sticky POISON word: every later kernel of this and the following frames becomes a
 //                           no-op until the host has read the header, fixed the sizes and replayed.
-//   3. g2pc_multisplit      stable one-pass-per-chunk multisplit of the depth-ordered stream into the leaves' lists:
-//        count    CTA c takes E = S x C consecutive sorted entries (2 sub-steps of C = 256 at C3) and counts its
-//                 instances per leaf (shared-memory histogram)
-//        scan     per leaf, exclusive prefix over the chunks (+ the leaf's list offset)          -> matrix[c][leaf]
-//        scatter  CTA c walks its sub-steps in order, starting from row c of the matrix; per sub-step it marks bit
-//                 (leaf, k) for every instance in a shared-memory bit matrix (order-free atomicOr); an instance's place
-//                 is the leaf's running offset + the set bits of its leaf before bit k (popc), then the offsets move past
-//                 the sub-step: the lists come out depth-ordered without any sort of the ~7 N instances (the round-1
-//                 path emitted (leaf, id) pairs and ran a 2-pass 20 M-pair radix sort per camera).  Splats that cover
-//                 many tiles are walked by the whole warp (colour_common.cuh warp_for_each_node).
+//   3. g2pc_multisplit      stable multisplit of the depth-ordered stream into the leaves' lists, without any sort of
+//                           the ~7 N instances (the round-1 path emitted (leaf, id) pairs and ran a 2-pass 20 M-pair
+//                           radix sort per camera).  A base-level leaf is one cell (ix, iy) of a grid of at most 256 x 256
+//                           (the quadtree's base level, or the CUDA back-end's super-tiles), and an entry covers a
+//                           rectangle of cells, so its base-level lists are two stable splits of <= 256 buckets each:
+//        rows     the sorted stream -> one list of 64-bit entries per row iy, in stream order       (row_list)
+//        columns  each row's list -> one list per cell, written straight into the leaf's list in inst_gid
+//                 Each split is count -> scan -> scatter over warp tiles of 512 consecutive entries.  Within a batch of
+//                 32 entries (one per lane) a 32 x 32 bit transpose gives lane b the ballot of the lanes whose entry
+//                 falls in bucket b; an entry's place is the bucket's running offset + its rank among those lanes, and
+//                 lane b keeps the running offset of bucket b in a register.  No shared-memory bit matrix and no CTA
+//                 barrier inside the walk; the count matrices are tiles x buckets, kilobytes.
+//        deeper   leaves below the base level (count-driven splits) come from the older chunked multisplit (count /
+//                 scan / scatter with a shared-memory bit matrix per sub-step), which runs only when the table has such
+//                 levels and emits only those leaves.  Splats that cover many tiles are walked by the whole warp
+//                 (colour_common.cuh warp_for_each_node).
 #include <cub/cub.cuh>
 #include "colour_common.cuh"
 
@@ -176,9 +182,9 @@ __global__ void __launch_bounds__(TB) tree_kernel(const TreeParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Multisplit.  An entry of the sorted stream is (range << 32 | gid); its leaves are enumerated from the packed node range
-// at the base level; Gaussians that touch a split node re-derive their rect from the projection record and query the
-// deeper candidate levels (count-driven splits only — rare).
+// Multisplit below the base level.  An entry of the sorted stream is (range << 32 | gid); Gaussians that touch a split
+// base node (or sit in the one-node overhang of one) re-derive their rect from the projection record and query the deeper
+// candidate levels.
 struct MsParams {
     const unsigned long long* val_sorted;
     int64_t n;
@@ -200,36 +206,29 @@ struct MsParams {
     int32_t leaf_cap;      // leaves the shared-memory tables are sized for (<= max_leaves of the tree)
     int32_t base_clean;    // the base level has no dropped / degenerate node: membership = the packed range, no table look-ups
     uint32_t clean_mask;   // the same, per level
-    int32_t grid_w;        // > 0: flat tile grid (s7_tiles.cu): leaf = iy * grid_w + ix, the packed range is the tile rect
+    const uint32_t* base_split;  // written by the row split: 1 iff a base-level node of this frame was split (else no list
+                                 // below the base level, and these kernels return at once)
     int32_t steps;         // sub-steps of C entries per chunk (ms_steps)
 };
 
-// f(leaf, owner_lane, owner_gid) for every leaf the lane's entry overlaps; warp-cooperative (all 32 lanes must call).
+// f(leaf, owner_lane, owner_gid) for every leaf BELOW the base level that the lane's entry overlaps (the base-level lists
+// come from the row / column split further down); warp-cooperative (all 32 lanes must call).
 template <typename F>
 __device__ __forceinline__ void for_each_leaf(const MsParams& p, const QtTables& T, const int32_t* __restrict__ s_leaf,
                                               uint32_t range, uint32_t gid, F f) {
-    if (p.grid_w > 0) {
-        warp_for_each_node(range, gid, [&](int ix, int iy, int owner, uint32_t og) { f(iy * p.grid_w + ix, owner, og); });
-        return;
-    }
     const int lb = p.base_level;
     const int o1 = (1 << lb) - 1;
     unsigned deeper = 0;
     if (p.base_clean) {
-        warp_for_each_node(range, gid, [&](int ix, int iy, int owner, uint32_t og) {
-            const int32_t v = s_leaf[(iy << lb) + ix];
-            if (v >= 0) f(v, owner, og);
-            else if (v == -2) deeper |= 1u << owner;
+        warp_for_each_node(range, gid, [&](int ix, int iy, int owner, uint32_t) {
+            if (s_leaf[(iy << lb) + ix] == -2) deeper |= 1u << owner;
         });
     } else {
-        warp_for_each_node(range, gid, [&](int ix, int iy, int owner, uint32_t og) {
+        warp_for_each_node(range, gid, [&](int ix, int iy, int owner, uint32_t) {
             if (!axis_member(T.ys + o1, T.ye + o1, T.yf + o1, iy) || !axis_member(T.xs + o1, T.xe + o1, T.xf + o1, ix)) return;
-            const int32_t v = s_leaf[(iy << lb) + ix];
-            if (v >= 0) f(v, owner, og);
-            else if (v == -2) deeper |= 1u << owner;
+            if (s_leaf[(iy << lb) + ix] == -2) deeper |= 1u << owner;
         });
     }
-    if (p.meta.num_levels <= lb + 1) return;
     int xlo, xhi, ylo, yhi;
     g2pc_unpack_range(range, xlo, xhi, ylo, yhi);
     // ---- count-driven splits below the base level ----
@@ -290,21 +289,14 @@ __device__ __forceinline__ void for_each_leaf(const MsParams& p, const QtTables&
 
 // The sorted stream is cut into chunks of E = steps x C consecutive entries, one CTA per chunk; a CTA walks its chunk in
 // `steps` sub-steps of C entries (one per thread), in stream order.  The per-chunk set-up (tables, node->leaf map, one
-// matrix row) is paid once per E entries, and the matrix (chunks x leaves) stays small enough to live in L2 (C3: 5.9 k
-// rows x 1024 leaves, 24 MB).
+// matrix row) is paid once per E entries.
 __device__ __forceinline__ unsigned long long ms_entry(const MsParams& p, int64_t k) {
     return k < p.n ? p.val_sorted[k] : (unsigned long long)G2PC_RANGE_EMPTY << 32;
 }
 
 // shared memory of the count / scatter kernels: [6 * n1 table ints][4^base node->leaf ints][payload]
 __device__ __forceinline__ int32_t* ms_load_common(const MsParams& p, int32_t* smem, QtTables& T) {
-    if (p.grid_w > 0) { T = p.tab; return smem; }  // tile grid: nothing to stage
-    if (p.base_clean && p.meta.num_levels <= p.base_level + 1) {
-        T = p.tab;  // never dereferenced: no table look-up at a clean base level, no deeper level
-        __syncthreads();
-    } else {
-        T = load_tables(p.tab, p.n1, smem);  // ends with __syncthreads()
-    }
+    T = load_tables(p.tab, p.n1, smem);  // ends with __syncthreads()
     int32_t* s_leaf = smem + 6 * p.n1;
     const int nb = 1 << (2 * p.base_level);
     const int32_t* src = p.node_leaf + off2d(p.base_level);
@@ -320,11 +312,11 @@ __device__ __forceinline__ int32_t* ms_load_common(const MsParams& p, int32_t* s
 template <int C>
 __global__ void __launch_bounds__(C, 1024 / C) ms_count_kernel(const MsParams p) {
     extern __shared__ int32_t smem_ms[];
-    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    if (g2pc_frame_skipped(p.fail, p.frame) || *p.base_split == 0u) return;
     const int nl = p.header[G2PC_HDR_NUM_LEAVES];
     QtTables T;
     int32_t* s_leaf = ms_load_common(p, smem_ms, T);
-    uint32_t* s_hist = reinterpret_cast<uint32_t*>(s_leaf + (p.grid_w > 0 ? 0 : (1 << (2 * p.base_level))));
+    uint32_t* s_hist = reinterpret_cast<uint32_t*>(s_leaf + (1 << (2 * p.base_level)));
     for (int i = threadIdx.x; i < nl; i += C) s_hist[i] = 0u;
     __syncthreads();
     // no barrier between the sub-steps: the warps only add to the histogram
@@ -347,7 +339,7 @@ __global__ void __launch_bounds__(C, 1024 / C) ms_count_kernel(const MsParams p)
 constexpr int SCAN_BATCH = 8;  // matrix loads in flight per thread
 __global__ void __launch_bounds__(1024) ms_scan_kernel(const MsParams p, int32_t rows) {
     __shared__ uint32_t s_sum[32][33];
-    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    if (g2pc_frame_skipped(p.fail, p.frame) || *p.base_split == 0u) return;
     const int nl = p.header[G2PC_HDR_NUM_LEAVES];
     if (blockIdx.x * 32 >= nl) return;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -381,12 +373,12 @@ __global__ void __launch_bounds__(1024) ms_scan_kernel(const MsParams p, int32_t
 template <int C>
 __global__ void __launch_bounds__(C, 768 / C) ms_scatter_kernel(const MsParams p) {
     extern __shared__ int32_t smem_ms[];
-    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    if (g2pc_frame_skipped(p.fail, p.frame) || *p.base_split == 0u) return;
     const int nl = p.header[G2PC_HDR_NUM_LEAVES];
     constexpr int WORDS = C / 32;
     QtTables T;
     int32_t* s_leaf = ms_load_common(p, smem_ms, T);
-    uint32_t* s_row = reinterpret_cast<uint32_t*>(s_leaf + (p.grid_w > 0 ? 0 : (1 << (2 * p.base_level))));  // [nl]
+    uint32_t* s_row = reinterpret_cast<uint32_t*>(s_leaf + (1 << (2 * p.base_level)));  // [nl]
     uint32_t* s_bits = s_row + p.leaf_cap;                                                                   // [WORDS][nl]
     {
         // the chunk's list offsets (one coalesced row of the matrix) and a zeroed bit matrix; 16-byte stores where the
@@ -438,7 +430,424 @@ __global__ void __launch_bounds__(C, 768 / C) ms_scatter_kernel(const MsParams p
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Base-level lists: two stable splits, rows then columns.  Level 1 splits the sorted stream into one list per row (the
+// 64-bit entries, in stream order); level 2 splits each row's list into its cells and writes the Gaussian ids straight
+// into the leaves' lists.  Each level is count -> scan -> scatter over warp tiles of SP_TILE consecutive entries; the
+// SP_WARPS tiles of a CTA form a band (level 2: a band never crosses a row).  The count kernel writes each tile's
+// exclusive offsets within its band (m) and the band's totals (b); the scan turns the band totals into absolute offsets
+// (level 1: also the rows' list offsets and the level-2 band layout); the scatter starts every bucket at b + m.
+constexpr int SP_BATCHES = 8;                // 32-entry batches per warp tile
+constexpr int SP_TILE = 32 * SP_BATCHES;     // entries per warp tile
+constexpr int SP_WARPS = 16;                 // warp tiles per CTA = per band
+constexpr int SP_BAND = SP_TILE * SP_WARPS;  // entries per band
+constexpr int SP_MAX_CELLS = 256;            // cells per axis (G2PC_RANGE_MAX_LEVEL)
+constexpr int SP_MAX_GROUPS = SP_MAX_CELLS / 32;
+constexpr int SP_STAGE_BYTES = 6 * 1024;     // per warp: a tile's output staged in shared memory, written out bucket by bucket
+
+struct SplitParams {
+    const unsigned long long* val_sorted;
+    int64_t n;
+    int32_t rows, cols;          // grid of base cells
+    int32_t rows_p, cols_p;      // rounded up to whole groups of 32 (row width of the count matrices)
+    const int32_t* cell_leaf;    // rows x cols leaf ids (< 0: no base-level leaf), or NULL: leaf = iy * cols + ix
+    QtTables tab;                // base-level axis tables (level offset applied) when the base level is not clean
+    int32_t clean;               // 1: every cell in an entry's range is a member, no table look-ups
+    const g2pc_leaf_t* leaves;
+    int32_t* header;
+    uint32_t* fail;
+    int32_t frame;
+    unsigned long long* row_list;
+    int64_t row_capacity;
+    uint32_t* m1;                // [bands1][SP_WARPS + 1][rows_p] (row SP_WARPS: the band's totals)
+    uint32_t* b1;                // [bands1][rows_p]
+    uint32_t* m2;                // [bands2][SP_WARPS + 1][cols_p]
+    uint32_t* b2;                // [bands2][cols_p]
+    uint32_t* row_begin;         // [rows + 1]: offset of each row's list in row_list
+    uint32_t* band_begin;        // [rows + 1]: first level-2 band of each row
+    uint32_t* base_split;        // quadtree only (else NULL): set to 1 iff a cell is a split node (cell_leaf == -2)
+    int32_t bands1;
+    uint32_t* inst_gid;
+};
+
+// bits of [lo, hi] inside the group of 32 buckets that starts at `base`
+__device__ __forceinline__ uint32_t span_bits(int lo, int hi, int base) {
+    lo = max(lo - base, 0);
+    hi = min(hi - base, 31);
+    return lo > hi ? 0u : ((0xFFFFFFFFu >> (31 - hi)) & (0xFFFFFFFFu << lo));
+}
+
+// 32 x 32 bit transpose across the warp: lane i brings row i, lane j gets column j (bit i = bit j of lane i).  Five
+// rounds of block swaps: at distance s the lanes with bit s clear trade their high s-bit halves for their partner's low.
+__device__ __forceinline__ uint32_t warp_transpose32(uint32_t x) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t masks[5] = {0x0000FFFFu, 0x00FF00FFu, 0x0F0F0F0Fu, 0x33333333u, 0x55555555u};
+#pragma unroll
+    for (int i = 0, s = 16; i < 5; ++i, s >>= 1) {
+        const uint32_t t = __shfl_xor_sync(0xffffffffu, x, s);
+        x = (lane & s) ? ((x & ~masks[i]) | ((t & ~masks[i]) >> s)) : ((x & masks[i]) | ((t & masks[i]) << s));
+    }
+    return x;
+}
+
+// One warp walks entries [beg, end) of src in batches of 32, in order.  Buckets are rows (LEVEL 1) or columns (LEVEL 2);
+// member[g]: the buckets of group g an entry may go to (warp-uniform).  COUNT: acc[g] (lane b: bucket 32 g + b) += the
+// batch's entries in the bucket.  Otherwise acc[g] is the bucket's running offset: lane b writes the bucket's entries of
+// the batch, in lane order, at acc[g]++ (level 1: the entry into row_list; level 2: its Gaussian id into inst_gid).
+template <int LEVEL, int G, bool COUNT, typename Out>
+__device__ __forceinline__ void split_walk(const SplitParams& p, const unsigned long long* __restrict__ src, int64_t beg,
+                                           int64_t end, const uint32_t (&member)[G], uint32_t (&acc)[G], Out out) {
+    const int lane = threadIdx.x & 31;
+    for (int64_t b = beg; b < end; b += 32) {  // (uniform)
+        const int64_t k = b + lane;
+        const unsigned long long v = k < end ? src[k] : (unsigned long long)G2PC_RANGE_EMPTY << 32;
+        int xlo, xhi, ylo, yhi;
+        g2pc_unpack_range((uint32_t)(v >> 32), xlo, xhi, ylo, yhi);
+        const bool some = xlo <= xhi && ylo <= yhi;
+        const int lo = LEVEL == 1 ? ylo : xlo, hi = LEVEL == 1 ? yhi : xhi;
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+            const uint32_t m = some ? span_bits(lo, hi, 32 * g) & member[g] : 0u;
+            if (G > 1 && !__any_sync(0xffffffffu, m != 0u)) continue;
+            const uint32_t bal = warp_transpose32(m);  // lanes whose entry falls in bucket 32 g + lane
+            if (COUNT) {
+                acc[g] += (uint32_t)__popc(bal);
+                continue;
+            }
+            uint32_t rem = bal, pos = acc[g];
+            while (__any_sync(0xffffffffu, rem != 0u)) {
+                const int s = rem ? __ffs(rem) - 1 : 0;
+                if (LEVEL == 1) {
+                    const uint32_t lo32 = __shfl_sync(0xffffffffu, (uint32_t)v, s);
+                    const uint32_t hi32 = __shfl_sync(0xffffffffu, (uint32_t)(v >> 32), s);
+                    if (rem) out(pos++, ((unsigned long long)hi32 << 32) | lo32);
+                } else {
+                    const uint32_t gid = __shfl_sync(0xffffffffu, (uint32_t)v, s);
+                    if (rem) out(pos++, (unsigned long long)gid);
+                }
+                rem &= rem - 1u;
+            }
+            acc[g] = pos;
+        }
+    }
+}
+
+// buckets of group g an entry may go to: level 1 the member rows, level 2 the cells of row `row` that are base-level
+// leaves (on a non-clean base level also member columns)
+template <int LEVEL, int G>
+__device__ __forceinline__ void split_members(const SplitParams& p, int row, uint32_t (&member)[G]) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+        const int c = 32 * g + lane;
+        bool in;
+        if (LEVEL == 1) {
+            in = c < p.rows && (p.clean || axis_member(p.tab.ys, p.tab.ye, p.tab.yf, c));
+        } else {
+            in = c < p.cols && (p.cell_leaf == nullptr || p.cell_leaf[row * p.cols + c] >= 0) &&
+                 (p.clean || axis_member(p.tab.xs, p.tab.xe, p.tab.xf, c));
+        }
+        member[g] = __ballot_sync(0xffffffffu, in);
+    }
+}
+
+// level-2 band -> its row (the last row whose first band is <= band) and the band's entries [beg, end) in row_list
+__device__ __forceinline__ int split_band_row(const SplitParams& p, int band, int64_t& beg, int64_t& end) {
+    int lo = 0, hi = p.rows - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if ((int)p.band_begin[mid] <= band) lo = mid; else hi = mid - 1;
+    }
+    beg = (int64_t)p.row_begin[lo] + (int64_t)(band - (int)p.band_begin[lo]) * SP_BAND;
+    end = min(beg + SP_BAND, (int64_t)p.row_begin[lo + 1]);
+    return lo;
+}
+
+// count: per warp tile, entries per bucket; per band, the tiles' exclusive offsets (m) and the band's totals (b)
+template <int LEVEL, int G>
+__global__ void __launch_bounds__(32 * SP_WARPS) split_count_kernel(const SplitParams p) {
+    __shared__ uint32_t s_cnt[SP_WARPS][32 * G];
+    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, band = blockIdx.x;
+    int64_t beg, end;
+    int row = 0;
+    if (LEVEL == 1) {
+        beg = (int64_t)band * SP_BAND;
+        end = min(beg + SP_BAND, p.n);
+    } else {
+        if (band >= (int)p.band_begin[p.rows]) return;  // (uniform: the launch covers the largest band count)
+        row = split_band_row(p, band, beg, end);
+    }
+    uint32_t member[G], cnt[G];
+    split_members<LEVEL, G>(p, row, member);
+#pragma unroll
+    for (int g = 0; g < G; ++g) cnt[g] = 0u;
+    const int64_t tb = beg + (int64_t)w * SP_TILE;
+    split_walk<LEVEL, G, true>(p, LEVEL == 1 ? p.val_sorted : p.row_list, tb, min(tb + SP_TILE, end), member, cnt,
+                               [](uint32_t, unsigned long long) {});
+#pragma unroll
+    for (int g = 0; g < G; ++g) s_cnt[w][32 * g + lane] = cnt[g];
+    __syncthreads();
+    const int width = 32 * G;
+    uint32_t* m = (LEVEL == 1 ? p.m1 : p.m2) + (int64_t)band * (SP_WARPS + 1) * width;
+    for (int c = threadIdx.x; c < width; c += 32 * SP_WARPS) {
+        uint32_t run = 0;
+#pragma unroll
+        for (int w2 = 0; w2 < SP_WARPS; ++w2) {
+            m[w2 * width + c] = run;
+            run += s_cnt[w2][c];
+        }
+        m[SP_WARPS * width + c] = run;
+        (LEVEL == 1 ? p.b1 : p.b2)[(int64_t)band * width + c] = run;
+    }
+}
+
+// scatter: every bucket starts at its band's offset + the tile's offset within the band.  A tile whose output fits
+// SP_STAGE_BYTES is first ranked into shared memory, bucket after bucket, then copied out one contiguous run per bucket
+// (coalesced stores; ranked straight into global memory every store of the warp hit 32 different runs).
+template <int LEVEL, int G>
+__global__ void __launch_bounds__(32 * SP_WARPS) split_scatter_kernel(const SplitParams p) {
+    using T = typename std::conditional<LEVEL == 1, unsigned long long, uint32_t>::type;
+    extern __shared__ __align__(16) unsigned char smem_sp[];
+    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, band = blockIdx.x;
+    int64_t beg, end;
+    int row = 0;
+    if (LEVEL == 1) {
+        beg = (int64_t)band * SP_BAND;
+        end = min(beg + SP_BAND, p.n);
+    } else {
+        if (band >= (int)p.band_begin[p.rows]) return;
+        row = split_band_row(p, band, beg, end);
+    }
+    const int64_t tb = beg + (int64_t)w * SP_TILE;
+    if (tb >= end) return;  // (uniform per warp; no barrier below)
+    const int width = 32 * G;
+    const uint32_t* m = (LEVEL == 1 ? p.m1 : p.m2) + ((int64_t)band * (SP_WARPS + 1) + w) * width;
+    const uint32_t* bo = (LEVEL == 1 ? p.b1 : p.b2) + (int64_t)band * width;
+    T* dst = LEVEL == 1 ? (T*)p.row_list : (T*)p.inst_gid;
+    uint32_t member[G], off[G], cnt[G], sbeg[G], pos[G];
+    split_members<LEVEL, G>(p, row, member);
+    uint32_t total = 0;
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+        const uint32_t m0 = m[32 * g + lane];
+        off[g] = bo[32 * g + lane] + m0;
+        cnt[g] = m[width + 32 * g + lane] - m0;
+        // exclusive scan of the counts over the buckets: where the bucket's run starts in the staging area
+        uint32_t inc = cnt[g];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += t;
+        }
+        sbeg[g] = total + inc - cnt[g];
+        total += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    const int64_t te = min(tb + SP_TILE, end);
+    constexpr int CAP = SP_STAGE_BYTES / (int)sizeof(T);
+    if (total > (uint32_t)CAP) {  // (uniform) a tile of wide splats: rank straight into global memory
+        split_walk<LEVEL, G, false>(p, LEVEL == 1 ? p.val_sorted : p.row_list, tb, te, member, off,
+                                    [&](uint32_t q, unsigned long long x) { dst[q] = (T)x; });
+        return;
+    }
+    T* stage = reinterpret_cast<T*>(smem_sp + w * SP_STAGE_BYTES);
+#pragma unroll
+    for (int g = 0; g < G; ++g) pos[g] = sbeg[g];
+    split_walk<LEVEL, G, false>(p, LEVEL == 1 ? p.val_sorted : p.row_list, tb, te, member, pos,
+                                [&](uint32_t q, unsigned long long x) { stage[q] = (T)x; });
+    __syncwarp();
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+        unsigned todo = __ballot_sync(0xffffffffu, cnt[g] != 0u);
+        while (todo) {
+            const int b = __ffs(todo) - 1;
+            todo &= todo - 1u;
+            const uint32_t len = __shfl_sync(0xffffffffu, cnt[g], b), s0 = __shfl_sync(0xffffffffu, sbeg[g], b);
+            const uint32_t d0 = __shfl_sync(0xffffffffu, off[g], b);
+            for (uint32_t k = lane; k < len; k += 32) dst[d0 + k] = stage[s0 + k];
+        }
+    }
+}
+
+// Level-1 scan (one CTA): per row, the total over the bands; the rows' list offsets and level-2 band layout; every band
+// total of b1 rewritten as the absolute offset of the band's first entry in its row.  Row lists that do not fit
+// row_capacity fail the frame (CAP_OVERFLOW, the row-list size in ROW_INST: the caller grows the buffer and replays).
+__global__ void __launch_bounds__(1024) split_rows_scan_kernel(const SplitParams p) {
+    __shared__ uint32_t s_part[SP_MAX_GROUPS][32][33];
+    __shared__ uint32_t s_begin[SP_MAX_CELLS];
+    __shared__ int s_over;
+    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    if (p.base_split) {
+        int split = 0;
+        for (int i = threadIdx.x; i < p.rows * p.cols; i += 1024) split |= p.cell_leaf[i] == -2;
+        split = __syncthreads_or(split);
+        if (threadIdx.x == 0) *p.base_split = split ? 1u : 0u;
+    }
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const int groups = p.rows_p / 32;
+    const int per = (p.bands1 + 31) / 32;
+    const int c0 = min(p.bands1, ty * per), c1 = min(p.bands1, c0 + per);
+    for (int g = 0; g < groups; ++g) {
+        const uint32_t* col = p.b1 + 32 * g + tx;
+        uint32_t sum = 0;
+#pragma unroll 8
+        for (int c = c0; c < c1; ++c) sum += col[(int64_t)c * p.rows_p];
+        s_part[g][ty][tx] = sum;
+    }
+    __syncthreads();
+    if (ty == 0) {
+        // warp 0: row totals, then an exclusive scan over the rows (each lane takes 8 consecutive rows)
+        unsigned long long tot[SP_MAX_GROUPS], bands[SP_MAX_GROUPS], st = 0, sb = 0;
+#pragma unroll
+        for (int i = 0; i < SP_MAX_GROUPS; ++i) {
+            const int r = tx * SP_MAX_GROUPS + i;
+            uint32_t t = 0;
+            if (r < p.rows)
+                for (int s = 0; s < 32; ++s) t += s_part[r >> 5][s][r & 31];
+            tot[i] = t;
+            bands[i] = (t + SP_BAND - 1) / SP_BAND;
+            st += tot[i];
+            sb += bands[i];
+        }
+        unsigned long long it = st, ib = sb;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long a = __shfl_up_sync(0xffffffffu, it, o), b = __shfl_up_sync(0xffffffffu, ib, o);
+            if (tx >= o) { it += a; ib += b; }
+        }
+        unsigned long long rt = it - st, rb = ib - sb;
+        const unsigned long long total = __shfl_sync(0xffffffffu, it, 31);
+        const bool over = total > (unsigned long long)p.row_capacity;
+        if (!over) {
+#pragma unroll
+            for (int i = 0; i < SP_MAX_GROUPS; ++i) {
+                const int r = tx * SP_MAX_GROUPS + i;
+                if (r < p.rows) {
+                    p.row_begin[r] = (uint32_t)rt;
+                    p.band_begin[r] = (uint32_t)rb;
+                    s_begin[r] = (uint32_t)rt;
+                }
+                rt += tot[i];
+                rb += bands[i];
+            }
+            if (tx == 31) {
+                p.row_begin[p.rows] = (uint32_t)rt;
+                p.band_begin[p.rows] = (uint32_t)rb;
+            }
+        }
+        if (tx == 0) {
+            s_over = over ? 1 : 0;
+            p.header[G2PC_HDR_ROW_INST] = (int32_t)min(total, 0x7FFFFFFFull);
+            if (over) {
+                p.header[G2PC_HDR_CAP_OVERFLOW] = 1;
+                atomicMin(p.fail, (uint32_t)(p.frame + 1));
+                p.header[G2PC_HDR_POISON] = (int32_t)*(volatile uint32_t*)p.fail;
+            }
+        }
+    }
+    __syncthreads();
+    if (s_over) return;
+    for (int g = 0; g < groups; ++g) {
+        const int r = 32 * g + tx;
+        if (r >= p.rows) continue;
+        uint32_t run = s_begin[r];
+        for (int s = 0; s < ty; ++s) run += s_part[g][s][tx];
+        uint32_t* col = p.b1 + r;
+        for (int c = c0; c < c1; ++c) {
+            const uint32_t t = col[(int64_t)c * p.rows_p];
+            col[(int64_t)c * p.rows_p] = run;
+            run += t;
+        }
+    }
+}
+
+// Level-2 scan: one thread per cell (row, column): its bands' totals rewritten as the absolute offset of each band's
+// first id in the leaf's list (starting at the leaf's inst_begin).
+__global__ void __launch_bounds__(256) split_cols_scan_kernel(const SplitParams p) {
+    if (g2pc_frame_skipped(p.fail, p.frame)) return;
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    const int row = i / p.cols_p, c = i - row * p.cols_p;
+    if (row >= p.rows) return;
+    uint32_t run = 0;
+    if (c < p.cols) {
+        const int leaf = p.cell_leaf ? p.cell_leaf[row * p.cols + c] : row * p.cols + c;
+        if (leaf >= 0) run = (uint32_t)p.leaves[leaf].inst_begin;
+    }
+    const int b0 = (int)p.band_begin[row], b1 = (int)p.band_begin[row + 1];
+    uint32_t* col = p.b2 + c;
+    for (int b = b0; b < b1; ++b) {
+        const uint32_t t = col[(int64_t)b * p.cols_p];
+        col[(int64_t)b * p.cols_p] = run;
+        run += t;
+    }
+}
+
 size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+int64_t split_bands1(int64_t n) { return (n + SP_BAND - 1) / SP_BAND; }
+int64_t split_bands2(int64_t row_capacity, int rows) { return (row_capacity + SP_BAND - 1) / SP_BAND + rows; }
+
+// workspace of the two splits: [base_split][row_list][m1][b1][m2][b2][row_begin][band_begin], each 256-byte aligned
+int64_t split_workspace_bytes(int64_t n, int64_t row_capacity, int rows, int cols) {
+    const int64_t rp = (rows + 31) / 32 * 32, cp = (cols + 31) / 32 * 32;
+    const int64_t b1 = split_bands1(n), b2 = split_bands2(row_capacity, rows);
+    return (int64_t)(align256(4) + align256((size_t)row_capacity * 8) + align256((size_t)(b1 * (SP_WARPS + 1) * rp * 4)) +
+                     align256((size_t)(b1 * rp * 4)) + align256((size_t)(b2 * (SP_WARPS + 1) * cp * 4)) +
+                     align256((size_t)(b2 * cp * 4)) + 2 * align256((size_t)(rows + 1) * 4));
+}
+
+template <int LEVEL, int G>
+void split_launch_level(const SplitParams& p, int64_t bands, cudaStream_t st) {
+    split_count_kernel<LEVEL, G><<<(unsigned)bands, 32 * SP_WARPS, 0, st>>>(p);
+    if (LEVEL == 1) split_rows_scan_kernel<<<1, 1024, 0, st>>>(p);
+    else split_cols_scan_kernel<<<(unsigned)((p.rows * p.cols_p + 255) / 256), 256, 0, st>>>(p);
+    constexpr size_t smem = (size_t)SP_WARPS * SP_STAGE_BYTES;
+    cudaFuncSetAttribute(split_scatter_kernel<LEVEL, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    split_scatter_kernel<LEVEL, G><<<(unsigned)bands, 32 * SP_WARPS, smem, st>>>(p);
+}
+
+template <int LEVEL>
+void split_level(const SplitParams& p, int64_t bands, cudaStream_t st) {
+    switch ((LEVEL == 1 ? p.rows_p : p.cols_p) / 32) {
+        case 1: split_launch_level<LEVEL, 1>(p, bands, st); break;
+        case 2: split_launch_level<LEVEL, 2>(p, bands, st); break;
+        case 3: split_launch_level<LEVEL, 3>(p, bands, st); break;
+        case 4: split_launch_level<LEVEL, 4>(p, bands, st); break;
+        case 5: split_launch_level<LEVEL, 5>(p, bands, st); break;
+        case 6: split_launch_level<LEVEL, 6>(p, bands, st); break;
+        case 7: split_launch_level<LEVEL, 7>(p, bands, st); break;
+        default: split_launch_level<LEVEL, 8>(p, bands, st); break;
+    }
+}
+
+// The base-level lists of an n-entry stream over a rows x cols grid (both <= 256).  Returns G2PC_OK or an error code.
+int run_split(SplitParams p, void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+    if (workspace_bytes < split_workspace_bytes(p.n, p.row_capacity, p.rows, p.cols)) {
+        g2pc_set_error("g2pc_multisplit: workspace smaller than g2pc_multisplit_workspace_bytes");
+        return G2PC_ERR_WORKSPACE;
+    }
+    p.rows_p = (p.rows + 31) / 32 * 32;
+    p.cols_p = (p.cols + 31) / 32 * 32;
+    const int64_t b1 = split_bands1(p.n), b2 = split_bands2(p.row_capacity, p.rows);
+    char* ws = (char*)workspace;
+    auto take = [&](size_t bytes) { char* q = ws; ws += align256(bytes); return q; };
+    uint32_t* flag = (uint32_t*)take(4);
+    p.base_split = p.cell_leaf ? flag : nullptr;
+    p.row_list = (unsigned long long*)take((size_t)p.row_capacity * 8);
+    p.m1 = (uint32_t*)take((size_t)(b1 * (SP_WARPS + 1) * p.rows_p * 4));
+    p.b1 = (uint32_t*)take((size_t)(b1 * p.rows_p * 4));
+    p.m2 = (uint32_t*)take((size_t)(b2 * (SP_WARPS + 1) * p.cols_p * 4));
+    p.b2 = (uint32_t*)take((size_t)(b2 * p.cols_p * 4));
+    p.row_begin = (uint32_t*)take((size_t)(p.rows + 1) * 4);
+    p.band_begin = (uint32_t*)take((size_t)(p.rows + 1) * 4);
+    p.bands1 = (int32_t)b1;
+    split_level<1>(p, b1, st);
+    split_level<2>(p, b2, st);
+    G2PC_CHECK_LAUNCH();
+    return G2PC_OK;
+}
+
 
 // Sub-steps per chunk for n entries: as many as keep about MS_TARGET_CTAS chunks, ~10 waves of the 3 scatter CTAs an SM
 // of an H100 SXM (132 SMs) holds at C = 256.  Measured at 3 M Gaussians / 1280x720 (count + scatter per camera, H100
@@ -458,7 +867,7 @@ int32_t ms_chunks(int64_t n, int C) {
 
 template <int C>
 int launch_multisplit(const MsParams& p, int32_t chunks, cudaStream_t st) {
-    const size_t common = p.grid_w > 0 ? 0 : ((size_t)6 * p.n1 + ((size_t)1 << (2 * p.base_level))) * sizeof(int32_t);
+    const size_t common = ((size_t)6 * p.n1 + ((size_t)1 << (2 * p.base_level))) * sizeof(int32_t);
     const size_t smem_count = common + (size_t)p.leaf_cap * sizeof(uint32_t);
     const size_t smem_scatter = common + (size_t)(C / 32 + 1) * p.leaf_cap * sizeof(uint32_t);
     if (smem_scatter > 200 * 1024 || smem_count > 200 * 1024) {
@@ -558,52 +967,75 @@ extern "C" int32_t g2pc_multisplit_rows(int64_t n, int32_t leaf_cap) {
     return ms_chunks(n, C);
 }
 
+extern "C" int64_t g2pc_multisplit_workspace_bytes(int64_t n, int64_t row_capacity, int32_t grid_w, int32_t grid_h) {
+    if (n < 0 || row_capacity < 0 || grid_w < 1 || grid_h < 1 || grid_w > SP_MAX_CELLS || grid_h > SP_MAX_CELLS) return -1;
+    return split_workspace_bytes(n, row_capacity, grid_h, grid_w);
+}
+
 extern "C" int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void* proj, int32_t width, int32_t height,
                                const int32_t* tables, int32_t num_levels, uint32_t level_mask, uint32_t clean_mask,
-                               const int32_t* node_leaf,
-                               const g2pc_leaf_t* leaves, const int32_t* header, const uint32_t* fail, int32_t frame,
-                               int32_t leaf_cap, uint32_t* matrix, uint32_t* inst_gid, void* stream) {
+                               const int32_t* node_leaf, const g2pc_leaf_t* leaves, int32_t* header,
+                               const uint32_t* fail, int32_t frame, int32_t leaf_cap, uint32_t* matrix,
+                               int64_t row_capacity, void* workspace, int64_t workspace_bytes, uint32_t* inst_gid,
+                               void* stream) {
     G2PC_CHECK_ARG(n >= 0, "n < 0");
     if (n == 0) return G2PC_OK;
-    G2PC_CHECK_ARG(val_sorted && proj && tables && node_leaf && leaves && header && fail && matrix && inst_gid,
+    G2PC_CHECK_ARG(val_sorted && proj && tables && node_leaf && leaves && header && fail && workspace && inst_gid,
                    "null pointer");
     G2PC_CHECK_ARG(num_levels >= 1 && num_levels <= G2PC_MAX_LEVELS && level_mask != 0u, "bad levels");
+    G2PC_CHECK_ARG(row_capacity >= 0 && row_capacity <= 0x7FFFFFFFll, "bad row capacity");
+    const int base = __builtin_ctz(level_mask);
+    G2PC_CHECK_ARG(base <= G2PC_RANGE_MAX_LEVEL, "first leaf-candidate level too deep");
+    const int n1 = (1 << num_levels) - 1, o1 = (1 << base) - 1;
+    const QtTables tab = make_tables(tables, n1);
+    cudaStream_t st = (cudaStream_t)stream;
+    SplitParams s{};
+    s.val_sorted = (const unsigned long long*)val_sorted; s.n = n;
+    s.rows = s.cols = 1 << base;
+    s.cell_leaf = node_leaf + off2d(base);
+    s.tab.xs = tab.xs + o1; s.tab.xe = tab.xe + o1; s.tab.xf = tab.xf + o1;
+    s.tab.ys = tab.ys + o1; s.tab.ye = tab.ye + o1; s.tab.yf = tab.yf + o1;
+    s.clean = (int32_t)((clean_mask >> base) & 1u);
+    s.leaves = leaves; s.header = header; s.fail = const_cast<uint32_t*>(fail); s.frame = frame;
+    s.row_capacity = row_capacity; s.inst_gid = inst_gid;
+    const int rc = run_split(s, workspace, workspace_bytes, st);
+    if (rc != G2PC_OK || num_levels <= base + 1) return rc;
+    // leaves below the base level (count-driven splits): the chunked multisplit
     const int C = g2pc_multisplit_chunk(leaf_cap);
     G2PC_CHECK_ARG(C > 0, "too many leaves for the multisplit");
+    G2PC_CHECK_ARG(matrix, "null matrix with levels below the base level");
     MsParams p;
     p.val_sorted = (const unsigned long long*)val_sorted; p.n = n; p.proj = (const float4*)proj;
     p.width = width; p.height = height;
     p.inv_width = 1.0f / (float)width; p.inv_height = 1.0f / (float)height;
     p.meta.num_levels = num_levels; p.meta.max_gaussians_per_tile = 0; p.meta.width = width; p.meta.height = height;
-    p.n1 = (1 << num_levels) - 1;
-    p.tab = make_tables(tables, p.n1);
-    p.level_mask = level_mask; p.base_level = __builtin_ctz(level_mask);
-    G2PC_CHECK_ARG(p.base_level <= G2PC_RANGE_MAX_LEVEL, "first leaf-candidate level too deep");
+    p.n1 = n1;
+    p.tab = tab;
+    p.level_mask = level_mask; p.base_level = base;
     p.node_leaf = node_leaf; p.header = header; p.fail = fail; p.frame = frame; p.leaves = leaves; p.matrix = matrix;
     p.inst_gid = inst_gid;
-    p.leaf_cap = leaf_cap; p.grid_w = 0;
-    p.base_clean = (int32_t)((clean_mask >> p.base_level) & 1u);
+    p.leaf_cap = leaf_cap;
+    p.base_clean = s.clean;
     p.clean_mask = clean_mask;
-    return run_multisplit(p, C, (cudaStream_t)stream);
+    p.base_split = (const uint32_t*)workspace;  // (first word of the workspace, run_split)
+    return run_multisplit(p, C, st);
 }
 
-/* The same multisplit over a flat grid of tiles (s7_tiles.cu): leaf = tile index, the packed range is the tile rect. */
+/* The same lists over a flat grid of tiles (s7_tiles.cu): leaf = tile index, the packed range is the tile rect. */
 extern "C" int g2pc_multisplit_grid(const uint64_t* val_sorted, int64_t n, int32_t grid_w, int32_t grid_h,
-                                    const g2pc_leaf_t* leaves, const int32_t* header, const uint32_t* fail,
-                                    int32_t frame, int32_t leaf_cap, uint32_t* matrix, uint32_t* inst_gid, void* stream) {
+                                    const g2pc_leaf_t* leaves, int32_t* header, const uint32_t* fail, int32_t frame,
+                                    int64_t row_capacity, void* workspace, int64_t workspace_bytes, uint32_t* inst_gid,
+                                    void* stream) {
     G2PC_CHECK_ARG(n >= 0, "n < 0");
     if (n == 0) return G2PC_OK;
-    G2PC_CHECK_ARG(val_sorted && leaves && header && fail && matrix && inst_gid, "null pointer");
-    G2PC_CHECK_ARG(grid_w >= 1 && grid_h >= 1 && grid_w <= 256 && grid_h <= 256 && leaf_cap >= grid_w * grid_h,
-                   "bad tile grid / leaf_cap");
-    const int C = g2pc_multisplit_chunk(leaf_cap);
-    G2PC_CHECK_ARG(C > 0, "too many tiles for the multisplit");
-    MsParams p{};  // no projection records, quadtree tables or node -> leaf map: the grid is one level of tiles
-    p.val_sorted = (const unsigned long long*)val_sorted; p.n = n;
-    p.meta.num_levels = 1;
-    p.level_mask = 1u;
-    p.header = header; p.fail = fail; p.frame = frame; p.leaves = leaves; p.matrix = matrix;
-    p.inst_gid = inst_gid;
-    p.leaf_cap = leaf_cap; p.grid_w = grid_w; p.base_clean = 1; p.clean_mask = 1u;
-    return run_multisplit(p, C, (cudaStream_t)stream);
+    G2PC_CHECK_ARG(val_sorted && leaves && header && fail && workspace && inst_gid, "null pointer");
+    G2PC_CHECK_ARG(grid_w >= 1 && grid_h >= 1 && grid_w <= SP_MAX_CELLS && grid_h <= SP_MAX_CELLS, "bad tile grid");
+    G2PC_CHECK_ARG(row_capacity >= 0 && row_capacity <= 0x7FFFFFFFll, "bad row capacity");
+    SplitParams s{};  // no quadtree tables or node -> leaf map: every cell is a leaf, every range is exact
+    s.val_sorted = (const unsigned long long*)val_sorted; s.n = n;
+    s.rows = grid_h; s.cols = grid_w;
+    s.clean = 1;
+    s.leaves = leaves; s.header = header; s.fail = const_cast<uint32_t*>(fail); s.frame = frame;
+    s.row_capacity = row_capacity; s.inst_gid = inst_gid;
+    return run_split(s, workspace, workspace_bytes, (cudaStream_t)stream);
 }

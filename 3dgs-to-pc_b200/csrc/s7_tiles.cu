@@ -8,9 +8,9 @@
 //   rasterizer_impl.cu:69-137,285-326        duplicateWithKeys / radix sort / identifyTileRanges  -> per-tile depth-ordered lists
 //   forward.cu:303-497      renderCUDA       (blend, max contribution :434-456, surface distance :460-477, mask :334,389,485)
 //   gaussian_pointcloud_rasterization/__init__.py:126-158   per-camera accumulator updates
-// Nothing of their structure is kept: the depth-ordered lists come from the same depth sort + bit-matrix multisplit as the
-// python-semantics path (s4_tree.cu), built per SUPER-TILE of 2x2 tiles (32x32 pixels: 900 lists at 1280x720 instead of
-// 3600 — the multisplit's cost grows with the number of lists); the blend of a tile walks its super-tile's list and skips
+// Nothing of their structure is kept: the depth-ordered lists come from the same depth sort + row / column multisplit as
+// the python-semantics path (s4_tree.cu), built per SUPER-TILE of 2x2 tiles (32x32 pixels: 900 lists at 1280x720 instead
+// of 3600 — fewer, longer lists); the blend of a tile walks its super-tile's list and skips
 // the entries whose tile rect (packed into the projection record) does not contain the tile, so every tile still sees
 // exactly its own list, in order, and the 256-entry rounds of the surface distance count the tile's own entries;
 // the blend is a persistent kernel with TMA-staged id chunks and cp.async record gathers (scalar FP32: the per-pixel keep /

@@ -144,8 +144,10 @@ SIGNATURES = {
                          _i64, _i32, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_multisplit_chunk": ([_i32], ctypes.c_int32),
     "g2pc_multisplit_rows": ([_i64, _i32], ctypes.c_int32),
+    "g2pc_multisplit_workspace_bytes": ([_i64, _i64, _i32, _i32], ctypes.c_int64),
     "g2pc_multisplit": ([_c_void_p, _i64, _c_void_p, _i32, _i32, _c_void_p, _i32, _u32, _u32, _c_void_p, _c_void_p,
-                         _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
+                         _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p],
+                        ctypes.c_int),
     "g2pc_blend": ([_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _i32, _c_void_p, _c_void_p, _c_void_p,
                     _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _f32, _f32, _c_void_p, _c_void_p, _c_void_p],
                    ctypes.c_int),
@@ -156,7 +158,7 @@ SIGNATURES = {
                                _c_void_p, _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_tiles_build": ([_c_void_p, _i32, _i32, _c_void_p, _c_void_p, _i32, _i64, _i64, _i32, _i32, _c_void_p,
                           _c_void_p, _c_void_p, _c_void_p], ctypes.c_int),
-    "g2pc_multisplit_grid": ([_c_void_p, _i64, _i32, _i32, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _c_void_p,
+    "g2pc_multisplit_grid": ([_c_void_p, _i64, _i32, _i32, _c_void_p, _c_void_p, _c_void_p, _i32, _i64, _c_void_p, _i64,
                               _c_void_p, _c_void_p], ctypes.c_int),
     "g2pc_tiles_blend": ([_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                           _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32, _c_void_p, _c_void_p, _c_void_p,
@@ -184,7 +186,7 @@ class Camera(ctypes.Structure):
 
 
 (HDR_NUM_LEAVES, HDR_TOTAL_INST, HDR_TOTAL_PIX, HDR_NEED_DEEPER, HDR_LEAF_OVERFLOW, HDR_CAP_OVERFLOW, HDR_POISON,
- HDR_FRAME, HDR_TOTAL_INST_HI) = range(9)
+ HDR_FRAME, HDR_TOTAL_INST_HI, HDR_ROW_INST) = range(10)
 HDR_WORDS = 16
 WORK_COUNTERS = 4
 STAT_WARP_GAUSSIANS, STAT_WORDS = 0, 4
@@ -222,8 +224,9 @@ LAUNCHES = 0      # number of hand-written g2pc kernels launched since the last 
 TIMING = None     # None, or a dict filled as {entry point name: [(start_event, end_event), ...]}: every launch is
                   # bracketed with CUDA events on the current stream (bench.py)
 # hand-written kernels launched per entry point (default 1); the radix sorts and selections inside g2pc_depth_sort,
-# the k-NN and the orientation entry points are cub's (library)
-_OWN_KERNELS = {"g2pc_multisplit": 3, "g2pc_multisplit_grid": 3, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
+# the k-NN and the orientation entry points are cub's (library); g2pc_multisplit launches 3 more on a table with levels
+# below the base level
+_OWN_KERNELS = {"g2pc_multisplit": 6, "g2pc_multisplit_grid": 6, "g2pc_depth_sort": 0, "g2pc_cull_select": 3,
                 "g2pc_points_per_gaussian": 5, "g2pc_knn_mean_dist": 6, "g2pc_knn_ids": 6, "g2pc_sor_mask": 5, "g2pc_mesh_splat": 5,
                 "g2pc_mesh_iso": 7, "g2pc_mesh_extract_count": 2, "g2pc_mesh_extract_emit": 2, "g2pc_mesh_gather": 3,
                 "g2pc_mesh_trim": 6, "g2pc_mesh_normals": 3, "g2pc_mesh_band_bricks": 4, "g2pc_mesh_band_cg_start": 4,

@@ -73,7 +73,7 @@ class FrameQueue:
                             depth_ws=torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev),
                             hdr=torch.zeros((capi.HDR_WORDS,), dtype=torch.int32, device=dev),
                             work=torch.zeros((capi.WORK_COUNTERS,), dtype=torch.int32, device=dev),
-                            inst_gid=None, matrix=None) for _ in range(self.num_slots)]
+                            inst_gid=None, matrix=None, ms_ws=None) for _ in range(self.num_slots)]
         # per-camera projection outputs of the batch sets; camera 0 of set s is slot s's own (allocated when first used)
         self._pre_sets = [[sl] + [None] * (preprocess_cameras - 1) for sl in self._slots]
         self._set_free = [None] * self.num_slots  # end event of the last frame that read each batch set
@@ -82,18 +82,24 @@ class FrameQueue:
         self._stats = torch.zeros((capi.STAT_WORDS,), dtype=torch.int64, device=dev)
         # (Gaussian, tile) instances the lists hold, grown when a frame does not fit
         self._inst_cap = max(8 * self._n, 1 << 16)
+        # entries of the multisplit's row lists (one per Gaussian and base-level row it covers), grown the same way
+        self._row_cap = max(4 * self._n, 1 << 16)
         self._tables = {}
         self._last_slot = 0
         self.last_stats = {}
 
-    def _grow_lists(self, sl, leaf_cap, rows):
-        """Grow the slot's depth-ordered lists and multisplit matrix (rows x leaf_cap) to the current capacities."""
+    def _grow_lists(self, sl, leaf_cap, rows, grid):
+        """Grow the slot's depth-ordered lists, multisplit matrix (rows x leaf_cap; 0 rows: none) and the multisplit
+        workspace of the base-level grid (grid_w, grid_h) to the current capacities."""
         need = self._inst_cap + 4 * leaf_cap + 64  # lists are padded to 16 bytes; slack for the last TMA unit
         if sl["inst_gid"] is None or sl["inst_gid"].numel() < need:
             sl["inst_gid"] = torch.empty((need,), dtype=torch.int32, device=self.device)
         mneed = rows * leaf_cap
-        if sl["matrix"] is None or sl["matrix"].numel() < mneed:
-            sl["matrix"] = torch.empty((max(mneed, 1),), dtype=torch.int32, device=self.device)
+        if mneed > 0 and (sl["matrix"] is None or sl["matrix"].numel() < mneed):
+            sl["matrix"] = torch.empty((mneed,), dtype=torch.int32, device=self.device)
+        wneed = int(self.lib.g2pc_multisplit_workspace_bytes(max(self._n, 1), self._row_cap, *grid))
+        if sl["ms_ws"] is None or sl["ms_ws"].numel() < wneed:
+            sl["ms_ws"] = capi.workspace(wneed, self.device)
 
     def _depth_sort(self, sl, stream, pre=None):
         """Enqueue the depth sort, into the slot's val_sorted, of the (depth key, value) pairs the preprocess wrote into
@@ -109,6 +115,14 @@ class FrameQueue:
         if total > 0x7FFFFFFF:
             raise capi.G2pcError(f"{total} (Gaussian, tile) instances in one camera: more than 2^31 - 1")
         self._inst_cap = max(self._inst_cap, int(1.25 * total) + 1024)
+
+    def _grow_row_cap(self, h):
+        """A frame's row lists did not fit the multisplit workspace: raise its capacity (the next _launch_batch grows
+        the buffers)."""
+        need = h[capi.HDR_ROW_INST]
+        if need >= 0x7FFFFFFF:
+            raise capi.G2pcError("2^31 - 1 or more row-list entries in one camera")
+        self._row_cap = max(self._row_cap, min(int(1.25 * need) + 1024, 0x7FFFFFFF))
 
     def _reset_counts(self):
         """Zero the per-slot tile counters of every table set (a failed frame left its counts behind)."""

@@ -162,10 +162,9 @@ class GaussianRasterizer(FrameQueue):
             # the depth-ordered lists are built per super-tile of 2x2 tiles (csrc/s7_tiles.cu)
             gx, gy = ((W + TILE - 1) // TILE + 1) // 2, ((H + TILE - 1) // TILE + 1) // 2
             ntiles = gx * gy
-            chunk = int(self.lib.g2pc_multisplit_chunk(ntiles))
-            if chunk <= 0:
-                raise capi.G2pcError(f"{ntiles} tiles: image too large for the multisplit tables")
-            t = dict(gx=gx, gy=gy, ntiles=ntiles, rows=int(self.lib.g2pc_multisplit_rows(self._n, ntiles)),
+            if gx > 256 or gy > 256:
+                raise capi.G2pcError(f"{gx} x {gy} super-tiles: image too large for the multisplit (256 per axis)")
+            t = dict(gx=gx, gy=gy, ntiles=ntiles,
                      slots=[dict(node_cnt=torch.zeros((ntiles,), dtype=torch.int32, device=dev),
                                  leaves=torch.zeros((ntiles, capi.LEAF_WORDS), dtype=torch.int32, device=dev),
                                  leaf_order=torch.zeros((ntiles,), dtype=torch.int32, device=dev))
@@ -189,7 +188,7 @@ class GaussianRasterizer(FrameQueue):
     def _ensure_buffers(self, rs, slot):
         self._pack(float(rs.scale_modifier))
         t = self._res_tables(int(rs.image_width), int(rs.image_height))
-        self._grow_lists(self._slots[slot], t["ntiles"], t["rows"])
+        self._grow_lists(self._slots[slot], t["ntiles"], 0, (t["gx"], t["gy"]))
         # (kept per slot: the tensor must outlive the frame's kernels, the slot is reused only after they have run)
         self._slots[slot]["mask"] = self._mask_of(rs, int(rs.image_width), int(rs.image_height))
 
@@ -208,11 +207,11 @@ class GaussianRasterizer(FrameQueue):
                   capi.ptr(sl["radii"]), st)
         self._depth_sort(sl, st)
         capi.call("g2pc_tiles_build", capi.ptr(ts["node_cnt"]), W, H, capi.ptr(ts["leaves"]), capi.ptr(ts["leaf_order"]),
-                  t["ntiles"], self._inst_cap, sl["matrix"].numel(), t["rows"], frame, capi.ptr(sl["hdr"]),
+                  t["ntiles"], self._inst_cap, 0, 0, frame, capi.ptr(sl["hdr"]),
                   capi.ptr(self._fail), capi.ptr(sl["work"]), st)
         capi.call("g2pc_multisplit_grid", capi.ptr(sl["val_sorted"]), n, t["gx"], t["gy"], capi.ptr(ts["leaves"]),
-                  capi.ptr(sl["hdr"]), capi.ptr(self._fail), frame, t["ntiles"], capi.ptr(sl["matrix"]),
-                  capi.ptr(sl["inst_gid"]), st)
+                  capi.ptr(sl["hdr"]), capi.ptr(self._fail), frame, self._row_cap, capi.ptr(sl["ms_ws"]),
+                  sl["ms_ws"].numel(), capi.ptr(sl["inst_gid"]), st)
         self._last, self._last_slot = t, slot
         return sl["hdr"]
 
@@ -256,6 +255,7 @@ class GaussianRasterizer(FrameQueue):
         if not h[capi.HDR_CAP_OVERFLOW]:
             raise capi.G2pcError("failed frame header without a recoverable cause")
         self._grow_inst_cap(h)
+        self._grow_row_cap(h)
 
     # ---- accumulator updates kept for API parity (the kernels fuse them) -------------------------------------------------
     def update_max_contributions(self, new_gauss_contributions, new_gauss_colours):

@@ -151,7 +151,9 @@ class GaussPythonRenderer(FrameQueue):
         if chunk <= 0:
             raise capi.G2pcError(f"the quadtree has more than {cap} leaves: too many for the multisplit tables")
         t["leaf_cap"], t["chunk"] = cap, chunk
-        t["chunks"] = int(self.lib.g2pc_multisplit_rows(self._n, cap))  # matrix rows: one per multisplit chunk
+        # matrix rows of the multisplit below the base level (one per chunk); none without such levels
+        deeper = t["qt"].num_levels > t["base_level"] + 1
+        t["chunks"] = int(self.lib.g2pc_multisplit_rows(self._n, cap)) if deeper else 0
         for ts in t["slots"]:
             ts["leaves"] = torch.zeros((cap, capi.LEAF_WORDS), dtype=torch.int32, device=self.device)
             ts["leaf_order"] = torch.zeros((cap,), dtype=torch.int32, device=self.device)
@@ -182,7 +184,7 @@ class GaussPythonRenderer(FrameQueue):
     def _ensure_buffers(self, camera, slot):
         """(Re)allocate the slot's frame buffers for the current capacities."""
         t = self._get_tables(int(camera.image_width), int(camera.image_height))
-        self._grow_lists(self._slots[slot], t["leaf_cap"], t["chunks"])
+        self._grow_lists(self._slots[slot], t["leaf_cap"], t["chunks"], (1 << max(t["base_level"], 0),) * 2)
         if self._leaf_colour is None or self._leaf_colour.numel() < 3 * t["pix_cap"]:
             self._leaf_colour = torch.empty((3 * t["pix_cap"],), dtype=torch.float32, device=self.device)
 
@@ -222,12 +224,14 @@ class GaussPythonRenderer(FrameQueue):
         self._depth_sort(sl, st, ps)
         capi.call("g2pc_build_tree", capi.ptr(t["tables"]), qt.num_levels, qt.max_gaussians_per_tile,
                   capi.ptr(node_cnt), capi.ptr(ts["node_state"]), capi.ptr(ts["node_leaf"]), capi.ptr(ts["leaves"]),
-                  capi.ptr(ts["leaf_order"]), t["leaf_cap"], self._inst_cap, t["pix_cap"], sl["matrix"].numel(),
+                  capi.ptr(ts["leaf_order"]), t["leaf_cap"], self._inst_cap, t["pix_cap"],
+                  sl["matrix"].numel() if t["chunks"] else 0,
                   t["chunks"], frame, capi.ptr(sl["hdr"]), capi.ptr(self._fail), capi.ptr(sl["work"]), st)
         capi.call("g2pc_multisplit", capi.ptr(sl["val_sorted"]), n, capi.ptr(ps["proj"]), W, H, capi.ptr(t["tables"]),
                   qt.num_levels, t["level_mask"], t["clean_mask"], capi.ptr(ts["node_leaf"]), capi.ptr(ts["leaves"]),
                   capi.ptr(sl["hdr"]),
-                  capi.ptr(self._fail), frame, t["leaf_cap"], capi.ptr(sl["matrix"]), capi.ptr(sl["inst_gid"]), st)
+                  capi.ptr(self._fail), frame, t["leaf_cap"], capi.ptr(sl["matrix"]) if t["chunks"] else None,
+                  self._row_cap, capi.ptr(sl["ms_ws"]), sl["ms_ws"].numel(), capi.ptr(sl["inst_gid"]), st)
         self._last_tables, self._last_slot = t, slot
         return sl["hdr"]
 
@@ -290,6 +294,7 @@ class GaussPythonRenderer(FrameQueue):
             self._set_leaf_cap(t, max(2 * t["leaf_cap"], int(1.25 * h[capi.HDR_NUM_LEAVES])))
         elif h[capi.HDR_CAP_OVERFLOW]:
             self._grow_inst_cap(h)
+            self._grow_row_cap(h)
             t["pix_cap"] = max(t["pix_cap"], int(1.25 * h[capi.HDR_TOTAL_PIX]) + 1024)
         else:
             raise capi.G2pcError("poisoned frame header without a cause")

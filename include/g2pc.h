@@ -451,11 +451,14 @@ typedef struct {
 #define G2PC_HDR_TOTAL_PIX 2
 #define G2PC_HDR_NEED_DEEPER 3    /* a tile at the deepest tabulated level still has to split: tabulate more levels */
 #define G2PC_HDR_LEAF_OVERFLOW 4  /* more leaves than max_leaves */
-#define G2PC_HDR_CAP_OVERFLOW 5   /* instance / leaf-pixel / multisplit-matrix capacity too small for this frame */
+#define G2PC_HDR_CAP_OVERFLOW 5   /* instance / leaf-pixel / multisplit-matrix / row-list capacity too small for this
+                                     frame */
 #define G2PC_HDR_POISON 6         /* snapshot of the shared failure word at the end of this frame's build_tree: 0 = no
                                      frame has failed, else 1 + the LOWEST frame number that did not fit */
 #define G2PC_HDR_FRAME 7          /* frame number of the header's contents */
 #define G2PC_HDR_TOTAL_INST_HI 8
+#define G2PC_HDR_ROW_INST 9       /* entries of the multisplit's row lists (written by the multisplit; saturates at
+                                     2^31 - 1) */
 #define G2PC_HDR_WORDS 16
 #define G2PC_WORK_COUNTERS 4      /* int32 work-distribution counters cleared by g2pc_build_tree */
 /* device-side statistics (uint64 words, accumulated by g2pc_blend when `stats` is not NULL) */
@@ -522,18 +525,25 @@ int g2pc_build_tree(const int32_t* tables, int32_t num_levels, int32_t max_gauss
                     void* stream);
 
 /* S4c.  Stable multisplit of the depth-ordered stream into the leaves' lists: inst_gid[leaf.inst_begin ..
- * + leaf.inst_count) = Gaussian ids overlapping the leaf, nearest first.  Three kernels (count, scan, scatter); one CTA
- * per chunk of S x C consecutive sorted entries, walked in S sub-steps of C = g2pc_multisplit_chunk(leaf_cap) entries
+ * + leaf.inst_count) = Gaussian ids overlapping the leaf, nearest first.
+ * Base-level leaves (cells of the first leaf-candidate level, 2^base x 2^base): the stream is split by rows into row
+ * lists of 64-bit entries, then each row list by columns into the leaves' lists.  workspace:
+ * g2pc_multisplit_workspace_bytes(n, row_capacity, 2^base, 2^base) bytes, 256-byte aligned, holding row_capacity
+ * row-list entries.  A frame whose row lists need more (at most the base level's instances when that level is clean) sets
+ * HDR_CAP_OVERFLOW and HDR_ROW_INST in `header`, lowers `fail` and is skipped like a frame build_tree refused.
+ * Leaves below the base level (num_levels > base + 1 only): three more kernels (count, scan, scatter); one CTA per
+ * chunk of S x C consecutive sorted entries, walked in S sub-steps of C = g2pc_multisplit_chunk(leaf_cap) entries
  * (S grows with n: a few waves of CTAs on the GPU); matrix: g2pc_multisplit_rows(n, leaf_cap) x leaves uint32 scratch
- * (pass that row count as ms_chunks to g2pc_build_tree, which checks the capacity).
+ * (pass that row count as ms_chunks to g2pc_build_tree, which checks the capacity; NULL and 0 rows without such levels).
  * leaf_cap = max_leaves given to g2pc_build_tree. */
 int32_t g2pc_multisplit_chunk(int32_t leaf_cap);           /* C: entries per sub-step (0: too many leaves) */
 int32_t g2pc_multisplit_rows(int64_t n, int32_t leaf_cap); /* rows of `matrix` needed: one per chunk */
+int64_t g2pc_multisplit_workspace_bytes(int64_t n, int64_t row_capacity, int32_t grid_w, int32_t grid_h);
 int g2pc_multisplit(const uint64_t* val_sorted, int64_t n, const void* proj, int32_t width, int32_t height,
                     const int32_t* tables, int32_t num_levels, uint32_t level_mask, uint32_t clean_mask,
-                    const int32_t* node_leaf, const g2pc_leaf_t* leaves, const int32_t* header, const uint32_t* fail,
-                    int32_t frame,
-                    int32_t leaf_cap, uint32_t* matrix, uint32_t* inst_gid, void* stream);
+                    const int32_t* node_leaf, const g2pc_leaf_t* leaves, int32_t* header, const uint32_t* fail,
+                    int32_t frame, int32_t leaf_cap, uint32_t* matrix, int64_t row_capacity, void* workspace,
+                    int64_t workspace_bytes, uint32_t* inst_gid, void* stream);
 
 /* S5.  Front-to-back blend of every leaf (gauss_render.py:337-369) + per-Gaussian maximum contribution / arg-max pixel
  * (:371-385) published as cam_best[g] = max((bits(contribution) << 32) | ~leaf_pixel_index).
@@ -606,10 +616,13 @@ int g2pc_tiles_build(uint32_t* node_cnt, int32_t width, int32_t height, g2pc_lea
                      int32_t max_leaves, int64_t inst_capacity, int64_t matrix_capacity, int32_t ms_rows, int32_t frame,
                      int32_t* header, uint32_t* fail, int32_t* work_counters, void* stream);
 
-/* g2pc_multisplit over a flat grid (grid_w x grid_h = SW x SH here; the packed range is the rect in grid cells). */
+/* The base-level split of g2pc_multisplit over a flat grid (grid_w x grid_h = SW x SH here, each <= 256; the packed
+ * range is the rect in grid cells, leaf = cell index).  workspace: g2pc_multisplit_workspace_bytes(n, row_capacity,
+ * grid_w, grid_h) bytes; row-list overflow as g2pc_multisplit. */
 int g2pc_multisplit_grid(const uint64_t* val_sorted, int64_t n, int32_t grid_w, int32_t grid_h,
-                         const g2pc_leaf_t* leaves, const int32_t* header, const uint32_t* fail, int32_t frame,
-                         int32_t leaf_cap, uint32_t* matrix, uint32_t* inst_gid, void* stream);
+                         const g2pc_leaf_t* leaves, int32_t* header, const uint32_t* fail, int32_t frame,
+                         int64_t row_capacity, void* workspace, int64_t workspace_bytes, uint32_t* inst_gid,
+                         void* stream);
 
 /* renderCUDA: per pixel front-to-back blend (power > 0 and alpha < 1/255 skipped, the pixel stops before T < 1e-4),
  * out_color (3,H,W) = C + T*bg, out_depth / out_invdepth (H,W) = sum depth*alpha*T / sum alpha*T/depth, written for
