@@ -1,7 +1,7 @@
-// mesh_common.cuh — device code the dense Poisson mesher (s10_mesh.cu), its narrow-band levels (s12_mesh_band.cu) and
-// the decimation (s13_decimate.cu) share: the frame words, a point's dual cell and trilinear weights, the fixed-order
-// float64 finish step, the marching-tetrahedra tables and the one-ring / incidence list builders.  Every kernel stays
-// in an anonymous namespace.
+// mesh_common.cuh — device code the dense Poisson mesher (s10_mesh.cu), its narrow-band levels (s12_mesh_band.cu),
+// the decimation (s13_decimate.cu) and the component filter (s15_components.cu) share: the frame words, a point's dual
+// cell and trilinear weights, the fixed-order float64 finish step, the marching-tetrahedra tables, the stable mesh
+// compaction and the one-ring / incidence list builders.  Every kernel stays in an anonymous namespace.
 #pragma once
 #include "cloud_common.cuh"
 
@@ -162,6 +162,46 @@ __device__ __forceinline__ int tet_triangles(int p, uint32_t inside, int (&tri)[
         }
     }
     return nt;
+}
+
+// ---- stable compaction of a mesh by vertex keep flags (density trim in s10_mesh.cu, s15_components.cu) ---------------
+// a triangle is kept iff its three vertices are; vmap / fmap are the exclusive scans of the vertex / triangle flags
+__global__ void __launch_bounds__(MB) tri_flag_kernel(const int32_t* __restrict__ faces, int64_t t,
+                                                      const uint8_t* __restrict__ keep, int32_t* __restrict__ flag) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t) return;
+    flag[f] = keep[faces[3 * f]] & keep[faces[3 * f + 1]] & keep[faces[3 * f + 2]];
+}
+
+__global__ void __launch_bounds__(MB) compact_vertices_kernel(const uint8_t* __restrict__ keep,
+                                                              const int32_t* __restrict__ vmap, int64_t m,
+                                                              const double* __restrict__ dens,
+                                                              const double* __restrict__ vpos,
+                                                              const uint8_t* __restrict__ vcol, double* __restrict__ dens_o,
+                                                              double* __restrict__ vpos_o, uint8_t* __restrict__ vcol_o) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m || !keep[v]) return;
+    const int64_t o = vmap[v];
+    dens_o[o] = dens[v];
+    for (int a = 0; a < 3; ++a) vpos_o[3 * o + a] = vpos[3 * v + a];
+    if (vcol)
+        for (int a = 0; a < 3; ++a) vcol_o[3 * o + a] = vcol[3 * v + a];
+}
+
+__global__ void __launch_bounds__(MB) compact_faces_kernel(const int32_t* __restrict__ faces, const int32_t* __restrict__ flag,
+                                                           const int32_t* __restrict__ fmap, int64_t t,
+                                                           const int32_t* __restrict__ vmap, int32_t* __restrict__ faces_o) {
+    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (f >= t || !flag[f]) return;
+    const int64_t o = fmap[f];
+    for (int s = 0; s < 3; ++s) faces_o[3 * o + s] = vmap[faces[3 * f + s]];
+}
+
+__global__ void trim_counts_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ map, int64_t m,
+                                   const int32_t* __restrict__ tflag, const int32_t* __restrict__ tmap, int64_t t,
+                                   long long* __restrict__ counts) {
+    counts[0] = m ? (long long)map[m - 1] + flag[m - 1] : 0;
+    counts[1] = t ? (long long)tmap[t - 1] + tflag[t - 1] : 0;
 }
 
 // ---- one-ring / incidence lists of a triangle mesh (smoothing and normals in s10_mesh.cu, s13_decimate.cu) --------

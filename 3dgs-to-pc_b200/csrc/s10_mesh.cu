@@ -492,44 +492,6 @@ __global__ void __launch_bounds__(MB) keep_kernel(const double* __restrict__ den
     flag[v] = k;
 }
 
-__global__ void __launch_bounds__(MB) tri_flag_kernel(const int32_t* __restrict__ faces, int64_t t,
-                                                      const uint8_t* __restrict__ keep, int32_t* __restrict__ flag) {
-    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (f >= t) return;
-    flag[f] = keep[faces[3 * f]] & keep[faces[3 * f + 1]] & keep[faces[3 * f + 2]];
-}
-
-__global__ void __launch_bounds__(MB) compact_vertices_kernel(const uint8_t* __restrict__ keep,
-                                                              const int32_t* __restrict__ vmap, int64_t m,
-                                                              const double* __restrict__ dens,
-                                                              const double* __restrict__ vpos,
-                                                              const uint8_t* __restrict__ vcol, double* __restrict__ dens_o,
-                                                              double* __restrict__ vpos_o, uint8_t* __restrict__ vcol_o) {
-    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (v >= m || !keep[v]) return;
-    const int64_t o = vmap[v];
-    dens_o[o] = dens[v];
-    for (int a = 0; a < 3; ++a) vpos_o[3 * o + a] = vpos[3 * v + a];
-    if (vcol)
-        for (int a = 0; a < 3; ++a) vcol_o[3 * o + a] = vcol[3 * v + a];
-}
-
-__global__ void __launch_bounds__(MB) compact_faces_kernel(const int32_t* __restrict__ faces, const int32_t* __restrict__ flag,
-                                                           const int32_t* __restrict__ fmap, int64_t t,
-                                                           const int32_t* __restrict__ vmap, int32_t* __restrict__ faces_o) {
-    const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (f >= t || !flag[f]) return;
-    const int64_t o = fmap[f];
-    for (int s = 0; s < 3; ++s) faces_o[3 * o + s] = vmap[faces[3 * f + s]];
-}
-
-__global__ void trim_counts_kernel(const int32_t* __restrict__ flag, const int32_t* __restrict__ map, int64_t m,
-                                   const int32_t* __restrict__ tflag, const int32_t* __restrict__ tmap, int64_t t,
-                                   long long* __restrict__ counts) {
-    counts[0] = m ? (long long)map[m - 1] + flag[m - 1] : 0;
-    counts[1] = t ? (long long)tmap[t - 1] + tflag[t - 1] : 0;
-}
-
 // ---- smoothing, normals (their one-ring / incidence lists: mesh_common.cuh) ----------------------------------------
 // one Jacobi step, lambda = 1/2: v + (sum w_j v_j / sum w_j - v) / 2, w_j = 1 / (|v - v_j| + 1e-12), distinct
 // neighbours in ascending index

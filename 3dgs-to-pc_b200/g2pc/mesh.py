@@ -14,6 +14,10 @@ band_depth and the same trim, smoothing and normals.
 
 With target_triangles (N9, s13_decimate.cu): between the smoothing and the normals, decimate(): g2pc_mesh_decimate_prepare,
 then per round _select (host reads the counts) -> _apply until the target is met or nothing is selected, then _finish.
+
+With min_component_triangles / keep_largest_components (N11, s15_components.cu): between the trim and the smoothing,
+remove_components(): g2pc_mesh_components_label (host reads the component count) -> _select (host reads the kept counts)
+-> _compact.
 """
 import collections
 import math
@@ -435,8 +439,120 @@ def decimate_mesh(mesh, target_triangles, stats=None):
     return Mesh(v, faces, vcol, vn, dens)
 
 
+def check_component_params(min_triangles, keep_largest, need_one=True):
+    """Refuses a component-filter parameter that is neither None nor an integer >= 1 (bool included), and, with need_one,
+    two Nones."""
+    for name, x in (("min_triangles", min_triangles), ("keep_largest", keep_largest)):
+        if x is not None and (isinstance(x, bool) or not isinstance(x, (int, np.integer)) or x < 1):
+            raise capi.G2pcError(f"{name} must be None or an integer >= 1, got {x!r}")
+    if need_one and min_triangles is None and keep_largest is None:
+        raise capi.G2pcError("give min_triangles, keep_largest or both")
+
+
+def remove_components(vpos, faces, colours=None, densities=None, min_triangles=None, keep_largest=None, stats=None,
+                      return_debug=False):
+    """Removes the small connected components of a triangle mesh (DESIGN.md §2, N11).  Two vertices are connected when a
+    face uses both; a component's size is its number of triangles.  A component is kept iff its size is >= 1, >=
+    min_triangles (when given) and its rank is < keep_largest (when given; ranked by size descending, ties to the smaller
+    label, a component's smallest vertex index).  vpos (m,3) float64, faces (t,3) int32, colours (m,3) uint8 or None,
+    densities (m,) float64 or None, all CUDA.  Returns (vpos, faces, colours, densities) of the kept vertices and faces,
+    in their order, with the faces renumbered; the values are copied unchanged.  Raises G2pcError when nothing is kept.
+
+    stats: a dict that receives components (with at least one triangle), kept, largest (size), removed_triangles and
+    removed_vertices.  return_debug: also a dict with labels (m,) int32, keep (m,) uint8 and sizes (m,) int32 (triangles
+    per label, 0 at an index that is no label)."""
+    check_component_params(min_triangles, keep_largest)
+    for name, x in (("vpos", vpos), ("faces", faces), ("colours", colours), ("densities", densities)):
+        if x is not None and not (torch.is_tensor(x) and x.is_cuda):
+            raise capi.G2pcError(f"{name} must be a CUDA tensor (the component filter has no CPU path)")
+    if vpos.dim() != 2 or vpos.shape[1] != 3 or vpos.dtype != torch.float64:
+        raise capi.G2pcError(f"vpos must be (m, 3) float64, got {tuple(vpos.shape)} {vpos.dtype}")
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype != torch.int32:
+        raise capi.G2pcError(f"faces must be (t, 3) int32, got {tuple(faces.shape)} {faces.dtype}")
+    m, t, dev = vpos.shape[0], faces.shape[0], vpos.device
+    if colours is not None and (colours.shape != (m, 3) or colours.dtype != torch.uint8):
+        raise capi.G2pcError(f"colours must be (m, 3) uint8, got {tuple(colours.shape)} {colours.dtype}")
+    if densities is not None and (densities.shape != (m,) or densities.dtype != torch.float64):
+        raise capi.G2pcError(f"densities must be (m,) float64, got {tuple(densities.shape)} {densities.dtype}")
+    if any(x is not None and x.device != dev for x in (faces, colours, densities)):
+        raise capi.G2pcError("vpos, faces, colours and densities must be on one device")
+    if m >= 2 ** 31 - 1 or 3 * t >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the mesh has {m} vertices and {t} triangles: more than the component filter's int32 "
+                             f"indices can address")
+    if t:
+        lo, hi = torch.stack([faces.min(), faces.max()]).tolist()
+        if lo < 0 or hi >= m:
+            raise capi.G2pcError(f"face indices must be in 0..{m - 1}, got {lo}..{hi}")
+    if t == 0:
+        raise capi.G2pcError("no component is kept: the mesh has no triangle (the largest component has 0)")
+    vpos, faces = vpos.contiguous(), faces.contiguous()
+    colours = colours.contiguous() if colours is not None else None
+    lib = capi.load()
+    ws_bytes = lib.g2pc_mesh_components_select_workspace_bytes(m, t)
+    # labels, sizes, keep, a density scratch when there are no densities, the select workspace, and outputs as large
+    # as the input mesh
+    check_memory(m * (4 + 4 + 1) + (8 * m if densities is None else 0) + ws_bytes + m * (24 + 8 + 3) + 12 * t, dev,
+                 f"the component filter of {m} vertices and {t} triangles", remedy="filter a smaller mesh")
+    st = capi.stream_ptr(dev)
+    labels = torch.empty((m,), dtype=torch.int32, device=dev)
+    sizes = torch.empty((m,), dtype=torch.int32, device=dev)
+    counts = torch.empty((3,), dtype=torch.int64, device=dev)
+    capi.call("g2pc_mesh_components_label", capi.ptr(faces), m, t, capi.ptr(labels), capi.ptr(sizes),
+              capi.ptr(counts), st)
+    components, largest = counts[:2].tolist()
+    keep = torch.empty((m,), dtype=torch.uint8, device=dev)
+    ws = capi.workspace(ws_bytes, dev)
+    capi.call("g2pc_mesh_components_select", capi.ptr(faces), m, t, capi.ptr(labels), capi.ptr(sizes), components,
+              int(min_triangles or 0), int(keep_largest or 0), capi.ptr(keep), capi.ptr(counts), capi.ptr(ws),
+              ws.numel(), st)
+    mk, tk, kept = counts.tolist()
+    if stats is not None:
+        stats.update(components=components, kept=kept, largest=largest, removed_triangles=t - tk,
+                     removed_vertices=m - mk)
+    if tk == 0:
+        raise capi.G2pcError(f"no component is kept: the largest of the {components} component(s) has {largest} "
+                             f"triangle(s) (min_triangles {min_triangles}, keep_largest {keep_largest})")
+    dens = densities.contiguous() if densities is not None else torch.empty((m,), dtype=torch.float64, device=dev)
+    vout = torch.empty((mk, 3), dtype=torch.float64, device=dev)
+    cout = torch.empty((mk, 3), dtype=torch.uint8, device=dev) if colours is not None else None
+    dout = torch.empty((mk,), dtype=torch.float64, device=dev)
+    fout = torch.empty((tk, 3), dtype=torch.int32, device=dev)
+    capi.call("g2pc_mesh_components_compact", capi.ptr(vpos), capi.ptr(colours), capi.ptr(dens), m, capi.ptr(faces), t,
+              capi.ptr(keep), capi.ptr(vout), capi.ptr(cout), capi.ptr(dout), capi.ptr(fout), capi.ptr(ws), ws.numel(),
+              st)
+    out = (vout, fout, cout, dout if densities is not None else None)
+    return (out, {"labels": labels, "keep": keep, "sizes": sizes}) if return_debug else out
+
+
+def remove_components_mesh(mesh, min_triangles=None, keep_largest=None, stats=None):
+    """remove_components() of a Mesh.  Its float32 vertices and normals are carried over unchanged: the kept vertices'
+    normals need no recomputation, because a vertex normal reads only the vertex's own faces, and they all stay."""
+    check_component_params(min_triangles, keep_largest)
+    # The compaction copies float64 words bit for bit, so each vertex's float32 position and normal (24 bytes) travel
+    # together as one float64 triple.
+    packed = torch.cat([mesh.vertices.to(torch.float32), mesh.normals.to(torch.float32)], 1).contiguous()
+    vn, faces, vcol, dens = remove_components(packed.view(torch.float64), mesh.faces.contiguous(), mesh.colours,
+                                              mesh.densities, min_triangles, keep_largest, stats=stats)
+    vn = vn.view(torch.float32)
+    return Mesh(vn[:, :3].contiguous(), faces, vcol, vn[:, 3:].contiguous(), dens)
+
+
+def filter_components(vpos, faces, vcol, dens, min_triangles, keep_largest, stats, timings, debug):
+    """The component filter of a mesher's trimmed mesh when min_triangles or keep_largest is given, else the mesh as it
+    is.  debug (a dict or None) receives component_labels."""
+    if min_triangles is None and keep_largest is None:
+        return vpos, faces, vcol, dens
+    with capi.phase(timings, "components"):
+        out, cdbg = remove_components(vpos, faces, vcol, dens, min_triangles, keep_largest, stats=stats,
+                                      return_debug=True)
+    if debug is not None:
+        debug["component_labels"] = cdbg["labels"]
+    return out
+
+
 def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, std_ratio=3.0, return_debug=False,
-                 timings=None, band_depth=None, band_stats=None, target_triangles=None):
+                 timings=None, band_depth=None, band_stats=None, target_triangles=None, min_component_triangles=None,
+                 keep_largest_components=None, component_stats=None):
     """Mesh of an oriented point cloud.  points (n,3) float32 CUDA; normals (n,3) float32 / float64 (outward for an
     outward-facing mesh); colours (n,3) in 0..255 or None.  Returns Mesh(vertices (m,3) float32, faces (t,3) int32,
     colours (m,3) uint8 or None, normals (m,3) float32, densities (m,) float64).  With return_debug also a dict: chi
@@ -454,10 +570,15 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
 
     target_triangles: None keeps every triangle.  An integer >= 1 decimates the smoothed mesh to target_triangles or
     target_triangles - 1 triangles (decimate(), DESIGN.md §2, N9) before the normals are computed; timings add
-    "decimate"."""
+    "decimate".
+
+    min_component_triangles, keep_largest_components: None and None keep every component.  Otherwise the trimmed mesh
+    goes through remove_components() (DESIGN.md §2, N11) before the smoothing; timings add "components", the debug dict
+    component_labels (per vertex of the trimmed mesh) and component_stats (a dict) receives remove_components' stats."""
     capi.check_cloud(points, normals, colours, what="Poisson meshing")
     if target_triangles is not None:
         check_target(target_triangles)
+    check_component_params(min_component_triangles, keep_largest_components, need_one=False)
     if int(depth) != depth or not DEPTH_MIN <= depth <= DEPTH_MAX:
         raise capi.G2pcError(f"depth must be an integer in {DEPTH_MIN}..{DEPTH_MAX} (the dense int64 right-hand side "
                              f"alone is 69 GB at depth 11), got {depth}")
@@ -499,7 +620,8 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
         dense = {"chi": chi}  # handed over, so that the band levels can free it
         del chi
         return _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, int(band_depth), laplacian_iters, debug,
-                          return_debug, timings, band_stats, target_triangles)
+                          return_debug, timings, band_stats, target_triangles,
+                          (min_component_triangles, keep_largest_components, component_stats))
     with capi.phase(timings, "extract"):
         # B is dead after the solve: its memory holds the node lists of the extraction and the cell lists of the gather
         vkey, vt, vpos, faces = extract(chi, depth, frame, iso, B)
@@ -508,6 +630,9 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     with capi.phase(timings, "gather_trim"):
         dens, vcol = gather(pts, cols.to(torch.int32) if cols is not None else None, cell, frame, depth, vkey, vt, B)
         dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
+    vpos, faces, vcol, dens = filter_components(vpos, faces, vcol, dens, min_component_triangles,
+                                                 keep_largest_components, component_stats, timings,
+                                                 debug if return_debug else None)
     with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
     smoothed = vpos
@@ -524,9 +649,10 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
 
 
 def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, laplacian_iters, debug, return_debug,
-               timings, band_stats, target_triangles):
+               timings, band_stats, target_triangles, components):
     """The band levels depth + 1 .. band_depth after the dense solve, then the mesh at band_depth.  dense: {"chi": the
-    dense level's chi}, emptied here."""
+    dense level's chi}, emptied here.  components: poisson_mesh's (min_component_triangles, keep_largest_components,
+    component_stats)."""
     dev = pts.device
     parent_chi, parent_map = dense.pop("chi"), None
     if return_debug:
@@ -578,6 +704,8 @@ def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, lapla
         dens, vcol = band_gather(pts, cols.to(torch.int32) if cols is not None else None, cell, bframe, band_depth,
                                  vkey, vt)
         dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
+    vpos, faces, vcol, dens = filter_components(vpos, faces, vcol, dens, *components, timings,
+                                                 debug if return_debug else None)
     with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
     smoothed = vpos

@@ -5,7 +5,8 @@ Steps: statistical outlier removal of the Gaussian means (k = 20, std_ratio 3; o
 -> memory check -> per camera, in order, on the CUDA back-end's frame queue: g2pc_tiles_blend_fusion (colour, final
 transmittance T, median depth z_med) then g2pc_tsdf_integrate into the 2^depth grid -> g2pc_mesh_extract_count / _emit
 (the Poisson mesher's marching tetrahedra, unchanged, iso 0) -> g2pc_tsdf_gather_compact (keep the surface of the
-observed voxels, vertex colours and weights) -> g2pc_mesh_smooth -> decimate (with target_triangles) ->
+observed voxels, vertex colours and weights) -> remove_components (with min_component_triangles or
+keep_largest_components) -> g2pc_mesh_smooth -> decimate (with target_triangles) ->
 g2pc_mesh_normals.  Host reads: the frame after the outlier removal, the extraction counts, the kept counts.
 """
 import collections
@@ -115,7 +116,8 @@ def gather_compact(weight, colour, depth, vkey, vt, vpos, faces):
 
 
 def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, depth=DEFAULT_DEPTH, trunc=DEFAULT_TRUNC,
-              laplacian_iters=10, target_triangles=None, timings=None, return_debug=False, async_mode=True):
+              laplacian_iters=10, target_triangles=None, timings=None, return_debug=False, async_mode=True,
+              min_component_triangles=None, keep_largest_components=None, component_stats=None):
     """Mesh of the Gaussians (xyz (n,3), opacities (n,) or (n,1), covariances (n,3,3) or (n,6), and exactly one of
     colours (n,3) in 0..1 or shs (n,3,K) channel-major, all CUDA) seen by `cameras` (the CUDA back-end's raster settings,
     camera_handler.get_camera("cuda", ...)), in order.  Returns mesh.Mesh(vertices (m,3) float32, faces (t,3) int32,
@@ -131,13 +133,17 @@ def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, dept
     mesh.poisson_mesh.  timings: a dict that receives CUDA event pairs per phase (frame, fusion, extract, gather,
     smooth, decimate, normals).  return_debug: also a dict with frame, tsdf, weight, colour (the grid), vkey, vt, vpos,
     faces (the extraction), keep (the vertex mask of the gather), images ({camera index: (colour, T, z_med)}) and
-    replays."""
+    replays.
+
+    min_component_triangles, keep_largest_components, component_stats: as mesh.poisson_mesh; the component filter runs
+    on the gathered mesh before the smoothing, timings add "components" and the debug dict component_labels."""
     check_depth(depth)
     check_trunc(trunc)
     if int(laplacian_iters) != laplacian_iters or laplacian_iters < 0:
         raise capi.G2pcError(f"laplacian_iters must be an integer >= 0, got {laplacian_iters}")
     if target_triangles is not None:
         mesh.check_target(target_triangles)
+    mesh.check_component_params(min_component_triangles, keep_largest_components, need_one=False)
     if (colours is None) == (shs is None):
         raise capi.G2pcError("give exactly one of colours and shs")
     capi.check_cloud(xyz.to(torch.float32).contiguous() if torch.is_tensor(xyz) else xyz)
@@ -199,6 +205,8 @@ def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, dept
     del grid, tsdf, weight, colour
     if fkept.shape[0] == 0:
         raise capi.G2pcError("no surface between observed voxels")
+    vkept, fkept, vcol, dens = mesh.filter_components(vkept, fkept, vcol, dens, min_component_triangles,
+                                                       keep_largest_components, component_stats, timings, debug)
     if laplacian_iters and 6 * fkept.shape[0] >= 2 ** 31 - 1:
         raise capi.G2pcError(f"the surface has {fkept.shape[0]} triangles: the Laplacian smoothing's one-ring lists "
                              f"(6 per triangle) exceed int32; use a smaller tsdf depth or laplacian_iters=0")

@@ -455,8 +455,9 @@ def config_parser(argv=None, mesh=False):
     mesh=True parses for gauss_to_mesh.py: --generate_mesh is implied and meshes with this project's GPU mesher
     (g2pc/mesh.py) instead of Open3D, which needs renderer_type cuda, a depth in mesh.DEPTH_MIN..DEPTH_MAX and
     laplacian_iterations >= 0.  It also adds --band_depth (narrow-band levels above --poisson_depth, up to
-    mesh.BAND_DEPTH_MAX; --poisson_depth 10 --band_depth 12 is the reference's depth 12) and --target_triangles (>= 1:
-    decimate the mesh to that many triangles)."""
+    mesh.BAND_DEPTH_MAX; --poisson_depth 10 --band_depth 12 is the reference's depth 12), --target_triangles (>= 1:
+    decimate the mesh to that many triangles), and --min_component_triangles / --keep_largest_components (>= 1: remove
+    the mesh's connected pieces with fewer triangles / all but the largest ones)."""
     try:
         import configargparse as ap
     except ImportError:
@@ -506,6 +507,12 @@ def config_parser(argv=None, mesh=False):
                             help="With --mesh_method tsdf: 2^depth voxels per axis (2..10)")
         parser.add_argument("--tsdf_trunc", default=4.0, type=float,
                             help="With --mesh_method tsdf: truncation distance in voxels (> 0)")
+        parser.add_argument("--min_component_triangles", default=None, type=int,
+                            help="Remove the connected pieces of the mesh with fewer triangles than this, before "
+                                 "smoothing; default: keep them all")
+        parser.add_argument("--keep_largest_components", default=None, type=int,
+                            help="Keep only this many of the largest connected pieces of the mesh; default: keep them "
+                                 "all")
 
     args = parser.parse_args(argv)
     if mesh:
@@ -522,6 +529,10 @@ def config_parser(argv=None, mesh=False):
             raise AttributeError(f"Band depth must be between {args.poisson_depth + 1} and {gmesh.BAND_DEPTH_MAX}")
         if args.target_triangles is not None and args.target_triangles < 1:
             raise AttributeError("Target triangles must be 1 or more")
+        if args.min_component_triangles is not None and args.min_component_triangles < 1:
+            raise AttributeError("Minimum component triangles must be 1 or more")
+        if args.keep_largest_components is not None and args.keep_largest_components < 1:
+            raise AttributeError("Largest components to keep must be 1 or more")
         if args.mesh_method == "tsdf":
             from g2pc import tsdf
             if args.band_depth is not None:
@@ -635,6 +646,9 @@ def main(argv=None, mesh=False):
     save_xyz_to_ply(total_point_cloud.points, args.output_path, rgb_colors=total_point_cloud.colours,
                     normals_points=total_point_cloud.normals, chunk_size=10**6, quiet=args.quiet)
 
+    if mesh:
+        from mesh_pc import component_line
+        cstats = {}
     if mesh and args.mesh_method == "tsdf":
         from g2pc import mesh as gmesh, tsdf
         scene = surface_point_cloud
@@ -642,9 +656,13 @@ def main(argv=None, mesh=False):
             print(f"Fusing the median depth of {len(scene.cameras)} cameras into a 2^{args.tsdf_depth} voxel grid")
         m = tsdf.fuse_mesh(scene.xyz, scene.opacities, scene.covariances, scene.cameras, colours=scene.colours,
                            shs=scene.shs, depth=args.tsdf_depth, trunc=args.tsdf_trunc,
-                           laplacian_iters=args.laplacian_iterations, target_triangles=args.target_triangles)
+                           laplacian_iters=args.laplacian_iterations, target_triangles=args.target_triangles,
+                           min_component_triangles=args.min_component_triangles,
+                           keep_largest_components=args.keep_largest_components, component_stats=cstats)
         gmesh.write_mesh_ply(args.mesh_output_path, m)
         if not args.quiet:
+            if cstats:
+                print(component_line(cstats))
             print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")
         return None, m
     if mesh:
@@ -657,9 +675,13 @@ def main(argv=None, mesh=False):
             print(f"Meshing {surface_point_cloud.points.shape[0]} surface points at depth {args.poisson_depth}{band}")
         m = gmesh.poisson_mesh(surface_point_cloud.points, surface_point_cloud.normals, surface_point_cloud.colours,
                                depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations, std_ratio=3.0,
-                               band_depth=args.band_depth, target_triangles=args.target_triangles)
+                               band_depth=args.band_depth, target_triangles=args.target_triangles,
+                               min_component_triangles=args.min_component_triangles,
+                               keep_largest_components=args.keep_largest_components, component_stats=cstats)
         gmesh.write_mesh_ply(args.mesh_output_path, m)
         if not args.quiet:
+            if cstats:
+                print(component_line(cstats))
             print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")
         return surface_point_cloud, m
     elif pointcloud_settings.generate_mesh:

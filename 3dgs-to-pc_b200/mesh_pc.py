@@ -2,14 +2,17 @@
 trim and Laplacian smoothing (g2pc/mesh.py).
 
     python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10] [--band_depth 12]
-                      [--laplacian_iterations 10] [--orient_normals] [--target_triangles N] [--quiet]
+                      [--laplacian_iterations 10] [--orient_normals] [--target_triangles N]
+                      [--min_component_triangles N] [--keep_largest_components K] [--quiet]
 
 The cloud must carry normals (nx ny nz), as gauss_to_pc.py writes them by default; its colours (red green blue) are
 carried over to the mesh's vertices.  A mesh faces the way its normals point.  By default the normals are used as they
 are; --orient_normals first gives them a consistent sign (g2pc/orient.py, k = 10), which the normals of a cloud sampled
 from Gaussians lack: each takes its sign from its Gaussian's rotation.  --band_depth adds finer levels stored only in a narrow band around the points:
 --poisson_depth 10 --band_depth 12 is the reference's Poisson depth 12.  --target_triangles decimates the smoothed mesh
-to N or N - 1 triangles on the GPU (quadric edge collapse, g2pc.mesh.decimate) before its normals are computed."""
+to N or N - 1 triangles on the GPU (quadric edge collapse, g2pc.mesh.decimate) before its normals are computed.
+--min_component_triangles and --keep_largest_components remove the small disconnected pieces of the trimmed mesh before
+it is smoothed (g2pc.mesh.remove_components): those with fewer than N triangles, and all but the K largest."""
 import argparse
 import time
 
@@ -41,6 +44,19 @@ def target(s):
     return n
 
 
+def add_component_flags(p):
+    p.add_argument("--min_component_triangles", type=target, default=None,
+                   help="remove the connected pieces of the mesh with fewer triangles than this; default: keep them all")
+    p.add_argument("--keep_largest_components", type=target, default=None,
+                   help="keep only this many of the largest connected pieces; default: keep them all")
+
+
+def component_line(stats):
+    """The one line the commands print about the component filter."""
+    return (f"Removed small pieces: {stats['components']} component(s) found, {stats['kept']} kept, "
+            f"{stats['removed_triangles']} triangle(s) removed")
+
+
 def config_parser(argv=None):
     p = argparse.ArgumentParser(description="Mesh a point cloud with oriented normals (Poisson reconstruction)")
     p.add_argument("--input_path", required=True, help="point-cloud PLY with x y z and nx ny nz (red green blue optional)")
@@ -56,6 +72,7 @@ def config_parser(argv=None):
                    help=f"orient the normals consistently (k = {orient.K_DEFAULT} nearest neighbours) before meshing")
     p.add_argument("--target_triangles", type=target, default=None,
                    help="decimate the mesh to this many triangles (or one fewer); default: keep every triangle")
+    add_component_flags(p)
     p.add_argument("--quiet", action="store_true", help="print nothing")
     args = p.parse_args(argv)
     if args.band_depth is not None and not args.poisson_depth < args.band_depth <= mesh.BAND_DEPTH_MAX:
@@ -86,10 +103,15 @@ def main(argv=None):
         normals, st = orient.orient_normals(points, normals, k=orient.K_DEFAULT)
         if not args.quiet:
             print(f"Oriented the normals: {st.flipped} flipped, {st.components} component(s), {st.skipped} skipped")
+    cstats = {}
     m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations,
-                          band_depth=args.band_depth, target_triangles=args.target_triangles)
+                          band_depth=args.band_depth, target_triangles=args.target_triangles,
+                          min_component_triangles=args.min_component_triangles,
+                          keep_largest_components=args.keep_largest_components, component_stats=cstats)
     mesh.write_mesh_ply(args.mesh_output_path, m)
     if not args.quiet:
+        if cstats:
+            print(component_line(cstats))
         print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path} "
               f"in {time.perf_counter() - t0:.2f} s")
     return m

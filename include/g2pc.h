@@ -367,6 +367,30 @@ int g2pc_mesh_decimate_finish(const double* vpos, int64_t m, const int32_t* face
                               double* vpos_out, uint8_t* colours_out, double* densities_out, int32_t* faces_out,
                               int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- N11: connected-component filter of a triangle mesh (s15_components.cu, g2pc/mesh.py remove_components) ------ */
+/* Rules in DESIGN.md §2, N11.  m vertices (1..2^31-2), faces (t,3 int32, 3 t < 2^31 - 1, indices in 0..m-1; a face may
+ * use a vertex twice).  Order of calls: label (host reads counts[0]) -> select (host reads counts) -> compact into
+ * buffers of the kept sizes. */
+/* Two vertices are connected when a face uses both.  labels (m int32) = the smallest vertex of each vertex's component;
+ * sizes (m int32, indexed by label) = triangles per component (0 for an unused vertex); counts (2 int64): components
+ * with at least one triangle, the largest size. */
+int g2pc_mesh_components_label(const int32_t* faces, int64_t m, int64_t t, int32_t* labels, int32_t* sizes,
+                               int64_t* counts, void* stream);
+/* keep (m uint8) = 1 iff the vertex's component has size >= max(1, min_triangles) and, when 0 < keep_largest <
+ * components (counts[0] of the label call), rank < keep_largest in (size descending, label ascending).  0 turns a
+ * parameter off.  counts (3 int64): kept vertices, kept triangles, kept components.  The workspace
+ * (g2pc_mesh_components_select_workspace_bytes(m, t)) carries the selection to the compact call with the same m, t. */
+int64_t g2pc_mesh_components_select_workspace_bytes(int64_t m, int64_t t);
+int g2pc_mesh_components_select(const int32_t* faces, int64_t m, int64_t t, const int32_t* labels, const int32_t* sizes,
+                                int64_t components, int64_t min_triangles, int64_t keep_largest, uint8_t* keep,
+                                int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream);
+/* The kept vertices (vpos (m,3 float64), vcolours (m,3 uint8, may be NULL), density (m float64)) and faces (renumbered)
+ * in their order into the *_out buffers, which hold the kept counts of the select call. */
+int g2pc_mesh_components_compact(const double* vpos, const uint8_t* vcolours, const double* density, int64_t m,
+                                 const int32_t* faces, int64_t t, const uint8_t* keep, double* vpos_out,
+                                 uint8_t* vcolours_out, double* density_out, int32_t* faces_out, const void* workspace,
+                                 int64_t workspace_bytes, void* stream);
+
 /* ---- N7: consistent orientation of point-cloud normals (s11_orient.cu, g2pc/orient.py) -------------------------- */
 /* Hoppe et al. 1992 (the rule behind Open3D's orient_normals_consistent_tangent_plane) with this project's own rules
  * (DESIGN.md §2): k-NN graph, edge weight 1 - |n_i . n_j|, minimum spanning forest, sign propagated from one seed per
