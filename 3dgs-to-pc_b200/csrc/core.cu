@@ -11,5 +11,5 @@ void g2pc_set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-extern "C" int g2pc_version(void) { return 112; }
+extern "C" int g2pc_version(void) { return 113; }
 extern "C" const char* g2pc_last_error(void) { return g_err; }

@@ -1,7 +1,8 @@
 // mesh_common.cuh — device code the dense Poisson mesher (s10_mesh.cu), its narrow-band levels (s12_mesh_band.cu),
-// the decimation (s13_decimate.cu) and the component filter (s15_components.cu) share: the frame words, a point's dual
-// cell and trilinear weights, the fixed-order float64 finish step, the marching-tetrahedra tables, the stable mesh
-// compaction and the one-ring / incidence list builders.  Every kernel stays in an anonymous namespace.
+// the decimation (s13_decimate.cu), the component filter (s15_components.cu) and the hole filling (s16_holes.cu) share:
+// the frame words, a point's dual cell and trilinear weights, the fixed-order float64 finish step, the
+// marching-tetrahedra tables, the stable mesh compaction, the union-find and the one-ring / incidence list builders.
+// Every kernel stays in an anonymous namespace.
 #pragma once
 #include "cloud_common.cuh"
 
@@ -202,6 +203,51 @@ __global__ void trim_counts_kernel(const int32_t* __restrict__ flag, const int32
                                    long long* __restrict__ counts) {
     counts[0] = m ? (long long)map[m - 1] + flag[m - 1] : 0;
     counts[1] = t ? (long long)tmap[t - 1] + tflag[t - 1] : 0;
+}
+
+// ---- concurrent union-find whose roots are their sets' smallest vertices (s15_components.cu, s16_holes.cu) ----------
+// Every read of a parent pointer goes to memory (volatile): a value cached in a register across iterations could be
+// stale.  Writes are atomics.
+__device__ __forceinline__ int parent_of(const int32_t* parent, int x) { return ((const volatile int32_t*)parent)[x]; }
+
+// The root of x's set as seen now.  Path halving: x's pointer moves to its grandparent, an ancestor below its parent.
+__device__ int find_root(int32_t* parent, int x) {
+    while (true) {
+        const int p = parent_of(parent, x);
+        if (p == x) return x;
+        const int g = parent_of(parent, p);
+        if (g == p) return p;
+        atomicMin(&parent[x], g);
+        x = g;
+    }
+}
+
+// Joins the sets of a and b: the larger root is hooked under the smaller one when it is still a root, else the union
+// retries from the root it was hooked under meanwhile.
+__device__ void unite(int32_t* parent, int a, int b) {
+    while (true) {
+        a = find_root(parent, a);
+        b = find_root(parent, b);
+        if (a == b) return;
+        const int hi = a > b ? a : b, lo = a > b ? b : a;
+        const int old = atomicCAS(&parent[hi], hi, lo);
+        if (old == hi) return;
+        a = old;
+        b = lo;
+    }
+}
+
+__global__ void __launch_bounds__(MB) parent_init_kernel(int32_t* __restrict__ parent, int64_t m) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v < m) parent[v] = (int32_t)v;
+}
+
+// after every union: parent[v] = the root of v (its label)
+__global__ void __launch_bounds__(MB) compress_kernel(int32_t* parent, int64_t m) {
+    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
+    if (v >= m) return;
+    const int r = find_root(parent, (int)v);
+    atomicMin(&parent[v], r);
 }
 
 // ---- one-ring / incidence lists of a triangle mesh (smoothing and normals in s10_mesh.cu, s13_decimate.cu) --------

@@ -15,56 +15,12 @@ namespace {
 
 unsigned grid_of(int64_t n) { return (unsigned)((n + MB - 1) / MB); }
 
-// Every read of a parent pointer goes to memory (volatile): a value cached in a register across iterations could be
-// stale.  Writes are atomics.
-__device__ __forceinline__ int parent_of(const int32_t* parent, int x) { return ((const volatile int32_t*)parent)[x]; }
-
-// The root of x's set as seen now.  Path halving: x's pointer moves to its grandparent, an ancestor below its parent.
-__device__ int find_root(int32_t* parent, int x) {
-    while (true) {
-        const int p = parent_of(parent, x);
-        if (p == x) return x;
-        const int g = parent_of(parent, p);
-        if (g == p) return p;
-        atomicMin(&parent[x], g);
-        x = g;
-    }
-}
-
-// Joins the sets of a and b: the larger root is hooked under the smaller one when it is still a root, else the union
-// retries from the root it was hooked under meanwhile.
-__device__ void unite(int32_t* parent, int a, int b) {
-    while (true) {
-        a = find_root(parent, a);
-        b = find_root(parent, b);
-        if (a == b) return;
-        const int hi = a > b ? a : b, lo = a > b ? b : a;
-        const int old = atomicCAS(&parent[hi], hi, lo);
-        if (old == hi) return;
-        a = old;
-        b = lo;
-    }
-}
-
-__global__ void __launch_bounds__(MB) parent_init_kernel(int32_t* __restrict__ parent, int64_t m) {
-    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (v < m) parent[v] = (int32_t)v;
-}
-
 __global__ void __launch_bounds__(MB) union_kernel(const int32_t* __restrict__ faces, int64_t t, int32_t* parent) {
     const int64_t f = (int64_t)blockIdx.x * MB + threadIdx.x;
     if (f >= t) return;
     const int a = faces[3 * f], b = faces[3 * f + 1], c = faces[3 * f + 2];
     unite(parent, a, b);
     unite(parent, a, c);
-}
-
-// after every union: parent[v] = the root of v (its label)
-__global__ void __launch_bounds__(MB) compress_kernel(int32_t* parent, int64_t m) {
-    const int64_t v = (int64_t)blockIdx.x * MB + threadIdx.x;
-    if (v >= m) return;
-    const int r = find_root(parent, (int)v);
-    atomicMin(&parent[v], r);
 }
 
 __global__ void __launch_bounds__(MB) size_kernel(const int32_t* __restrict__ faces, int64_t t,

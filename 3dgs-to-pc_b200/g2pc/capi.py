@@ -113,6 +113,14 @@ SIGNATURES = {
                                      _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_mesh_components_compact": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p,
                                       _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_holes_workspace_bytes": ([_i64, _i64], ctypes.c_int64),
+    "g2pc_mesh_holes_find": ([_c_void_p, _i64, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64,
+                              _c_void_p], ctypes.c_int),
+    "g2pc_mesh_holes_plan": ([_i64, _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
+                              _i64, _c_void_p], ctypes.c_int),
+    "g2pc_mesh_holes_fill": ([_c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
+                              _i64, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p],
+                             ctypes.c_int),
     "g2pc_tsdf_frame_workspace_bytes": ([_i64], ctypes.c_int64),
     "g2pc_tsdf_frame": ([_c_void_p, _i64, _i32, _c_void_p, _c_void_p, _i64, _c_void_p], ctypes.c_int),
     "g2pc_tsdf_integrate": ([_c_void_p, _i32, ctypes.c_double, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _i32, _i32,
@@ -240,7 +248,8 @@ _OWN_KERNELS = {"g2pc_multisplit": 6, "g2pc_multisplit_grid": 6, "g2pc_depth_sor
                 "g2pc_mesh_band_iso": 4, "g2pc_mesh_band_extract_count": 2, "g2pc_mesh_band_extract_emit": 2,
                 "g2pc_mesh_band_gather": 2, "g2pc_mesh_decimate_prepare": 4, "g2pc_mesh_decimate_select": 8,
                 "g2pc_mesh_decimate_apply": 5, "g2pc_mesh_decimate_finish": 4, "g2pc_mesh_components_label": 5,
-                "g2pc_mesh_components_select": 4, "g2pc_mesh_components_compact": 2,"g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
+                "g2pc_mesh_components_select": 4, "g2pc_mesh_components_compact": 2,"g2pc_mesh_holes_find": 7,
+                "g2pc_mesh_holes_plan": 2, "g2pc_mesh_holes_fill": 1, "g2pc_orient_prepare": 2, "g2pc_orient_edges": 2,
                 "g2pc_orient_round": 5, "g2pc_orient_finish": 3, "g2pc_tsdf_frame": 2, "g2pc_tsdf_gather_compact": 4}
 # host-only entry points, besides every *_workspace_bytes size query
 _NOT_KERNELS = {"g2pc_version", "g2pc_last_error", "g2pc_sample_emit_chunk_points", "g2pc_multisplit_chunk",

@@ -18,6 +18,9 @@ then per round _select (host reads the counts) -> _apply until the target is met
 With min_component_triangles / keep_largest_components (N11, s15_components.cu): between the trim and the smoothing,
 remove_components(): g2pc_mesh_components_label (host reads the component count) -> _select (host reads the kept counts)
 -> _compact.
+
+With max_hole_edges (N12, s16_holes.cu): after the component filter and before the smoothing, fill_holes():
+g2pc_mesh_holes_find (host reads the boundary counts) -> _plan (host reads the added counts) -> _fill.
 """
 import collections
 import math
@@ -45,6 +48,7 @@ FRAME_WORDS = 8
 MAX_CYCLES = 40
 TOLERANCE = 1e-5
 NB_NEIGHBORS = 20
+MAX_HOLE_EDGES = 1024  # the longest hole fill_holes() closes: bounds each loop's walk and a centre's valence
 
 Mesh = collections.namedtuple("Mesh", ["vertices", "faces", "colours", "normals", "densities"])
 
@@ -550,9 +554,153 @@ def filter_components(vpos, faces, vcol, dens, min_triangles, keep_largest, stat
     return out
 
 
+def check_max_hole_edges(max_hole_edges):
+    """Refuses a hole length that is not an integer in 3..MAX_HOLE_EDGES (bool included)."""
+    x = max_hole_edges
+    if isinstance(x, bool) or not isinstance(x, (int, np.integer)) or not 3 <= x <= MAX_HOLE_EDGES:
+        raise capi.G2pcError(f"max_hole_edges must be an integer in 3..{MAX_HOLE_EDGES}, got {x!r}")
+
+
+def fill_holes(vpos, faces, colours=None, densities=None, max_hole_edges=64, stats=None, return_debug=False):
+    """Closes the holes of a triangle mesh whose boundary loop has at most max_hole_edges edges (DESIGN.md §2, N12).  A
+    half-edge is on the boundary when its undirected edge is used by exactly one face; a boundary set (vertices joined
+    by boundary half-edges, labelled by its smallest vertex) is a hole when each of its vertices has exactly one
+    outgoing and one incoming boundary half-edge, else it is pinched and stays open.  A hole of 3 edges gets one face
+    (unless its three half-edges belong to one face: a lone triangle), a longer one a fan around a new centre vertex
+    (the mean position, colour and density of its loop).  Every new face runs the opposite way to its boundary edge.
+
+    vpos (m,3) float64, faces (t,3) int32 (no face uses a vertex twice), colours (m,3) uint8 or None, densities (m,)
+    float64 or None, all CUDA; max_hole_edges an integer in 3..1024.  Returns (vpos, faces, colours, densities): the
+    input vertices and faces unchanged and in their order, then the centres and the new faces in ascending label order.
+    When nothing is filled, the input tensors themselves.
+
+    stats: a dict that receives boundary_edges, holes, filled, too_long, lone_triangles, pinched, added_vertices and
+    added_triangles.  return_debug: also a dict with labels (m,) int32 (-1 off the boundary), succ (m,) int32 (the
+    target of a vertex's only outgoing boundary half-edge, else -1), lengths (m,) int32 (vertices per label, 0 at an
+    index that is no label) and filled (m,) uint8 (per label)."""
+    check_max_hole_edges(max_hole_edges)
+    for name, x in (("vpos", vpos), ("faces", faces), ("colours", colours), ("densities", densities)):
+        if x is not None and not (torch.is_tensor(x) and x.is_cuda):
+            raise capi.G2pcError(f"{name} must be a CUDA tensor (the hole filling has no CPU path)")
+    if vpos.dim() != 2 or vpos.shape[1] != 3 or vpos.dtype != torch.float64:
+        raise capi.G2pcError(f"vpos must be (m, 3) float64, got {tuple(vpos.shape)} {vpos.dtype}")
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype != torch.int32:
+        raise capi.G2pcError(f"faces must be (t, 3) int32, got {tuple(faces.shape)} {faces.dtype}")
+    m, t, dev = vpos.shape[0], faces.shape[0], vpos.device
+    if colours is not None and (colours.shape != (m, 3) or colours.dtype != torch.uint8):
+        raise capi.G2pcError(f"colours must be (m, 3) uint8, got {tuple(colours.shape)} {colours.dtype}")
+    if densities is not None and (densities.shape != (m,) or densities.dtype != torch.float64):
+        raise capi.G2pcError(f"densities must be (m,) float64, got {tuple(densities.shape)} {densities.dtype}")
+    if any(x is not None and x.device != dev for x in (faces, colours, densities)):
+        raise capi.G2pcError("vpos, faces, colours and densities must be on one device")
+    if m >= 2 ** 31 - 1 or 3 * t >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the mesh has {m} vertices and {t} triangles: more than the hole filling's int32 lists "
+                             f"(3 half-edges per triangle) can hold")
+    if t:
+        f = faces.long()
+        lo, hi, rep = torch.stack([f.min(), f.max(), ((f[:, 0] == f[:, 1]) | (f[:, 1] == f[:, 2]) |
+                                                       (f[:, 0] == f[:, 2])).sum()]).tolist()
+        del f
+        if lo < 0 or hi >= m:
+            raise capi.G2pcError(f"face indices must be in 0..{m - 1}, got {lo}..{hi}")
+        if rep:
+            raise capi.G2pcError(f"{rep} face(s) use a vertex twice")
+    st_keys = ("boundary_edges", "holes", "filled", "too_long", "lone_triangles", "pinched", "added_vertices",
+               "added_triangles")
+    if t == 0:  # no edge, no boundary
+        if stats is not None:
+            stats.update(dict.fromkeys(st_keys, 0))
+        out = (vpos, faces, colours, densities)
+        if return_debug:
+            return out, {"labels": torch.full((m,), -1, dtype=torch.int32, device=dev),
+                         "succ": torch.full((m,), -1, dtype=torch.int32, device=dev),
+                         "lengths": torch.zeros((m,), dtype=torch.int32, device=dev),
+                         "filled": torch.zeros((m,), dtype=torch.uint8, device=dev)}
+        return out
+    fcont = faces.contiguous()
+    lib = capi.load()
+    ws_bytes = lib.g2pc_mesh_holes_workspace_bytes(m, t)
+    # labels, succ, lengths, filled and the workspace (sorted edge keys, per-vertex degrees, flags and ranks)
+    check_memory(m * (4 + 4 + 4 + 1) + ws_bytes, dev, f"the hole search of {m} vertices and {t} triangles",
+                 remedy="fill the holes of a smaller mesh")
+    st = capi.stream_ptr(dev)
+    labels = torch.empty((m,), dtype=torch.int32, device=dev)
+    succ = torch.empty((m,), dtype=torch.int32, device=dev)
+    lengths = torch.empty((m,), dtype=torch.int32, device=dev)
+    filled = torch.empty((m,), dtype=torch.uint8, device=dev)
+    counts = torch.empty((5,), dtype=torch.int64, device=dev)
+    ws = capi.workspace(ws_bytes, dev)
+    capi.call("g2pc_mesh_holes_find", capi.ptr(fcont), m, t, capi.ptr(labels), capi.ptr(succ), capi.ptr(lengths),
+              capi.ptr(counts), capi.ptr(ws), ws.numel(), st)
+    boundary, holes, pinched = counts[:3].tolist()
+    capi.call("g2pc_mesh_holes_plan", m, t, capi.ptr(labels), capi.ptr(succ), capi.ptr(lengths), int(max_hole_edges),
+              capi.ptr(filled), capi.ptr(counts), capi.ptr(ws), ws.numel(), st)
+    av, af, nfilled, too_long, lone = counts.tolist()
+    if stats is not None:
+        stats.update(boundary_edges=boundary, holes=holes, filled=nfilled, too_long=too_long, lone_triangles=lone,
+                     pinched=pinched, added_vertices=av, added_triangles=af)
+    debug = {"labels": labels, "succ": succ, "lengths": lengths, "filled": filled}
+    if nfilled == 0:
+        out = (vpos, faces, colours, densities)
+        return (out, debug) if return_debug else out
+    M, T = m + av, t + af
+    if M >= 2 ** 31 - 1 or 3 * T >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the filled mesh would have {M} vertices and {T} triangles: more than int32 lists "
+                             f"(3 entries per triangle) can hold")
+    check_memory(M * (24 + (3 if colours is not None else 0) + (8 if densities is not None else 0)) + 12 * T, dev,
+                 f"the filled mesh of {M} vertices and {T} triangles", remedy="fill the holes of a smaller mesh")
+    vcont = vpos.contiguous()
+    ccont = colours.contiguous() if colours is not None else None
+    dcont = densities.contiguous() if densities is not None else None
+    vout = torch.empty((M, 3), dtype=torch.float64, device=dev)
+    cout = torch.empty((M, 3), dtype=torch.uint8, device=dev) if colours is not None else None
+    dout = torch.empty((M,), dtype=torch.float64, device=dev) if densities is not None else None
+    fout = torch.empty((T, 3), dtype=torch.int32, device=dev)
+    capi.call("g2pc_mesh_holes_fill", capi.ptr(vcont), capi.ptr(ccont), capi.ptr(dcont), m, capi.ptr(fcont), t,
+              capi.ptr(succ), capi.ptr(lengths), capi.ptr(filled), av, af, capi.ptr(vout), capi.ptr(cout),
+              capi.ptr(dout), capi.ptr(fout), capi.ptr(ws), ws.numel(), st)
+    out = (vout, fout, cout, dout)
+    return (out, debug) if return_debug else out
+
+
+def fill_holes_mesh(mesh, max_hole_edges, stats=None):
+    """fill_holes() of a Mesh, its float32 positions taken as float64.  Vertices on no filled loop keep their stored
+    normals bit for bit; the vertices of the filled loops and the centres get vertex_normals() of the filled mesh
+    (area-weighted).  A mesh with nothing to fill is returned as it is."""
+    check_max_hole_edges(max_hole_edges)
+    vpos = mesh.vertices.to(torch.float64)
+    (p, faces, vcol, dens), dbg = fill_holes(vpos, mesh.faces, mesh.colours, mesh.densities, max_hole_edges,
+                                             stats=stats, return_debug=True)
+    if p is vpos:
+        return mesh
+    m = vpos.shape[0]
+    labels = dbg["labels"].long()
+    on_loop = (labels >= 0) & (dbg["filled"][labels.clamp(min=0)] != 0)
+    v, vn = vertex_normals(p, faces)
+    normals = torch.cat([torch.where(on_loop[:, None], vn[:m], mesh.normals.to(torch.float32)), vn[m:]])
+    return Mesh(v, faces, vcol, normals, dens)
+
+
+def close_holes(vpos, faces, vcol, dens, max_hole_edges, stats, timings, debug, smoothing):
+    """fill_holes() of a mesher's mesh before the smoothing when max_hole_edges is given, else the mesh as it is.
+    debug (a dict or None) receives hole_labels.  smoothing: the mesh goes on to g2pc_mesh_smooth, whose one-ring lists
+    hold 6 entries per triangle in int32."""
+    if max_hole_edges is None:
+        return vpos, faces, vcol, dens
+    with capi.phase(timings, "holes"):
+        out, hdbg = fill_holes(vpos, faces, vcol, dens, max_hole_edges, stats=stats, return_debug=True)
+    if debug is not None:
+        debug["hole_labels"] = hdbg["labels"]
+    t = out[1].shape[0]
+    if smoothing and 6 * t >= 2 ** 31 - 1:
+        raise capi.G2pcError(f"the filled surface has {t} triangles: the Laplacian smoothing's one-ring lists (6 per "
+                             f"triangle) exceed int32; use a smaller depth or laplacian_iters=0")
+    return out
+
+
 def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, std_ratio=3.0, return_debug=False,
                  timings=None, band_depth=None, band_stats=None, target_triangles=None, min_component_triangles=None,
-                 keep_largest_components=None, component_stats=None):
+                 keep_largest_components=None, component_stats=None, max_hole_edges=None, hole_stats=None):
     """Mesh of an oriented point cloud.  points (n,3) float32 CUDA; normals (n,3) float32 / float64 (outward for an
     outward-facing mesh); colours (n,3) in 0..255 or None.  Returns Mesh(vertices (m,3) float32, faces (t,3) int32,
     colours (m,3) uint8 or None, normals (m,3) float32, densities (m,) float64).  With return_debug also a dict: chi
@@ -574,11 +722,17 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
 
     min_component_triangles, keep_largest_components: None and None keep every component.  Otherwise the trimmed mesh
     goes through remove_components() (DESIGN.md §2, N11) before the smoothing; timings add "components", the debug dict
-    component_labels (per vertex of the trimmed mesh) and component_stats (a dict) receives remove_components' stats."""
+    component_labels (per vertex of the trimmed mesh) and component_stats (a dict) receives remove_components' stats.
+
+    max_hole_edges: None leaves the holes open.  An integer in 3..1024 closes the holes of at most that many edges with
+    fill_holes() (DESIGN.md §2, N12) after the component filter and before the smoothing; timings add "holes", the debug
+    dict hole_labels (per vertex of the mesh before the fill) and hole_stats (a dict) receives fill_holes' stats."""
     capi.check_cloud(points, normals, colours, what="Poisson meshing")
     if target_triangles is not None:
         check_target(target_triangles)
     check_component_params(min_component_triangles, keep_largest_components, need_one=False)
+    if max_hole_edges is not None:
+        check_max_hole_edges(max_hole_edges)
     if int(depth) != depth or not DEPTH_MIN <= depth <= DEPTH_MAX:
         raise capi.G2pcError(f"depth must be an integer in {DEPTH_MIN}..{DEPTH_MAX} (the dense int64 right-hand side "
                              f"alone is 69 GB at depth 11), got {depth}")
@@ -621,7 +775,8 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
         del chi
         return _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, int(band_depth), laplacian_iters, debug,
                           return_debug, timings, band_stats, target_triangles,
-                          (min_component_triangles, keep_largest_components, component_stats))
+                          (min_component_triangles, keep_largest_components, component_stats),
+                          (max_hole_edges, hole_stats))
     with capi.phase(timings, "extract"):
         # B is dead after the solve: its memory holds the node lists of the extraction and the cell lists of the gather
         vkey, vt, vpos, faces = extract(chi, depth, frame, iso, B)
@@ -633,6 +788,8 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
     vpos, faces, vcol, dens = filter_components(vpos, faces, vcol, dens, min_component_triangles,
                                                  keep_largest_components, component_stats, timings,
                                                  debug if return_debug else None)
+    vpos, faces, vcol, dens = close_holes(vpos, faces, vcol, dens, max_hole_edges, hole_stats, timings,
+                                          debug if return_debug else None, smoothing=laplacian_iters > 0)
     with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
     smoothed = vpos
@@ -649,10 +806,10 @@ def poisson_mesh(points, normals, colours=None, depth=10, laplacian_iters=10, st
 
 
 def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, laplacian_iters, debug, return_debug,
-               timings, band_stats, target_triangles, components):
+               timings, band_stats, target_triangles, components, holes):
     """The band levels depth + 1 .. band_depth after the dense solve, then the mesh at band_depth.  dense: {"chi": the
     dense level's chi}, emptied here.  components: poisson_mesh's (min_component_triangles, keep_largest_components,
-    component_stats)."""
+    component_stats); holes: its (max_hole_edges, hole_stats)."""
     dev = pts.device
     parent_chi, parent_map = dense.pop("chi"), None
     if return_debug:
@@ -706,6 +863,8 @@ def _band_mesh(pts, nrm, cols, cell, frame, dense, iso, depth, band_depth, lapla
         dens, vpos, vcol, faces, keep, thr = trim(dens, vpos, vcol, faces)
     vpos, faces, vcol, dens = filter_components(vpos, faces, vcol, dens, *components, timings,
                                                  debug if return_debug else None)
+    vpos, faces, vcol, dens = close_holes(vpos, faces, vcol, dens, *holes, timings, debug if return_debug else None,
+                                          smoothing=laplacian_iters > 0)
     with capi.phase(timings, "smooth"):
         smooth(vpos, faces, laplacian_iters)
     smoothed = vpos

@@ -6,7 +6,7 @@ Steps: statistical outlier removal of the Gaussian means (k = 20, std_ratio 3; o
 transmittance T, median depth z_med) then g2pc_tsdf_integrate into the 2^depth grid -> g2pc_mesh_extract_count / _emit
 (the Poisson mesher's marching tetrahedra, unchanged, iso 0) -> g2pc_tsdf_gather_compact (keep the surface of the
 observed voxels, vertex colours and weights) -> remove_components (with min_component_triangles or
-keep_largest_components) -> g2pc_mesh_smooth -> decimate (with target_triangles) ->
+keep_largest_components) -> fill_holes (with max_hole_edges) -> g2pc_mesh_smooth -> decimate (with target_triangles) ->
 g2pc_mesh_normals.  Host reads: the frame after the outlier removal, the extraction counts, the kept counts.
 """
 import collections
@@ -117,7 +117,8 @@ def gather_compact(weight, colour, depth, vkey, vt, vpos, faces):
 
 def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, depth=DEFAULT_DEPTH, trunc=DEFAULT_TRUNC,
               laplacian_iters=10, target_triangles=None, timings=None, return_debug=False, async_mode=True,
-              min_component_triangles=None, keep_largest_components=None, component_stats=None):
+              min_component_triangles=None, keep_largest_components=None, component_stats=None, max_hole_edges=None,
+              hole_stats=None):
     """Mesh of the Gaussians (xyz (n,3), opacities (n,) or (n,1), covariances (n,3,3) or (n,6), and exactly one of
     colours (n,3) in 0..1 or shs (n,3,K) channel-major, all CUDA) seen by `cameras` (the CUDA back-end's raster settings,
     camera_handler.get_camera("cuda", ...)), in order.  Returns mesh.Mesh(vertices (m,3) float32, faces (t,3) int32,
@@ -136,7 +137,10 @@ def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, dept
     replays.
 
     min_component_triangles, keep_largest_components, component_stats: as mesh.poisson_mesh; the component filter runs
-    on the gathered mesh before the smoothing, timings add "components" and the debug dict component_labels."""
+    on the gathered mesh before the smoothing, timings add "components" and the debug dict component_labels.
+
+    max_hole_edges, hole_stats: as mesh.poisson_mesh; the hole filling runs after the component filter and before the
+    smoothing, timings add "holes" and the debug dict hole_labels."""
     check_depth(depth)
     check_trunc(trunc)
     if int(laplacian_iters) != laplacian_iters or laplacian_iters < 0:
@@ -144,6 +148,8 @@ def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, dept
     if target_triangles is not None:
         mesh.check_target(target_triangles)
     mesh.check_component_params(min_component_triangles, keep_largest_components, need_one=False)
+    if max_hole_edges is not None:
+        mesh.check_max_hole_edges(max_hole_edges)
     if (colours is None) == (shs is None):
         raise capi.G2pcError("give exactly one of colours and shs")
     capi.check_cloud(xyz.to(torch.float32).contiguous() if torch.is_tensor(xyz) else xyz)
@@ -207,6 +213,8 @@ def fuse_mesh(xyz, opacities, covariances, cameras, colours=None, shs=None, dept
         raise capi.G2pcError("no surface between observed voxels")
     vkept, fkept, vcol, dens = mesh.filter_components(vkept, fkept, vcol, dens, min_component_triangles,
                                                        keep_largest_components, component_stats, timings, debug)
+    vkept, fkept, vcol, dens = mesh.close_holes(vkept, fkept, vcol, dens, max_hole_edges, hole_stats, timings, debug,
+                                                smoothing=False)  # the one-ring check follows
     if laplacian_iters and 6 * fkept.shape[0] >= 2 ** 31 - 1:
         raise capi.G2pcError(f"the surface has {fkept.shape[0]} triangles: the Laplacian smoothing's one-ring lists "
                              f"(6 per triangle) exceed int32; use a smaller tsdf depth or laplacian_iters=0")

@@ -3,7 +3,7 @@
     python gauss_to_mesh.py --input_path scene.ply --transform_path transforms.json [gauss_to_pc.py's flags]
                             [--mesh_output_path 3dgs_mesh.ply] [--poisson_depth 10] [--laplacian_iterations 10]
                             [--band_depth D] [--target_triangles N]
-                            [--min_component_triangles N] [--keep_largest_components K]
+                            [--min_component_triangles N] [--keep_largest_components K] [--max_hole_edges H]
                             [--mesh_method {poisson,tsdf}] [--tsdf_depth 9] [--tsdf_trunc 4]
 
 Same flags and validation as gauss_to_pc.py; it writes the same point cloud to --output_path.  Then, as the reference's
@@ -14,7 +14,9 @@ best (g2pc.orient.face_cameras), and that cloud is meshed by g2pc/mesh.py (outli
 to --mesh_output_path.  Needs --renderer_type cuda and a depth in
 2..10 (DESIGN.md §2).  With --min_component_triangles N and --keep_largest_components K, the connected pieces of the
 trimmed mesh with fewer than N triangles, and all but the K largest, are removed before the smoothing
-(g2pc.mesh.remove_components, DESIGN.md §2, N11); both methods take them.
+(g2pc.mesh.remove_components, DESIGN.md §2, N11); both methods take them.  With --max_hole_edges H the holes
+whose boundary loop has at most H edges (3..1024) are then closed, also before the smoothing (g2pc.mesh.fill_holes,
+DESIGN.md §2, N12); both methods take it.
 
 With --mesh_method tsdf no surface cloud is sampled: the Gaussians the point cloud is sampled from are rendered again
 from the same cameras with a median depth per pixel, every depth map is fused in order into a 2^tsdf_depth voxel grid

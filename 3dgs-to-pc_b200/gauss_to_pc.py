@@ -456,8 +456,9 @@ def config_parser(argv=None, mesh=False):
     (g2pc/mesh.py) instead of Open3D, which needs renderer_type cuda, a depth in mesh.DEPTH_MIN..DEPTH_MAX and
     laplacian_iterations >= 0.  It also adds --band_depth (narrow-band levels above --poisson_depth, up to
     mesh.BAND_DEPTH_MAX; --poisson_depth 10 --band_depth 12 is the reference's depth 12), --target_triangles (>= 1:
-    decimate the mesh to that many triangles), and --min_component_triangles / --keep_largest_components (>= 1: remove
-    the mesh's connected pieces with fewer triangles / all but the largest ones)."""
+    decimate the mesh to that many triangles), --min_component_triangles / --keep_largest_components (>= 1: remove
+    the mesh's connected pieces with fewer triangles / all but the largest ones), and --max_hole_edges (3..1024: close
+    the mesh's holes whose boundary loop has at most that many edges)."""
     try:
         import configargparse as ap
     except ImportError:
@@ -513,6 +514,9 @@ def config_parser(argv=None, mesh=False):
         parser.add_argument("--keep_largest_components", default=None, type=int,
                             help="Keep only this many of the largest connected pieces of the mesh; default: keep them "
                                  "all")
+        parser.add_argument("--max_hole_edges", default=None, type=int,
+                            help="Close the holes of the mesh whose boundary loop has at most this many edges (3..1024), "
+                                 "before smoothing; default: leave them open")
 
     args = parser.parse_args(argv)
     if mesh:
@@ -533,6 +537,8 @@ def config_parser(argv=None, mesh=False):
             raise AttributeError("Minimum component triangles must be 1 or more")
         if args.keep_largest_components is not None and args.keep_largest_components < 1:
             raise AttributeError("Largest components to keep must be 1 or more")
+        if args.max_hole_edges is not None and not 3 <= args.max_hole_edges <= gmesh.MAX_HOLE_EDGES:
+            raise AttributeError(f"Maximum hole edges must be between 3 and {gmesh.MAX_HOLE_EDGES}")
         if args.mesh_method == "tsdf":
             from g2pc import tsdf
             if args.band_depth is not None:
@@ -647,8 +653,8 @@ def main(argv=None, mesh=False):
                     normals_points=total_point_cloud.normals, chunk_size=10**6, quiet=args.quiet)
 
     if mesh:
-        from mesh_pc import component_line
-        cstats = {}
+        from mesh_pc import component_line, hole_line
+        cstats, hstats = {}, {}
     if mesh and args.mesh_method == "tsdf":
         from g2pc import mesh as gmesh, tsdf
         scene = surface_point_cloud
@@ -658,11 +664,14 @@ def main(argv=None, mesh=False):
                            shs=scene.shs, depth=args.tsdf_depth, trunc=args.tsdf_trunc,
                            laplacian_iters=args.laplacian_iterations, target_triangles=args.target_triangles,
                            min_component_triangles=args.min_component_triangles,
-                           keep_largest_components=args.keep_largest_components, component_stats=cstats)
+                           keep_largest_components=args.keep_largest_components, component_stats=cstats,
+                           max_hole_edges=args.max_hole_edges, hole_stats=hstats)
         gmesh.write_mesh_ply(args.mesh_output_path, m)
         if not args.quiet:
             if cstats:
                 print(component_line(cstats))
+            if hstats:
+                print(hole_line(hstats))
             print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")
         return None, m
     if mesh:
@@ -677,11 +686,14 @@ def main(argv=None, mesh=False):
                                depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations, std_ratio=3.0,
                                band_depth=args.band_depth, target_triangles=args.target_triangles,
                                min_component_triangles=args.min_component_triangles,
-                               keep_largest_components=args.keep_largest_components, component_stats=cstats)
+                               keep_largest_components=args.keep_largest_components, component_stats=cstats,
+                               max_hole_edges=args.max_hole_edges, hole_stats=hstats)
         gmesh.write_mesh_ply(args.mesh_output_path, m)
         if not args.quiet:
             if cstats:
                 print(component_line(cstats))
+            if hstats:
+                print(hole_line(hstats))
             print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path}")
         return surface_point_cloud, m
     elif pointcloud_settings.generate_mesh:

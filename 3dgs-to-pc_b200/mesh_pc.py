@@ -3,7 +3,7 @@ trim and Laplacian smoothing (g2pc/mesh.py).
 
     python mesh_pc.py --input_path cloud.ply [--mesh_output_path mesh.ply] [--poisson_depth 10] [--band_depth 12]
                       [--laplacian_iterations 10] [--orient_normals] [--target_triangles N]
-                      [--min_component_triangles N] [--keep_largest_components K] [--quiet]
+                      [--min_component_triangles N] [--keep_largest_components K] [--max_hole_edges H] [--quiet]
 
 The cloud must carry normals (nx ny nz), as gauss_to_pc.py writes them by default; its colours (red green blue) are
 carried over to the mesh's vertices.  A mesh faces the way its normals point.  By default the normals are used as they
@@ -12,7 +12,9 @@ from Gaussians lack: each takes its sign from its Gaussian's rotation.  --band_d
 --poisson_depth 10 --band_depth 12 is the reference's Poisson depth 12.  --target_triangles decimates the smoothed mesh
 to N or N - 1 triangles on the GPU (quadric edge collapse, g2pc.mesh.decimate) before its normals are computed.
 --min_component_triangles and --keep_largest_components remove the small disconnected pieces of the trimmed mesh before
-it is smoothed (g2pc.mesh.remove_components): those with fewer than N triangles, and all but the K largest."""
+it is smoothed (g2pc.mesh.remove_components): those with fewer than N triangles, and all but the K largest.
+--max_hole_edges then closes the holes whose boundary loop has at most H edges (3..1024), also before the smoothing
+(g2pc.mesh.fill_holes)."""
 import argparse
 import time
 
@@ -51,6 +53,25 @@ def add_component_flags(p):
                    help="keep only this many of the largest connected pieces; default: keep them all")
 
 
+def hole_edges(s):
+    n = int(s)
+    if not 3 <= n <= mesh.MAX_HOLE_EDGES:
+        raise argparse.ArgumentTypeError(f"must be in 3..{mesh.MAX_HOLE_EDGES}")
+    return n
+
+
+def add_hole_flag(p):
+    p.add_argument("--max_hole_edges", type=hole_edges, default=None,
+                   help=f"close the holes of the mesh whose boundary loop has at most this many edges "
+                        f"(3..{mesh.MAX_HOLE_EDGES}); default: leave them open")
+
+
+def hole_line(stats):
+    """The one line the commands print about the hole filling."""
+    return (f"Closed holes: {stats['holes']} hole(s) found, {stats['filled']} filled, {stats['too_long']} too long, "
+            f"{stats['pinched']} pinched, {stats['added_triangles']} triangle(s) added")
+
+
 def component_line(stats):
     """The one line the commands print about the component filter."""
     return (f"Removed small pieces: {stats['components']} component(s) found, {stats['kept']} kept, "
@@ -73,6 +94,7 @@ def config_parser(argv=None):
     p.add_argument("--target_triangles", type=target, default=None,
                    help="decimate the mesh to this many triangles (or one fewer); default: keep every triangle")
     add_component_flags(p)
+    add_hole_flag(p)
     p.add_argument("--quiet", action="store_true", help="print nothing")
     args = p.parse_args(argv)
     if args.band_depth is not None and not args.poisson_depth < args.band_depth <= mesh.BAND_DEPTH_MAX:
@@ -103,15 +125,18 @@ def main(argv=None):
         normals, st = orient.orient_normals(points, normals, k=orient.K_DEFAULT)
         if not args.quiet:
             print(f"Oriented the normals: {st.flipped} flipped, {st.components} component(s), {st.skipped} skipped")
-    cstats = {}
+    cstats, hstats = {}, {}
     m = mesh.poisson_mesh(points, normals, colours, depth=args.poisson_depth, laplacian_iters=args.laplacian_iterations,
                           band_depth=args.band_depth, target_triangles=args.target_triangles,
                           min_component_triangles=args.min_component_triangles,
-                          keep_largest_components=args.keep_largest_components, component_stats=cstats)
+                          keep_largest_components=args.keep_largest_components, component_stats=cstats,
+                          max_hole_edges=args.max_hole_edges, hole_stats=hstats)
     mesh.write_mesh_ply(args.mesh_output_path, m)
     if not args.quiet:
         if cstats:
             print(component_line(cstats))
+        if hstats:
+            print(hole_line(hstats))
         print(f"Wrote {m.vertices.shape[0]} vertices and {m.faces.shape[0]} triangles to {args.mesh_output_path} "
               f"in {time.perf_counter() - t0:.2f} s")
     return m

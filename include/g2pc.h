@@ -391,6 +391,31 @@ int g2pc_mesh_components_compact(const double* vpos, const uint8_t* vcolours, co
                                  uint8_t* vcolours_out, double* density_out, int32_t* faces_out, const void* workspace,
                                  int64_t workspace_bytes, void* stream);
 
+/* ---- N12: closing small holes of a triangle mesh (s16_holes.cu, g2pc/mesh.py fill_holes) ------------------------- */
+/* Rules in DESIGN.md §2, N12.  m vertices (1..2^31-2), faces (t,3 int32, 1 <= t, 3 t < 2^31 - 1, indices in 0..m-1, no
+ * face uses a vertex twice).  Order of calls, all with one workspace (g2pc_mesh_holes_workspace_bytes(m, t)) and the
+ * same m, t: find (host reads counts) -> plan (host reads counts) -> fill into buffers of m + added vertices and
+ * t + added faces. */
+int64_t g2pc_mesh_holes_workspace_bytes(int64_t m, int64_t t);
+/* A half-edge is on the boundary when its undirected edge is used by exactly one face.  labels (m int32) = the smallest
+ * vertex of each vertex's boundary set, -1 off the boundary; succ (m int32) = the target of the vertex's boundary
+ * half-edge where it has exactly one, else -1; lengths (m int32, indexed by label) = vertices per set, 0 at an index
+ * that is no label.  counts (3 int64): boundary half-edges, holes, pinched sets. */
+int g2pc_mesh_holes_find(const int32_t* faces, int64_t m, int64_t t, int32_t* labels, int32_t* succ, int32_t* lengths,
+                         int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream);
+/* filled (m uint8, indexed by label) = 1 iff the set is a hole of length <= max_hole_edges (3..1024) that is not a lone
+ * triangle.  counts (5 int64): added vertices, added faces, filled, too long, lone triangles. */
+int g2pc_mesh_holes_plan(int64_t m, int64_t t, const int32_t* labels, const int32_t* succ, const int32_t* lengths,
+                         int64_t max_hole_edges, uint8_t* filled, int64_t* counts, void* workspace,
+                         int64_t workspace_bytes, void* stream);
+/* The input mesh (vcolours and density may be NULL, each with its output) copied into the *_out buffers, then the
+ * centres from index m and the added faces from index t, in ascending label order.  added_* are plan's counts. */
+int g2pc_mesh_holes_fill(const double* vpos, const uint8_t* vcolours, const double* density, int64_t m,
+                         const int32_t* faces, int64_t t, const int32_t* succ, const int32_t* lengths,
+                         const uint8_t* filled, int64_t added_vertices, int64_t added_faces, double* vpos_out,
+                         uint8_t* vcolours_out, double* density_out, int32_t* faces_out, const void* workspace,
+                         int64_t workspace_bytes, void* stream);
+
 /* ---- N7: consistent orientation of point-cloud normals (s11_orient.cu, g2pc/orient.py) -------------------------- */
 /* Hoppe et al. 1992 (the rule behind Open3D's orient_normals_consistent_tangent_plane) with this project's own rules
  * (DESIGN.md §2): k-NN graph, edge weight 1 - |n_i . n_j|, minimum spanning forest, sign propagated from one seed per
